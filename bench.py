@@ -18,9 +18,9 @@ suggest_e2e (N=1): wall-clock of a whole `VizierGPBandit.suggest(1)` (trial conv
            M=100k random-pool optimiser (the metric's configuration) and with the default Eagle optimiser,
            next to the same pipeline restated on the CPU (NumPy/SciPy oracle, all host cores).
 roofline : the scoring kernel is FP64-pipe bound (N^2 flops per candidate against 8(D+1) bytes), so
-           `achieved` is algorithmic TFLOP/s against the FP64 DMMA peak measured on this pool's B200 by
-           tools/fp64_peak.cu (profiles/fp64_peak_r01.json; MEASURED_PEAKS.json has no fp64 entry); the
-           HBM view is reported beside it.
+           `achieved` is algorithmic TFLOP/s against the H100 SXM data-sheet FP64 tensor-core peak; the HBM view
+           is reported beside it.
+--dump-outputs DIR: the last timed step's pool scores and winner as DIR/<name>.npy (float64, seeded inputs).
 cpu_baseline / --impl reference: the NumPy/SciPy oracle (a port: the reference's JAX/TFP stack cannot be
            installed here, SURVEY 8c) on all host cores, on a bounded candidate sample.
 """
@@ -65,20 +65,12 @@ def algorithmic_bytes_per_candidate(d):
 
 
 def fp64_peak_tflops():
-  p = os.path.join(ROOT, 'profiles', 'fp64_peak_r01.json')
-  if os.path.exists(p):
-    try:
-      j = json.load(open(p))
-      return float(max(j['dfma_tflops'], j['dmma_m8n8k4_tflops'])), 'measured (tools/fp64_peak.cu, profiles/fp64_peak_r01.json)'
-    except Exception:  # pylint: disable=broad-except
-      pass
-  return 37.0, 'nominal B200 FP64 (no measurement found)'
+  return 67.0, 'H100 SXM data sheet, FP64 tensor core at 700 W (not measured)'
 
 
 def int8_peak_tops():
-  """Dense int8 tensor roof.  tcgen05 kind::i8 runs at the fp8 rate = 2 x bf16 (tools/umma_rate.cu: identical cycles per
-  MMA for i8 and f8f6f4 at equal bytes); MEASURED_PEAKS.json carries the measured bf16 figure - the sustained one, the
-  kernel is timed inside a long step."""
+  """Dense int8 tensor roof (wgmma s8 runs at the fp8 rate = 2 x bf16); MEASURED_PEAKS.json, where present, carries
+  a measured bf16 figure - the sustained one, the kernel is timed inside a long step."""
   p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
   if os.path.exists(p):
     try:
@@ -86,7 +78,7 @@ def int8_peak_tops():
       return 2.0 * float(j.get('bf16_tflops_sustained', j['bf16_tflops'])), '2 x measured sustained dense bf16 (MEASURED_PEAKS.json)'
     except Exception:  # pylint: disable=broad-except
       pass
-  return 2.0 * 1590.0, '2 x the fallback dense bf16 figure of B200_PROFILING.md (1.59 PFLOP/s)'
+  return 1979.0, 'H100 SXM data sheet, dense INT8 at 700 W (not measured)'
 
 
 def i8_ops_per_candidate(n):
@@ -101,25 +93,7 @@ def hbm_peak_gbs():
       return float(json.load(open(p))['hbm_gbs']), 'measured'
     except Exception:  # pylint: disable=broad-except
       pass
-  return 6650.0, 'fallback'
-
-
-def score_kernel_traffic(i8=False):
-  """dram__bytes_read.sum + dram__bytes_write.sum of one k_score launch (ncu --set full), newest summary."""
-  for name in (('score_i8_kernel_ncu_r02.json',) if i8 else ('score_kernel_ncu_r02.json', 'score_kernel_ncu_r01_latest.json')):
-    tp = os.path.join(ROOT, 'profiles', name)
-    if not os.path.exists(tp):
-      continue
-    try:
-      j = json.load(open(tp))
-
-      def _b(k):
-        v, u = float(j[k]['value']), j[k]['unit'].lower()
-        return v * {'gbyte': 1e9, 'mbyte': 1e6, 'kbyte': 1e3, 'byte': 1.0}[u]
-      return _b('dram__bytes_read.sum') + _b('dram__bytes_write.sum'), name
-    except Exception:  # pylint: disable=broad-except
-      continue
-  return None, None
+  return 3350.0, 'H100 SXM data sheet (not measured)'
 
 
 class ClockSampler:
@@ -394,7 +368,7 @@ def run_gpu(args):
   from vizier_b200.multi_gpu import trust_radius, TopkExchange
   acq = gp.Acquisition(1.8, True, trust_radius(n_trials, dim, 0))
 
-  # rotating candidate pools, together larger than the 126 MB L2, so no step re-reads its inputs from L2
+  # rotating candidate pools, together larger than the 50 MB L2, so no step re-reads its inputs from L2
   pool_bytes = m_pool * dim * 8
   n_pools = max(2, int(np.ceil(160e6 / pool_bytes)))
   pools = [dev.random_pool(m_pool, dim, seed=SEED + 17, index_base=(rank * n_pools + i) * m_pool)
@@ -443,6 +417,14 @@ def run_gpu(args):
   if dist is not None:
     dist.barrier()
   launches = dev.launch_count - l0
+  if args.dump_outputs and rank == 0:
+    # what the last timed step computed: the pool's scores and the merged winner
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    w_idx, w_val, w_x = state['winner']
+    dump = {'scores': outs[(args.steps - 1) % 2], 'winner_index': w_idx, 'winner_score': w_val, 'winner_x': w_x}
+    for name, arr in dump.items():
+      arr = arr.cpu().numpy() if hasattr(arr, 'cpu') else np.asarray(arr)
+      np.save(os.path.join(args.dump_outputs, f'{name}.npy'), np.asarray(arr, dtype=np.float64))
   total_ms = step_ev[0].elapsed_time(step_ev[-1])
   per_step = np.array([step_ev[i].elapsed_time(step_ev[i + 1]) for i in range(args.steps)])
   exchange_ok = exchange.peer.status() == 0 if exchange.peer is not None else True
@@ -473,7 +455,7 @@ def run_gpu(args):
     ev[i][1].record(stream)
   torch.cuda.synchronize()
   kern_ms = float(np.mean([a.elapsed_time(b) for a, b in ev]))
-  # which kernel that was: the tcgen05 integer-split kernel (default for pools of this size) or the FP64 DMMA kernel
+  # which kernel that was: the wgmma integer-split kernel or the FP64 DMMA kernel
   i8_before = dev.get_int('score_i8_launches')
   dev.score(pools[0], acq, out=out_k)
   used_i8 = dev.get_int('score_i8_launches') > i8_before
@@ -557,7 +539,6 @@ def run_gpu(args):
   achieved = flops / (dmma_ms * 1e-3) * 1e-12
   hbm_peak, hbm_src = hbm_peak_gbs()
   hbm_ach = algorithmic_bytes_per_candidate(dim) * m_pool / (kern_ms * 1e-3) * 1e-9
-  traffic, traffic_src = score_kernel_traffic(used_i8) if args.workload == 'c2' else (None, None)
   dmma_roof = {'bound': 'tensor', 'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak,
                'kernel': 'k_score', 'kernel_ms': dmma_ms,
                'note': 'the FP64 DMMA kernel (mma.sync m8n8k4 f64) on the same pools; peak ' + peak_src}
@@ -565,31 +546,28 @@ def run_gpu(args):
     i8_peak, i8_src = int8_peak_tops()
     i8_ach = i8_ops_per_candidate(n_trials) * m_pool / (kern_ms * 1e-3) * 1e-12
     roofline = {'bound': 'tensor', 'achieved': i8_ach, 'peak': i8_peak, 'unit': 'TOP/s', 'frac': i8_ach / i8_peak,
-                'traffic': traffic, 'traffic_source': traffic_src, 'kernel': 'k_score_i8', 'kernel_ms': kern_ms,
-                'note': 'frac is against the INT8 tensor roof of the kernel that now runs; measured against round 1\'s FP64 DMMA roof '
-                        '(frac 0.755 then) the same work is fp64_equivalent.of_fp64_dmma_peak.  '
-                        'tcgen05.mma kind::i8 (s8 x s8 -> s32 in TMEM): W = K* Linv^T as 28 exact products of balanced base-256 '
-                        'digit planes, recombined in fp64; peak = ' + i8_src + '.  M = 128, N = 64 MMAs (7 accumulator groups x 64 '
-                        'columns fill TMEM) read 6 KB of shared memory per 32-cycle MMA: the operand bandwidth bounds them at 48 '
-                        'cycles = 0.67 of the tensor peak (tools/umma_rate.cu)',
+                'kernel': 'k_score_i8', 'kernel_ms': kern_ms,
+                'note': 'frac is against the INT8 tensor roof of the kernel that runs; against the FP64 DMMA roof the same work '
+                        'is fp64_equivalent.of_fp64_dmma_peak.  wgmma s8 x s8 -> s32 (register accumulators): W = K* Linv^T as '
+                        '28 exact products of balanced base-256 digit planes, recombined in fp64; peak = ' + i8_src,
                 'int8_ops_per_candidate': i8_ops_per_candidate(n_trials),
                 'fp64_equivalent': {'tflops': flops / (kern_ms * 1e-3) * 1e-12, 'of_fp64_dmma_peak': flops / (kern_ms * 1e-3) * 1e-12 / peak,
                                     'flops_per_candidate': algorithmic_flops_per_candidate(n_trials, dim)},
                 'fp64_dmma_kernel': dmma_roof,
                 'hbm': {'achieved': hbm_ach, 'peak': hbm_peak, 'unit': 'GB/s', 'frac': hbm_ach / hbm_peak, 'peak_source': hbm_src}}
   else:
-    roofline = dict(dmma_roof, traffic=traffic, traffic_source=traffic_src,
-                    note='fp64: tcgen05 has no f64 kind, the binding roof is the FP64 DMMA pipe; peak ' + peak_src,
+    roofline = dict(dmma_roof,
+                    note='fp64: the binding roof is the FP64 DMMA pipe; peak ' + peak_src,
                     flops_per_candidate=algorithmic_flops_per_candidate(n_trials, dim),
                     hbm={'achieved': hbm_ach, 'peak': hbm_peak, 'unit': 'GB/s', 'frac': hbm_ach / hbm_peak, 'peak_source': hbm_src})
   cname = args.workload.upper()
   line = {
       'metric': 'GP-UCB candidates scored/sec', 'value': value, 'unit': 'candidates/s', 'n_gpus': world,
       'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': total_ms / args.steps,
-      'higher_is_better': True, 'scaling': wl['scaling'], 'vs_baseline': None, 'dtype': 'f64 (W = K* Linv^T as exact s8 digit products on tcgen05)' if used_i8 else 'f64', 'data': 'synthetic',
+      'higher_is_better': True, 'scaling': wl['scaling'], 'vs_baseline': None, 'dtype': 'f64 (W = K* Linv^T as exact s8 digit products on the int8 tensor cores)' if used_i8 else 'f64', 'data': 'synthetic',
       'config': {'workload': f'{cname}: GP posterior mu/var + UCB + trust region + top-1, N={n_trials}, D={dim}, M={m_pool} per GPU'
                              + (f' ({wl["m_total"]} in total)' if wl['m_total'] else ''),
-                 'l2': f'{n_pools} rotating candidate pools ({n_pools * pool_bytes / 1e6:.0f} MB > 126 MB L2)',
+                 'l2': f'{n_pools} rotating candidate pools ({n_pools * pool_bytes / 1e6:.0f} MB > 50 MB L2)',
                  'parallelism': (f'candidate-pool shards x{world}; global arg-max by ONE fused kernel per step (NVLink peer stores + '
                                  f'release/acquire flags + merge), transport={exchange.transport}') if world > 1 else 'single GPU',
                  'suggest_latency_ms': suggest_latency_ms, 'ranks_agree': ranks_agree, 'exchange_ok': exchange_ok,
@@ -628,8 +606,12 @@ def main():
   ap.add_argument('--workload', default='c2', choices=sorted(WORKLOADS))
   ap.add_argument('--no-suggest', action='store_true', help='skip the suggest() end-to-end leg (N=1)')
   ap.add_argument('--no-cpu', action='store_true',
-                  help='skip the cpu_baseline leg and everything that spawns processes (runs under ncu)')
+                  help='skip the cpu_baseline leg and everything that spawns processes')
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                  help='after the timed steps, write the last timed step\'s outputs to DIR/<name>.npy')
   args = ap.parse_args()
+  if args.dump_outputs and args.impl == 'reference':
+    ap.error('--dump-outputs writes what the GPU path computed; --impl reference has no such outputs')
   args.warmup = max(args.warmup, 3) if args.impl == 'b200' else args.warmup
   if args.impl == 'reference':
     run_reference(args)

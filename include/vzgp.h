@@ -1,10 +1,10 @@
 /*
- * vzgp.h -- C ABI of libvzgp.so: the B200 (sm_100a) GP-Bandit hot path.
+ * vzgp.h -- C ABI of libvzgp.so: the H100 (sm_90a) GP-Bandit hot path.
  *
  * The reference (google/vizier @ b0651861) has NO native/FFI layer: its
  * GP-bandit arithmetic is reached through JAX/TFP Python calls.  Each entry
  * point below replaces one of those Python call sites (cited as
- * file:line under /root/reference); the Python host (vizier_b200/) binds them
+ * file:line in the reference); the Python host (vizier_b200/) binds them
  * with ctypes, and INTEGRATION.md shows the stub a Vizier maintainer would
  * add to vizier/_src/algorithms/designers/gp_bandit.py.
  *
@@ -111,10 +111,10 @@ int64_t vzgp_launch_count(const vzgp_handle* h);
 /* Tuning knobs.  "dataflow_ctas": worker CTAs the dataflow factorisation launches (0 = every resident slot;
  * callers that run several handles concurrently, like the ARD restarts, give each an equal share).
  * "score_i8": 1 = large candidate pools (>= one 64-candidate tile per SM, 128 <= padded N <= 4096, no linear
- * kernel) are scored by the tcgen05 integer-split kernel, 0 = always the FP64 DMMA kernel, -1 = the process
- * default (environment VZGP_SCORE_I8, default 1). */
+ * kernel) are scored by the wgmma integer-split kernel, 0 = always the FP64 DMMA kernel, -1 = the process
+ * default (environment VZGP_SCORE_I8, default 0). */
 int vzgp_set_int(vzgp_handle* h, const char* key, int value);
-/* Counters.  "launches" (= vzgp_launch_count), "score_i8_launches": launches of the tcgen05 scoring kernel. */
+/* Counters.  "launches" (= vzgp_launch_count), "score_i8_launches": launches of the integer-split scoring kernel. */
 int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value);
 
 /* ---- stage-wise entry points (parity tests call these one by one) -------- */

@@ -1,7 +1,7 @@
-"""The tcgen05 / TMEM integer-split scoring kernel (score_i8.cu) against the oracle and against the DMMA kernel.
+"""The wgmma integer-split scoring kernel (score_i8.cu) against the oracle and against the DMMA kernel.
 
 `vzgp_set_int(h, "score_i8", 1)` routes pools of at least one 64-candidate tile per SM through `k_score_i8`
-(exact int8 digit products with int32 accumulation in TMEM, recombined in fp64); everything else about the
+(exact int8 digit products with int32 accumulation in registers, recombined in fp64); everything else about the
 call is unchanged, so the same oracle checks apply with the same tolerances.
 """
 import numpy as np
@@ -47,12 +47,12 @@ def _pool(dev, m, d, seed):
 
 
 @pytest.mark.parametrize('n,d,sf2', [(1000, 20, 1.0), (520, 7, 2.7), (192, 3, 0.31), (1030, 12, 1.0), (300, 40, 1.0),
-                                     (2000, 50, 0.9999999)])
+                                     (2000, 50, 0.9999999), (300, 64, 1.0)])
 def test_i8_scores_match_oracle_and_dmma(dev, n, d, sf2):
-  """np = 1024 / 576 (a half k chunk and a half j tile) / 192 / 1088; sf2 off a power of two; Dc = 40 and 50: the
-  phase-1 staging no longer fits next to the operand ring (nbuf = 1, phases back to back); C4's N = 2000 with sf2
-  just below a power of two (the balanced top digit needs the extra scale bit)."""
-  m = 148 * 64 + 37
+  """np = 1024 / 576 (a half k chunk) / 192 / 1088; sf2 off a power of two; Dc = 40 and 50: one phase-1 trial
+  buffer; Dc = 64: the phase-1 staging no longer fits next to the operand ring (nbuf = 1, phases back to back); C4's
+  N = 2000 with sf2 just below a power of two (the balanced top digit needs the extra scale bit)."""
+  m = 148 * 64 + 37     # 149 tiles: more than one per SM on 132 SMs, so some CTAs reuse their digit buffers
   x, y, _ = _problem(n, d, n)
   po, pg = _params(d, sf2=sf2)
   dev.fit(x, y, pg)
@@ -137,7 +137,7 @@ def test_i8_refit_invalidates_digit_planes(dev):
 
 def test_i8_two_handles_on_two_streams_concurrently():
   """Two models scoring large pools at the same time from two host threads (separate handles and streams): the
-  kernels take turns on the SMs (one CTA per SM: shared memory and the 512 TMEM columns); results equal the serial ones."""
+  kernels take turns on the SMs (one CTA per SM: shared memory and registers); results equal the serial ones."""
   import threading
   gp = _gp()
   devs, pools, want = [], [], []

@@ -1,4 +1,4 @@
-"""k_score (DMMA) against k_score_i8 (tcgen05 int8 split) on the C2 pool: CUDA-event time per pass."""
+"""k_score (DMMA) against k_score_i8 (wgmma int8 split) on the C2 pool: CUDA-event time per pass."""
 import json
 import sys
 import numpy as np

@@ -1,7 +1,7 @@
 // Measures the achievable FP64 throughput of this GPU: DFMA (vector pipe) and DMMA
 // (mma.sync m8n8k4 / m16n8k8 / m16n8k16 f64) alone and together.  The result is the roofline
 // denominator for the posterior-variance contraction (MEASURED_PEAKS.json has no fp64 entry).
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/_bin/fp64_peak tools/fp64_peak.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/_bin/fp64_peak tools/fp64_peak.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>

@@ -8,8 +8,7 @@ import torch
 sys.path.insert(0, '.')
 from vizier_b200 import _lib, gp  # noqa: E402
 
-NAMES = ['phase1', 'epi_wait', 'epi', 'tile', 'mma_wait_epi', 'mma_wait_B', 'mma_wait_A', 'mma_total',
-         'prod_wait_B', 'prod_wait_A', 'prod_total', 'prod_wait_kready', 'k_wait_kfree']
+NAMES = {0: 'phase1', 3: 'tile', 12: 'k_wait_kfree'}
 
 
 def main():
@@ -42,7 +41,7 @@ def main():
   t = np.array(buf[:], dtype=np.int64)
   tiles = max(int(t[15]), 1)
   res = {'ms_per_pass': e0.elapsed_time(e1) / 8, 'tiles_cta0': tiles,
-         'cycles_per_tile': {k: int(t[i] // tiles) for i, k in enumerate(NAMES)}}
+         'cycles_per_tile': {k: int(t[i] // tiles) for i, k in NAMES.items()}}
   print(json.dumps(res))
 
 

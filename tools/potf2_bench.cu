@@ -1,9 +1,12 @@
 // Times k_potf2_inv (64x64 diagonal-block Cholesky + inverse) in isolation: back-to-back launches
 // with CUDA events, on a warmed-up GPU.  Build:
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/_bin/potf2_bench tools/potf2_bench.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/_bin/potf2_bench tools/potf2_bench.cu
 #define VZ_POTF2_TIMING 1
 #include "../vizier_b200/csrc/linalg.cu"
-namespace vzgp { void set_error(const char*, ...) {} }
+namespace vzgp {
+void set_error(const char*, ...) {}
+int raise_dyn_smem(const void* k, size_t b) { return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b) == cudaSuccess ? 0 : -2; }
+}
 #include <vector>
 #include <cstdio>
 __global__ void k_spin(double* x, int n) { double v = x[0]; for (int i = 0; i < n; ++i) v = fma(v, 1.0000001, 1e-9); x[0] = v; }
@@ -18,7 +21,7 @@ int main() {
   cudaMemcpy(A, h.data(), sizeof(double) * 4096, cudaMemcpyHostToDevice);
   cudaFuncSetAttribute(k_potf2_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiagSmem);
   // warm the whole GPU so clocks are up
-  for (int i = 0; i < 20; ++i) k_spin<<<148 * 8, 256>>>(sp, 200000);
+  for (int i = 0; i < 20; ++i) k_spin<<<132 * 8, 256>>>(sp, 200000);
   cudaDeviceSynchronize();
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   const int reps = 500;

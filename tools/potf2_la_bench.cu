@@ -1,7 +1,7 @@
 // potf2_inv_64 (round 1) against potf2_inv_64_la (look-ahead, round 2) in isolation: one CTA of 256 threads
 // factors + inverts the same 64 x 64 SPD block REPS times from shared memory; cycles per call from clock64
 // around the whole loop (no stamps inside the routines), results compared with each other.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -maxrregcount=96 -o tools/_bin/potf2_la_bench tools/potf2_la_bench.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -maxrregcount=96 -o tools/_bin/potf2_la_bench tools/potf2_la_bench.cu
 #include <cstdio>
 #include <vector>
 #include "../vizier_b200/csrc/potf2.cuh"

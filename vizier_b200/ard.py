@@ -207,7 +207,7 @@ def _cta_share(n_concurrent: int) -> int:
   """Worker CTAs of the dataflow factorisation per concurrent evaluation (0 = every slot, a lone evaluation).
   The persistent CTAs of k_chol_dataflow fill an SM's shared memory and registers two by two; the small kernels
   around the factorisation (kernel matrix, alpha solve, gradient tiles) of the OTHER evaluations need somewhere
-  to run meanwhile, so the restarts together take only part of the 2 x 148 slots."""
+  to run meanwhile, so the restarts together take only part of the 2 x 132 slots."""
   import os
   if n_concurrent <= 1:
     return 0
@@ -233,7 +233,7 @@ def loss_functions(dev: gp.DeviceGP, xt, yt, zt, dc: int, dk: int, n_valid: Opti
     pool.append(gp.DeviceGP(dev.device.index))
   devs = [dev] + pool[:workers - 1]
   # The evaluations of the restarts run concurrently, one dataflow-factorisation launch each: an equal
-  # share of the 2 x 148 resident CTA slots keeps all of them on the GPU at once (csrc/dataflow.cu).
+  # share of the 2 x 132 resident CTA slots keeps all of them on the GPU at once (csrc/dataflow.cu).
   share = _cta_share(len(devs))
   for d in devs:
     d.set_int('dataflow_ctas', share)

@@ -2,6 +2,9 @@
 #include <climits>
 #include <cstdarg>
 #include <cstring>
+#include <map>
+#include <mutex>
+#include <utility>
 #include <vector>
 
 #include "launchers.h"
@@ -17,6 +20,18 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int raise_dyn_smem(const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, size_t> limits;
+  int dev = 0;
+  VZ_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& cur = limits[{dev, kernel}];
+  if (bytes <= cur) return 0;
+  VZ_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  cur = bytes;
+  return 0;
+}
 
 // Layout of handle->small (device, 64 KiB).
 constexpr size_t kSmallBytes = 65536;
@@ -743,8 +758,7 @@ static int score_host_enqueue(vzgp_handle* h, const double* Xs, const int32_t* Z
   int nchunk = 0;
   {
     int pos = 0;
-    // one wave, three waves, the rest: every copy lands while the previous chunk is being scored (two chunks were
-    // tried with the tcgen05 kernel to save one launch: the 14 MB second copy is then exposed, 2.95 vs 2.69 ms)
+    // one wave, three waves, the rest: every copy lands while the previous chunk is being scored
     const int plan[2] = {wave, 3 * wave};
     for (int i = 0; i < 2 && M - pos > 2 * plan[i]; ++i) { pos += plan[i]; bounds[++nchunk] = pos; }
     bounds[++nchunk] = M;

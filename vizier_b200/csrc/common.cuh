@@ -20,6 +20,8 @@ constexpr int kMaxMetrics = 8; // metrics of the independent multi-task GP (one 
 constexpr int kNllBufs = 15;   // handle buffers a captured NLL graph points into
 
 void set_error(const char* fmt, ...);
+// Raises (never lowers: other threads may be about to launch larger) `kernel`'s dynamic shared-memory limit.
+int raise_dyn_smem(const void* kernel, size_t bytes);
 
 #define VZ_CUDA(expr)                                                              \
   do {                                                                             \
@@ -113,7 +115,7 @@ struct vzgp_handle {
   int device = 0;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
-  int sm_count = 148;
+  int sm_count = 132;
   int64_t launches = 0;
 
   // Fitted model (all padded to np = round_up(n, 64); pad rows are identity/zero).
@@ -167,8 +169,8 @@ struct vzgp_handle {
   int df_nb[2] = {0, 0}, df_ntasks[2] = {0, 0}, df_ncrit[2] = {0, 0};
   int df_ctas = 0;                              // worker CTAs per launch (0: all slots); vzgp_set_int
 
-  // Integer-split scoring on tcgen05 (score_i8.cu): digit planes of Linv, their row scales, K* digit scratch.
-  int score_i8 = -1;                            // -1: environment VZGP_SCORE_I8 (default on), 0 / 1: vzgp_set_int
+  // Integer-split scoring on the int8 tensor cores (score_i8.cu): digit planes of Linv, their row scales, K* digit scratch.
+  int score_i8 = -1;                            // -1: environment VZGP_SCORE_I8 (default off), 0 / 1: vzgp_set_int
   bool i8_ready = false;                        // the digit planes describe the current Linv
   int64_t i8_launches = 0;
   vzgp::DevBuf i8_planes, i8_scale, i8_kdig;

@@ -445,10 +445,8 @@ size_t eagle_update_smem(const EagleDev& e) {
   return sizeof(double) * (size_t)(e.B + e.count) + (size_t)(e.B + e.count) + 16;
 }
 int eagle_prepare(const EagleDev& e) {
-  VZ_CUDA(cudaFuncSetAttribute(k_eagle_suggest, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)eagle_suggest_smem(e)));
-  VZ_CUDA(cudaFuncSetAttribute(k_eagle_update, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)eagle_update_smem(e)));
+  VZ_TRY(raise_dyn_smem((const void*)k_eagle_suggest, eagle_suggest_smem(e)));
+  VZ_TRY(raise_dyn_smem((const void*)k_eagle_update, eagle_update_smem(e)));
   return 0;
 }
 int launch_eagle_suggest(vzgp_handle* h, const EagleDev& e) {
@@ -516,7 +514,7 @@ int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e
                                       (size_t)nm * 64 + 128 + 128 + 64 + 256) +
                     sizeof(int32_t) * ((size_t)(nm + 1) * h->dk * kPXLD + 2) + eagle_persistent_state_bytes(e);
   if (sm > 227 * 1024) { set_error("persistent eagle kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
-  VZ_CUDA(cudaFuncSetAttribute(k_eagle_persistent64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  VZ_TRY(raise_dyn_smem((const void*)k_eagle_persistent64, sm));
   k_eagle_persistent64<<<1, kPThreads, sm, h->stream>>>(e, m, mb, q, steps, scratch, h->small.as<int>());
   VZ_CHECK_LAUNCH();
   h->launches++;

@@ -187,7 +187,7 @@ int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const 
   if (s_c > sm) sm = s_c;
   if (s_v > sm) sm = s_v;
   if (sm > 227 * 1024) { set_error("eagle grid kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
-  VZ_CUDA(cudaFuncSetAttribute(k_eagle_grid, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  VZ_TRY(raise_dyn_smem((const void*)k_eagle_grid, sm));
   int occ = 0;
   VZ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_eagle_grid, kSmallThreads, sm));
   if (occ < 1) { set_error("eagle grid kernel does not fit on an SM"); return VZGP_ERR_UNSUPPORTED; }

@@ -75,7 +75,7 @@ int chol_dataflow_timed_out(vzgp_handle* h, int* out);
 
 int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
                  double* score, double* mu, double* sigma, double* linf);
-// tcgen05 / TMEM integer-split variant of the large-pool scoring kernel (score_i8.cu).
+// wgmma integer-split variant of the large-pool scoring kernel (score_i8.cu).
 bool score_i8_eligible(const vzgp_handle* h, int M);
 int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
                     double* score, double* mu, double* sigma, double* linf);

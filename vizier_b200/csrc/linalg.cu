@@ -500,7 +500,7 @@ int launch_kernel_matrix(vzgp_handle* h, const double* X, const int32_t* Z, int 
                          const KernelParams& kp, double diag_add, double* K, int ldk) {
   int nb = (n + 63) / 64;
   size_t sm = kernel_smem_bytes(kp.dc, kp.dk, 64, 64);
-  VZ_CUDA(cudaFuncSetAttribute(k_kernel_matrix, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  VZ_TRY(raise_dyn_smem((const void*)k_kernel_matrix, sm));
   k_kernel_matrix<<<dim3(nb, nb), 256, sm, h->stream>>>(X, Z, n, n_valid, kp, diag_add, K, ldk);
   VZ_CHECK_LAUNCH();
   h->launches++;
@@ -511,7 +511,7 @@ int launch_cross_kernel(vzgp_handle* h, const double* Xs, const int32_t* Zs, int
                         const int32_t* Z, int n, int n_valid, const KernelParams& kp, double* Ks,
                         int ldks) {
   size_t sm = kernel_smem_bytes(kp.dc, kp.dk, 128, 64);
-  VZ_CUDA(cudaFuncSetAttribute(k_cross_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  VZ_TRY(raise_dyn_smem((const void*)k_cross_kernel, sm));
   dim3 grid((n + 63) / 64, (M + 127) / 128);
   k_cross_kernel<<<grid, 256, sm, h->stream>>>(Xs, Zs, M, X, Z, n, n_valid, kp, Ks, ldks);
   VZ_CHECK_LAUNCH();
@@ -528,7 +528,7 @@ int potrf_blocked(vzgp_handle* h, double* L, int ld, double* Linv, int ldi, int 
   VZ_CUDA(cudaFuncSetAttribute(k_potf2_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDiagSmem));
   const size_t sm = G64::kSmemBytes;
   const size_t sm2 = sm > kDiagSmem ? sm : kDiagSmem;
-  VZ_CUDA(cudaFuncSetAttribute(k_syrk_potf2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
+  VZ_TRY(raise_dyn_smem((const void*)k_syrk_potf2, sm2));
   // Right-looking with one block of look-ahead: block 0 is factored alone; afterwards the trailing
   // update of step kb also factors diagonal block kb+1 (k_syrk_potf2).
   k_potf2_inv<<<1, 256, kDiagSmem, h->stream>>>(L, ld, 0, Linv, ldi, flag);

@@ -150,12 +150,12 @@ int launch_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int 
   none.tr_rows = 0; none.tr_strict = 0;
   VZ_TRY(launch_score(h, Xs, Zs, M, &none, dummy, nullptr, sd, nullptr));
   const size_t sm = sizeof(double) * (2 * h->dc * 66 + kMaxMetrics * 64) + sizeof(int32_t) * 2 * h->dk * 66;
-  VZ_CUDA(cudaFuncSetAttribute(k_mean_multi, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  VZ_TRY(raise_dyn_smem((const void*)k_mean_multi, sm));
   k_mean_multi<<<(M + 63) / 64, 256, sm, h->stream>>>(Xs, Zs, M, h->X.as<double>(), h->Z.as<int32_t>(), h->np, h->n_valid,
                                                       h->kp, h->alpha.as<double>(), nm, mu, M);
   VZ_CHECK_LAUNCH();
   const size_t sm2 = sizeof(double) * (wn + S);
-  VZ_CUDA(cudaFuncSetAttribute(k_scalarize, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
+  VZ_TRY(raise_dyn_smem((const void*)k_scalarize, sm2));
   k_scalarize<<<(M + 255) / 256, 256, sm2, h->stream>>>(M, a, mu, M, sd, h->scal.as<double>(),
                                                         h->scal.as<double>() + wn, score);
   VZ_CHECK_LAUNCH();

@@ -152,7 +152,7 @@ int launch_nll_grad_tiles(vzgp_handle* h, const double* X, const int32_t* Z, int
                           double* partial, double* out, int plane_rows, int n_metrics) {
   const int nb = np / 64, nq = kp.dc + kp.dk + 2 + (kp.use_linear ? kp.dc + 2 : 0), ntiles = nb * (nb + 1) / 2;
   size_t sm = sizeof(double) * (kp.dc * 2 * 66 + 8 * nq) + sizeof(int32_t) * kp.dk * 2 * 66;
-  VZ_CUDA(cudaFuncSetAttribute(k_nll_grad_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  VZ_TRY(raise_dyn_smem((const void*)k_nll_grad_tiles, sm));
   k_nll_grad_tiles<<<dim3(nb, nb), 256, sm, h->stream>>>(X, Z, np, n_valid, kp, Kinv, ldk, plane_rows > 0 ? plane_rows : lauum_plane_rows(np), alpha,
                                                          partial, nb, n_metrics, np);
   VZ_CHECK_LAUNCH();

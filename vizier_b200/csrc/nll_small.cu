@@ -199,7 +199,7 @@ size_t nll_small_smem_bytes(int dc, int dk) {
 int launch_nll_grad_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int n_valid,
                           const KernelParams& kp, double sn2, double jitter0, int max_iters, double* out) {
   const size_t sm = nll_small_smem_bytes(kp.dc, kp.dk);
-  VZ_CUDA(cudaFuncSetAttribute(k_nll_grad_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  VZ_TRY(raise_dyn_smem((const void*)k_nll_grad_small, sm));
   k_nll_grad_small<<<1, 256, sm, h->stream>>>(X, Z, y, N, n_valid, kp, sn2, jitter0, max_iters, out);
   VZ_CHECK_LAUNCH();
   h->launches++;

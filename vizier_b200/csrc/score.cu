@@ -13,7 +13,7 @@
 //            staged rows; mu = K* alpha and the L-inf trust-region distance are reduced on the
 //            fly; the tile goes to a CTA-private scratch (L2 resident, never re-read by others).
 //   phase 2  W = K* . Linv^T in 64 x 128 blocks on the FP64 tensor pipe (mma.sync m8n8k4 f64;
-//            tcgen05 has no f64 kind), operands streamed by a TMA producer warp (cp.async.bulk.tensor,
+//            the only fp64 tensor-core instruction), operands streamed by a TMA producer warp (cp.async.bulk.tensor,
 //            128-byte swizzle) through a 4-stage ring with full/empty mbarriers, exploiting that
 //            Linv is lower triangular (k <= j, all-zero fragments skipped); each block is squared
 //            and row-summed in registers, W is never stored.
@@ -643,14 +643,14 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
     const size_t sm1 = cross_small_smem_bytes(h->dc, h->dk), sm2 = var_small_smem_bytes();
     const dim3 g1(nmb, ntiles * 4), g2(nvb, ntiles);
     if (with_linf) {
-      VZ_CUDA(cudaFuncSetAttribute(k_cross_small<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
+      VZ_TRY(raise_dyn_smem((const void*)k_cross_small<true>, sm1));
       k_cross_small<true><<<g1, kSmallThreads, sm1, h->stream>>>(a);
     } else {
-      VZ_CUDA(cudaFuncSetAttribute(k_cross_small<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1));
+      VZ_TRY(raise_dyn_smem((const void*)k_cross_small<false>, sm1));
       k_cross_small<false><<<g1, kSmallThreads, sm1, h->stream>>>(a);
     }
     VZ_CHECK_LAUNCH();
-    VZ_CUDA(cudaFuncSetAttribute(k_var_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2));
+    VZ_TRY(raise_dyn_smem((const void*)k_var_small, sm2));
     k_var_small<<<g2, kSmallThreads, sm2, h->stream>>>(a);
     VZ_CHECK_LAUNCH();
     if (with_linf) k_small_finalize<true><<<(M + 31) / 32, 256, 0, h->stream>>>(a);
@@ -660,7 +660,9 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
     return 0;
   }
   {
-    static const int env_i8 = [] { const char* e = getenv("VZGP_SCORE_I8"); return e ? atoi(e) : 1; }();
+    // Default off: on the H100 the 28 int8 digit products per fp64 product cost more than the FP64 DMMA pipe
+    // (C2 pool: 5.18 ms for k_score_i8 against 4.35 ms for k_score, H100 80GB HBM3 at a 700 W power limit).
+    static const int env_i8 = [] { const char* e = getenv("VZGP_SCORE_I8"); return e ? atoi(e) : 0; }();
     const int want = h->score_i8 >= 0 ? h->score_i8 : env_i8;
     if (want && score_i8_eligible(h, M)) return launch_score_i8(h, Xs, Zs, M, acq, score, mu, sigma, linf);
   }
@@ -686,10 +688,10 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
     return VZGP_ERR_UNSUPPORTED;
   }
   if (need_linf) {
-    VZ_CUDA(cudaFuncSetAttribute(k_score<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    VZ_TRY(raise_dyn_smem((const void*)k_score<true>, sm));
     k_score<true><<<grid, kBlockThreads, sm, h->stream>>>(a);
   } else {
-    VZ_CUDA(cudaFuncSetAttribute(k_score<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    VZ_TRY(raise_dyn_smem((const void*)k_score<false>, sm));
     k_score<false><<<grid, kBlockThreads, sm, h->stream>>>(a);
   }
   VZ_CHECK_LAUNCH();

@@ -1,11 +1,10 @@
-// The W = K* . Linv^T contraction of the scoring path on the 5th-generation tensor cores (tcgen05, TMEM),
+// The W = K* . Linv^T contraction of the scoring path on the Hopper tensor cores (wgmma, s8 x s8 -> s32),
 // by an Ozaki-style exact integer split of the fp64 operands.
 //
 // Same contract as k_score (score.cu): posterior mean / variance + UCB + trust region for a candidate pool;
-// replaces BayesianScoringFunction.score_with_aux (acquisitions.py:177-207).  The FP64 tensor pipe (DMMA) tops
-// out at ~37 TFLOP/s on this chip; tcgen05 has no f64 kind but multiplies 8-bit integers with exact 32-bit
-// accumulation at ~100x that rate.  So both operands are written as fixed-point numbers of 7 base-256 digits
-// relative to a power-of-two row scale, with BALANCED digits,
+// replaces BayesianScoringFunction.score_with_aux (acquisitions.py:177-207).  The tensor cores have no fp64 kind
+// beyond DMMA; wgmma multiplies 8-bit integers with exact 32-bit accumulation.  So both operands are written as
+// fixed-point numbers of 7 base-256 digits relative to a power-of-two row scale, with BALANCED digits,
 //     K*[i,k]   = 2^ea   * sum_{s=1..7} a_s[i,k] 2^(-8s)      a_s in [-128,127]
 //     Linv[j,k] = 2^eb_j * sum_{t=1..7} b_t[j,k] 2^(-8t)      b_t in [-128,127]
 // i.e. 55 bits below the row maximum - what fp64 carries for the entries that dominate the sum - and
@@ -16,16 +15,14 @@
 // same order as the rounding of an fp64 accumulation.
 //
 // One persistent CTA per SM, 64 candidates per tile:
-//   phase 1   (16 worker warps)  K* tile by 64-column steps as in k_score; mu and the L-inf distance on the
-//             fly; every K* value is cut into its 7 digits and stored to a CTA-private scratch
+//   phase 1   (8 K* warps)  K* tile by 64-column steps as in k_score; mu and the L-inf distance on the fly;
+//             every K* value is cut into its 7 digits and stored to a CTA-private scratch
 //             [7 digit planes][64 candidates][np] (L2 resident).
-//   phase 2   MMA D[128 x 64] (TMEM, s32) += A[128 x 32] B[64 x 32]^T with A = a digit plane of Linv rows
-//             (j tile of 128), B = a digit plane of the candidates' K*; 7 accumulator groups (g) of 64 TMEM
-//             columns.  A TMA producer thread streams, per 128-byte k chunk, the 7 K* planes (56 KB, double
-//             buffered) and the 7 Linv planes (16 KB each through a 4-slot ring); ONE thread issues the 112
-//             tcgen05.mma of the chunk and hands the buffers back with tcgen05.commit.
-//   epilogue  (worker warps) tcgen05.ld the 7 groups, recombine in 64-bit integers, scale, square and add
-//             into per-candidate sums; after the last j tile: variance, sigma, UCB, trust region.
+//   phase 2   (one consumer warpgroup)  D[64 x 32] (s32 registers) += A B^T, A = a Linv digit plane (j tile of
+//             64 rows), B = a K* digit plane of 32 candidates; 7 accumulator groups (g).  Per 128-byte k chunk the
+//             14 planes are TMA-loaded into one of two stages, one chunk ahead of its 112 wgmma.
+//   epilogue  (the same warpgroup) recombine the 7 groups in 64-bit integers, scale, square and add into
+//             per-candidate sums; after the last j tile: variance, sigma, UCB, trust region.
 #include <cuda.h>
 
 #include <climits>
@@ -50,30 +47,27 @@ namespace vzgp {
 
 namespace {
 
-constexpr int kKWarps = 16;                   // K* warps (phase 1); 22 warps in all -> 80 registers per thread
-constexpr int kEWarps = 4;                    // epilogue warps: 4 TMEM lane quarters x kEWarps / 4 column blocks (8 warps:
-                                              // 72 registers, same 2.48 ms - the shorter epilogue buys nothing)
-constexpr int kEGroups = 8 / (kEWarps / 4);   // 8-candidate column groups per epilogue warp
-constexpr int kI8Threads = (kKWarps + kEWarps + 2) * 32;     // + TMA producer warp + MMA issuer warp
+// The consumer warpgroup needs 160 registers per thread (112 accumulators); ptxas gives all threads that budget.
+constexpr int kKWarps = 8;                    // K* warps (phase 1)
+constexpr int kEWarps = 4;                    // the consumer warpgroup: MMA issue and epilogue
+constexpr int kI8Threads = (kKWarps + kEWarps) * 32;
 constexpr int kDigits = 7;
 constexpr int kGroups = 7;                    // g = s + t - 2 in [0, 6]
-constexpr int kJT = 128;                      // Linv rows per j tile = MMA M
+constexpr int kJT = 64;                       // Linv rows per j tile = wgmma M
+constexpr int kCN = 32;                       // candidates per wgmma = N (half of the 64-candidate tile)
 constexpr int kKC = 128;                      // bytes (= k values) per chunk: one 128-byte swizzle atom per row
-constexpr int kASlotBytes = kJT * kKC;        // 16 KB: one digit plane of a j tile x k chunk
-constexpr int kASlots = 4;                   // most; large Dc trades slots for the phase-1 staging (I8Args::n_aslots)
-constexpr int kBPlaneBytes = kTM * kKC;       // 8 KB
-constexpr int kBBufBytes = kDigits * kBPlaneBytes;   // 56 KB: all digit planes of the candidates' k chunk
-constexpr int kRingBytes = 2 * kBBufBytes + kASlots * kASlotBytes;   // 176 KB
-constexpr int kTmemCols = 512;
+constexpr int kAPlaneBytes = kJT * kKC;       // 8 KB: one digit plane of a j tile x k chunk
+constexpr int kBPlaneBytes = kCN * kKC;       // 4 KB: one digit plane of a candidate half x k chunk
+constexpr int kStageBytes = kDigits * (kAPlaneBytes + kBPlaneBytes);   // 84 KB
+constexpr int kRingBytes = 2 * kStageBytes;   // 168 KB
 
 struct I8Args {
-  alignas(64) CUtensorMap mapK;   // K* digit scratch as u8 [grid*7*64 rows][np], box 64 x 128, SWIZZLE_128B
-  alignas(64) CUtensorMap mapL;   // Linv digit planes as u8 [7][np][np], box 1 x 128 x 128, SWIZZLE_128B
+  alignas(64) CUtensorMap mapK;   // K* digit scratch as u8 [grid*7*64 rows][np], box 32 x 128, SWIZZLE_128B
+  alignas(64) CUtensorMap mapL;   // Linv digit planes as u8 [7][np][np], box 1 x 64 x 128, SWIZZLE_128B
   ScoreArgs s;                    // candidates, model, outputs (mapA / mapB / scratch unused)
   uint8_t* kdig;                  // [grid][nbuf][7][64][np]
   int nbuf;                       // 2: phase 1 of the next tile overlaps phase 2; 1: back to back (large Dc)
   int misc_bytes;                 // shared memory between the operand ring and the (nbuf = 2) phase-1 staging
-  int n_aslots;                   // Linv plane slots in the ring (2 .. kASlots)
   int sb_bufs;                    // trial staging buffers of phase 1: 2 (copy of step jb + 1 under the math of jb) or 1
   const double* lscale;           // [np]  2^(ea + eb_j - 32)
   double kscale;                  // 2^(56 - ea)
@@ -99,29 +93,44 @@ __device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, unsigned parity
   }
 }
 
-__device__ __forceinline__ void tma_load_3d_elect(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
   asm volatile(
-      "{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-      "@e cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];\n\t}\n" ::"r"(smem_u32(smem_dst)),
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];\n" ::"r"(smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
       : "memory");
 }
 
-// K-major operand tile in the 128-byte-swizzle layout TMA writes: rows of 128 bytes, 8-row groups 1024 bytes
-// apart (SBO), descriptor version 1, layout type 2 (SWIZZLE_128B).  The tile base is 1024-byte aligned; a
-// 32-byte k step inside the atom adds 2 to the (16-byte unit) start address.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// wgmma shared-memory matrix descriptor of a K-major operand tile in the 128-byte-swizzle layout TMA writes: rows
+// of 128 bytes, 8-row groups 1024 bytes apart (stride byte offset), swizzle mode 1 (128B) in bits 62-63.  The tile
+// base is 1024-byte aligned; a 32-byte k step inside the atom adds 2 to the (16-byte unit) start address.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// kind::i8 instruction descriptor: D = s32, A = B = s8, both K-major, M = 128, N = 64.
-__host__ __device__ constexpr uint32_t umma_idesc_i8() {
-  return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kTM >> 3) << 17) | ((uint32_t)(kJT >> 4) << 24);
+// D[64 x 32] (+)= A[64 x 32] B[32 x 32]^T, s8 operands from shared memory, s32 accumulators in registers.
+__device__ __forceinline__ void wgmma_i8(int32_t (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accumulator reads or writes across a wgmma fence / wait.
+__device__ __forceinline__ void acc_fence(int32_t (&acc)[kGroups][16]) {
+#pragma unroll
+  for (int g = 0; g < kGroups; ++g)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) asm volatile("" : "+r"(acc[g][i])::"memory");
 }
 // Power-of-two scale exponent e with |x| 2^-e <= 0.498 for |x| <= m: the top balanced digit stays in [-128, 127].
 __host__ __device__ inline int balanced_scale_exp(double m) {
@@ -129,46 +138,9 @@ __host__ __device__ inline int balanced_scale_exp(double m) {
   const double f = frexp(m, &e);
   return f < 0.996 ? e + 1 : e + 2;
 }
-// The issuing warps run their loops with warp-uniform control flow and elect the issuing lane INSIDE the asm
-// statement: ptxas then keeps descriptors and addresses in uniform registers.  (Issuing from an `if (lane == 0)`
-// region costs an ELECT + R2UR round trip per instruction: 131 cycles per MMA instead of 48, tools/umma_rate.cu.)
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, e;\n\telect.sync _|e, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx_elect(uint64_t* bar, unsigned bytes) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-      "@e mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}\n" ::"r"(smem_u32(bar)), "r"(bytes)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_elect(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-      "@e cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n\t}\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld4(uint32_t addr, int32_t (&v)[4]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];\n"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
-               : "r"(addr));
-}
 __device__ __forceinline__ void st_u16_keep(void* p, uint16_t v, uint64_t policy) {
   asm volatile("st.global.L2::cache_hint.u16 [%0], %1, %2;\n" ::"l"(p), "h"(v), "l"(policy) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
 
 __device__ __forceinline__ void g_i8_t_tiles() {
 #ifdef VZ_I8_TIMING
@@ -176,11 +148,10 @@ __device__ __forceinline__ void g_i8_t_tiles() {
 #endif
 }
 
-// Warp roles: 8 K* warps (phase 1 of tile n+1 while tile n is in phase 2), 8 epilogue warps, one TMA producer
-// warp, one MMA issuer warp.  Hand-over by mbarriers only:
-//   kready[b]  K* warps -> producer + epilogue: digit planes / mu / L-inf of the tile in buffer b are complete
-//   kfree[b]   epilogue -> K* warps: the tile that used buffer b is finished (all its TMA reads are consumed)
-//   bfull/bempty, afull/aempty   TMA <-> MMA operand buffers;  tfull/tempty   MMA <-> epilogue accumulators
+// Hand-over between the K* warps and the consumer warpgroup by mbarriers only:
+//   kready[b]  K* warps -> consumer: digit planes / mu / L-inf of the tile in buffer b are complete
+//   kfree[b]   consumer -> K* warps: the tile that used buffer b is finished (all its TMA reads are consumed)
+//   full[s]    TMA -> consumer: operand stage s has landed
 // nbuf = 2 overlaps the phases (digit scratch and phase-1 staging have their own memory); nbuf = 1 (large Dc:
 // the staging does not fit next to the operand ring) runs them back to back with the staging aliased onto the ring.
 template <bool WITH_LINF>
@@ -191,160 +162,49 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
                   ((1024u - (static_cast<unsigned>(__cvta_generic_to_shared(smem_raw)) & 1023u)) & 1023u);
   constexpr int LD = kLD1;
   const int dc = a.kp.dc, dk = a.kp.dk, np = a.np, nbuf = ia.nbuf;
-  uint8_t* bbuf = smem;                                  // [2][7][64][128]
-  uint8_t* aring = smem + 2 * kBBufBytes;                // [kASlots][128][128]
-  const int ring_bytes = 2 * kBBufBytes + ia.n_aslots * kASlotBytes;
-  double* s_alpha = reinterpret_cast<double*>(smem + ring_bytes);   // [2][64]
+  uint8_t* ring = smem;                                  // [2 stages][7 A planes | 7 B planes]
+  double* s_alpha = reinterpret_cast<double*>(smem + kRingBytes);   // [2][64]
   double* s_mu = s_alpha + 128;                          // [2][64]
   double* s_linf = s_mu + 128;                           // [2][64]
-  double* s_red = s_linf + 128;                          // [4][64] row sums of the four TMEM lane quarters
+  double* s_red = s_linf + 128;                          // [4][64] candidate sums of the four consumer warps
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_red + 256);
-  uint64_t* bfull = bars;              // [2]
-  uint64_t* bempty = bars + 2;         // [2]
-  uint64_t* afull = bars + 4;          // [kASlots]
-  uint64_t* aempty = bars + 4 + kASlots;
-  uint64_t* tfull = bars + 4 + 2 * kASlots;     // accumulators of a j tile complete
-  uint64_t* tempty = tfull + 1;                 // ... drained by the epilogue warps
-  uint64_t* kready = tempty + 1;                // [2]
-  uint64_t* kfree = kready + 2;                 // [2]
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(kfree + 2);
-  int32_t* za = reinterpret_cast<int32_t*>(s_tmem + 2);  // [dk][LD]
+  uint64_t* full = bars;                       // [2]
+  uint64_t* kready = bars + 2;                 // [2]
+  uint64_t* kfree = kready + 2;                // [2]
+  int32_t* za = reinterpret_cast<int32_t*>(kfree + 2);   // [dk][LD]
   int32_t* zb = za + dk * LD;                            // [dk][LD]
   uint8_t* s_mask = reinterpret_cast<uint8_t*>(zb + dk * LD);  // [kMaxDc]
   // phase-1 staging: behind everything else (nbuf = 2) or aliased onto the operand ring (nbuf = 1)
-  double* stage = nbuf == 2 ? reinterpret_cast<double*>(smem + ((ring_bytes + ia.misc_bytes + 15) & ~15)) : reinterpret_cast<double*>(smem);
+  double* stage = nbuf == 2 ? reinterpret_cast<double*>(smem + ((kRingBytes + ia.misc_bytes + 15) & ~15)) : reinterpret_cast<double*>(smem);
   double* sa = stage;                                    // [dc][LD]     candidates (transposed)
   double* sb = sa + dc * LD;                             // [2][dc][LD]  trials, double buffered
 
-  // the warp index through a shuffle: provably warp-uniform, so the role branches below are uniform branches and
-  // the issuing warps keep their descriptors in uniform registers
+  // the warp index through a shuffle: provably warp-uniform, so the role branches below are uniform branches
   const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   const bool is_kwarp = warp < kKWarps;
-  const bool is_epi = warp >= kKWarps && warp < kKWarps + kEWarps;
-  const bool is_producer = warp == kKWarps + kEWarps;
-  const bool is_mma = warp == kKWarps + kEWarps + 1;
   if (tid < kMaxDc) s_mask[tid] = a.tr_mask[tid];
   if (tid == 0) {
-    for (int i = 0; i < 2; ++i) { mbar_init(bfull + i, 1); mbar_init(bempty + i, 1); }
-    for (int i = 0; i < kASlots; ++i) { mbar_init(afull + i, 1); mbar_init(aempty + i, 1); }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, kEWarps);
+    for (int i = 0; i < 2; ++i) mbar_init(full + i, 1);
     for (int i = 0; i < 2; ++i) { mbar_init(kready + i, kKWarps * 32); mbar_init(kfree + i, kEWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
-  if (is_mma) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(s_tmem)), "r"((uint32_t)kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *s_tmem;
 
   const int ntiles = (a.M + kTM - 1) / kTM;
-  const int njt = (np + kJT - 1) / kJT;
+  const int njt = np / kJT;
 
-  if (is_producer) {
-    // ================= TMA producer warp (uniform control flow, elected issue) =================
-    unsigned b_n = 0, it = 0;
-    int slot = 0;
-    unsigned aph = 0;                  // parity of the current pass over the A slots
-    const int n_aslots = ia.n_aslots;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int kb = it % nbuf;
-      VZ_I8T_DECL;
-      VZ_I8T_START(t_a);
-      mbar_wait_bounded(kready + kb, (it / nbuf) & 1);     // the tile's digit planes are complete and fenced
-      VZ_I8T_ADD(11, t_a);
-      VZ_I8T_START(t_a);
-      const int krow0 = ((int)blockIdx.x * nbuf + kb) * kDigits * kTM;
-      for (int jj = 0; jj < njt; ++jj) {
-        const int jt = njt - 1 - jj;     // descending: k chunk kc is last needed by j tile kc, so the digit scratch dies front to back
-        for (int kc = 0; kc <= jt; ++kc) {
-          const int buf = b_n & 1;
-          VZ_I8T_START(t_b);
-          mbar_wait_bounded(bempty + buf, ((b_n >> 1) & 1) ^ 1);
-          VZ_I8T_ADD(8, t_b);
-          mbar_expect_tx_elect(bfull + buf, kBBufBytes);
-          for (int s = 0; s < kDigits; ++s)
-            tma_load_2d_elect(bbuf + buf * kBBufBytes + s * kBPlaneBytes, &ia.mapK, kc * kKC, krow0 + s * kTM, bfull + buf);
-          ++b_n;
-          for (int t = 0; t < kDigits; ++t) {
-            VZ_I8T_START(t_b);
-            mbar_wait_bounded(aempty + slot, aph ^ 1);
-            VZ_I8T_ADD(9, t_b);
-            mbar_expect_tx_elect(afull + slot, kASlotBytes);
-            tma_load_3d_elect(aring + slot * kASlotBytes, &ia.mapL, kc * kKC, jt * kJT, t, afull + slot);
-            if (++slot == n_aslots) { slot = 0; aph ^= 1; }
-          }
-        }
-      }
-      VZ_I8T_ADD(10, t_a);
-    }
-  } else if (is_mma) {
-    // ================= MMA issuer warp (uniform control flow, elected issue) =================
-    unsigned b_n = 0, jt_n = 0;
-    int slot = 0;
-    unsigned aph = 0;
-    const int n_aslots = ia.n_aslots;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      VZ_I8T_DECL;
-      VZ_I8T_START(t_a);
-      for (int jj = 0; jj < njt; ++jj) {
-        const int jt = njt - 1 - jj;     // descending: k chunk kc is last needed by j tile kc, so the digit scratch dies front to back
-        VZ_I8T_START(t_b);
-        mbar_wait_bounded(tempty, (jt_n & 1) ^ 1);   // the previous j tile's accumulators have been read
-        VZ_I8T_ADD(4, t_b);
-        tc_fence_after();
-        unsigned touched = 0;
-        for (int kc = 0; kc <= jt; ++kc) {
-          const int buf = b_n & 1;
-          VZ_I8T_START(t_b);
-          mbar_wait_bounded(bfull + buf, (b_n >> 1) & 1);
-          VZ_I8T_ADD(5, t_b);
-          ++b_n;
-          const int ksteps = (np - kc * kKC) >= kKC ? 4 : (np - kc * kKC + 31) / 32;   // the last chunk may be half
-          const uint32_t bbase = smem_u32(bbuf + buf * kBBufBytes);
-          for (int t = 0; t < kDigits; ++t) {
-            VZ_I8T_START(t_b);
-            mbar_wait_bounded(afull + slot, aph);
-            VZ_I8T_ADD(6, t_b);
-            tc_fence_after();
-            const uint64_t da = umma_desc_sw128(smem_u32(aring + slot * kASlotBytes));
-            uint64_t* const slot_empty = aempty + slot;
-            if (++slot == n_aslots) { slot = 0; aph ^= 1; }
-            constexpr uint32_t idesc = umma_idesc_i8();
-            // (The A-operand collector - collector::a::fill/use/lastuse over the MMAs that share a Linv plane and
-            // k step - was tried: correct, but the MMAs then no longer overlap their operand fetches: 99 instead of
-            // 84 cycles per MMA in this loop, 92 against 83 in tools/umma_rate.cu.)
-            for (int s = 0; s + t < kGroups; ++s) {     // digit pair (s+1, t+1): group g = s + t
-              const int g = s + t;
-              const uint64_t db = umma_desc_sw128(bbase + s * kBPlaneBytes);
-              for (int kk = 0; kk < ksteps; ++kk) {
-                umma_i8(tmem + g * kTM, da + 2 * kk, db + 2 * kk, idesc, (touched >> g) & 1u);
-                touched |= 1u << g;
-              }
-            }
-            umma_commit(slot_empty);   // slot reusable once these MMAs have read it
-          }
-          umma_commit(bempty + buf);
-        }
-        umma_commit(tfull);
-        ++jt_n;
-      }
-      VZ_I8T_ADD(7, t_a);
-    }
-  } else if (is_kwarp) {
+  if (is_kwarp) {
     // ================= K* warps: phase 1 of every tile, one tile ahead of phase 2 =================
-    // 512 threads, 2 x 4 outputs each on the 64 x 64 block: rows 2 ty + i, columns (j/2) 32 + 2 tx + j%2
-    // (ty = tid / 16, tx = tid % 16)
+    // 256 threads, 2 x 4 outputs each on each half of the 64 x 64 block: rows 2 ty + i, columns (j/2) 32 + 2 tx + j%2
+    // (ty = tid / 16 + 16 p for the row halves p, tx = tid % 16)
     struct GP {
       __device__ static int row_of(int ty, int i) { return ty * 2 + i; }
       __device__ static int col_of(int tx, int j) { return (j >> 1) * 32 + tx * 2 + (j & 1); }
     };
     constexpr int kKT = kKWarps * 32;
+    constexpr int kRowSets = kTM * 16 / (2 * kKT);
     auto ksync = [&]() { asm volatile("bar.sync 1, %0;\n" ::"n"(kKT) : "memory"); };
-    const int ty = tid / 16, tx = tid % 16;
+    const int ty0 = tid / 16, tx = tid % 16;
     // the digits are written a tile ahead of their use: ask L2 to evict them last (the dead ones are discarded by the
     // epilogue warps), so that they are still resident when phase 2 streams them
     uint64_t keep_policy;
@@ -377,9 +237,11 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
         }
         if (tid < 32) cp_async16(s_alpha + buf * 64 + tid * 2, a.alpha + jb * 64 + tid * 2, true);
       };
-      double mu_part[2], lmin[2];
+      double mu_part[kRowSets][2], lmin[kRowSets][2];
 #pragma unroll
-      for (int i = 0; i < 2; ++i) { mu_part[i] = 0.0; lmin[i] = INFINITY; }
+      for (int p = 0; p < kRowSets; ++p)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) { mu_part[p][i] = 0.0; lmin[p][i] = INFINITY; }
       const int nj = np / 64;
       const bool dbl = ia.sb_bufs == 2;
       stage_trials(0, 0);
@@ -398,7 +260,9 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
           stage_rows_T_i32(a.Z, np, dk, jb * 64, 64, zb, LD, kKT);
           ksync();
         }
-        {
+#pragma unroll
+        for (int p = 0; p < kRowSets; ++p) {
+          const int ty = ty0 + p * (kKT / 16);
           constexpr int zoff = 0;
           const double* sbj = sb + buf * dc * LD + zoff;
           const double* alj = s_alpha + buf * 64 + zoff;
@@ -450,8 +314,8 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
               const int cj = zoff + GP::col_of(tx, j);
               const bool valid = (jb * 64 + cj) < a.n_valid;
               const double kv = valid ? matern52(d2[i][j], a.kp.sf2) : 0.0;
-              mu_part[i] = fma(kv, alj[GP::col_of(tx, j)], mu_part[i]);
-              if (WITH_LINF && (jb * 64 + cj) < a.tr_rows) lmin[i] = fmin(lmin[i], lf[i][j]);
+              mu_part[p][i] = fma(kv, alj[GP::col_of(tx, j)], mu_part[p][i]);
+              if (WITH_LINF && (jb * 64 + cj) < a.tr_rows) lmin[p][i] = fmin(lmin[p][i], lf[i][j]);
               q[j] = __double2ll_rn(kv * ia.kscale);    // |q| < 2^55
             }
             uint8_t* row = kd + (size_t)GP::row_of(ty, i) * np + jb * 64 + zoff;
@@ -474,117 +338,143 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
       }
       cp_async_wait<0>();
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
+      for (int p = 0; p < kRowSets; ++p)
 #pragma unroll
-        for (int o = 8; o > 0; o >>= 1) {
-          mu_part[i] += __shfl_xor_sync(0xffffffffu, mu_part[i], o);
-          if (WITH_LINF) lmin[i] = fmin(lmin[i], __shfl_xor_sync(0xffffffffu, lmin[i], o));
+        for (int i = 0; i < 2; ++i) {
+#pragma unroll
+          for (int o = 8; o > 0; o >>= 1) {
+            mu_part[p][i] += __shfl_xor_sync(0xffffffffu, mu_part[p][i], o);
+            if (WITH_LINF) lmin[p][i] = fmin(lmin[p][i], __shfl_xor_sync(0xffffffffu, lmin[p][i], o));
+          }
+          if (tx == 0) {
+            s_mu[kb * 64 + GP::row_of(ty0 + p * (kKT / 16), i)] = mu_part[p][i];
+            s_linf[kb * 64 + GP::row_of(ty0 + p * (kKT / 16), i)] = lmin[p][i];
+          }
         }
-        if (tx == 0) {
-          s_mu[kb * 64 + GP::row_of(ty, i)] = mu_part[i];
-          s_linf[kb * 64 + GP::row_of(ty, i)] = lmin[i];
-        }
-      }
       fence_proxy_async();  // generic-proxy writes (digit scratch, aliased smem) before async-proxy (TMA) accesses
       asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(kready + kb)) : "memory");
       if (tid == 0) { VZ_I8T_ADD(0, t_a); }
     }
-  } else if (is_epi) {
-    // ================= epilogue warps: TMEM -> sum_j W[i,j]^2 -> scores =================
-    // warp e reads TMEM lanes 32 (e % 4) .. +31 (Linv rows j), all 64 columns (candidates)
+  } else {
+    // ================= consumer warpgroup: operand loads, wgmma, epilogue =================
     constexpr int kET = kEWarps * 32;
     auto esync = [&]() { asm volatile("bar.sync 2, %0;\n" ::"n"(kET) : "memory"); };
     const int etid = tid - kKWarps * 32;
-    const int quarter = warp & 3, cbase = ((warp - kKWarps) >> 2) * (kEGroups * 8);   // first candidate column of this warp
+    const int ew = etid >> 5;                    // consumer warp: rows 16 ew .. 16 ew + 15 of the j tile
     int clamped = 0;
-    unsigned jt_n = 0, it = 0;
+    unsigned it = 0;
+    unsigned n_ld = 0, n_use = 0;                // chunks loaded / consumed: stage n & 1, phase parity (n >> 1) & 1
     const bool can_discard = (np % kKC) == 0;    // discard.L2 wants 128-byte aligned lines
+    int32_t acc[kGroups][16];
+#pragma unroll
+    for (int g = 0; g < kGroups; ++g)
+#pragma unroll
+      for (int i = 0; i < 16; ++i) acc[g][i] = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
       const int m0 = tile * kTM;
       const int kb = it % nbuf;
-      const uint8_t* kdt = ia.kdig + ((size_t)blockIdx.x * nbuf + kb) * kDigits * kTM * np;
+      const int krow0 = ((int)blockIdx.x * nbuf + kb) * kDigits * kTM;
+      const uint8_t* kdt = ia.kdig + (size_t)krow0 * np;
       VZ_I8T_DECL;
       VZ_I8T_START(t_a);
-      // acc[grp]: this warp's sum over its 32 Linv rows (and over the j tiles) for candidate 8 grp + c(lane),
-      // c(lane) = 4 bit4 + 2 bit3 + bit2 - the 32 x 8 -> 8 reduce-scatter below leaves it replicated on 4 lanes
-      double acc[kEGroups];
+      // Each candidate sum s_red[ew][c] is owned by one lane (c = 32 half + 8 q + 2 lane + cc, lane < 4).
+      if (lane < 4) {
 #pragma unroll
-      for (int grp = 0; grp < kEGroups; ++grp) acc[grp] = 0.0;
-      for (int jj = 0; jj < njt; ++jj) {
-        const int jt = njt - 1 - jj;     // descending: k chunk kc is last needed by j tile kc, so the digit scratch dies front to back
-        VZ_I8T_START(t_b);
-        mbar_wait_bounded(tfull, jt_n & 1);
-        if (etid == 0) { VZ_I8T_ADD(1, t_b); }
-        VZ_I8T_START(t_b);
-        ++jt_n;
-        tc_fence_after();
-        const int j = jt * kJT + quarter * 32 + lane;
-        const double sc = j < np ? __ldg(ia.lscale + j) : 0.0;
-        const uint32_t taddr = tmem + ((uint32_t)(quarter * 32) << 16) + cbase;
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int grp = 0; grp < kEGroups; ++grp) {
-          double v[8];
-#pragma unroll
-          for (int c4 = 0; c4 < 2; ++c4) {
-            int32_t G[kGroups][4];
-#pragma unroll
-            for (int g = 0; g < kGroups; ++g) tmem_ld4(taddr + g * kTM + grp * 8 + c4 * 4, G[g]);
-            tmem_ld_wait();
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              // sum_g G_g 2^(-8(g+2)) = 2^-32 (hi + lo 2^-32),  hi = G0 2^16 + G1 2^8 + G2,  lo = G3 2^24 + ... + G6
-              const long long hi = ((long long)G[0][c] << 16) + ((long long)G[1][c] << 8) + (long long)G[2][c];
-              const long long lo = ((long long)G[3][c] << 24) + ((long long)G[4][c] << 16) + ((long long)G[5][c] << 8) +
-                                   (long long)G[6][c];
-              const double w = sc * fma((double)lo, 0x1p-32, (double)hi);
-              v[c4 * 4 + c] = w * w;
-            }
+          for (int q = 0; q < 4; ++q) {
+            s_red[ew * 64 + h * kCN + 8 * q + 2 * lane] = 0.0;
+            s_red[ew * 64 + h * kCN + 8 * q + 2 * lane + 1] = 0.0;
           }
-          // reduce-scatter over the lanes (fixed order): keep the half of the values selected by the lane bit
-          {
-            const bool up = lane & 16;
+      }
+      mbar_wait_bounded(kready + kb, (it / nbuf) & 1);     // the tile's digit planes, mu and L-inf are complete
+      auto load = [&](int jt, int half, int kc) {
+        if (etid == 0) {
+          const int st = n_ld & 1;
+          uint8_t* dst = ring + st * kStageBytes;
+          mbar_expect_tx(full + st, kStageBytes);
+          for (int t = 0; t < kDigits; ++t) tma_load_3d(dst + t * kAPlaneBytes, &ia.mapL, kc * kKC, jt * kJT, t, full + st);
+          for (int s = 0; s < kDigits; ++s)
+            tma_load_2d(dst + kDigits * kAPlaneBytes + s * kBPlaneBytes, &ia.mapK, kc * kKC, krow0 + s * kTM + half * kCN, full + st);
+        }
+        __syncwarp();
+        ++n_ld;
+      };
+      // The chunks of the tile in order: j tiles descending (k chunk kc is last needed by j tile 2 kc, so the digit
+      // scratch dies front to back), the two candidate halves, k chunks 0 .. jt / 2 (Linv is lower triangular).
+      int jt = njt - 1, half = 0, kc = 0;
+      load(jt, half, kc);
+      for (;;) {
+        int jt_next = jt, half_next = half, kc_next = kc + 1;
+        if (kc_next > (jt >> 1)) {
+          kc_next = 0;
+          if (++half_next == 2) { half_next = 0; --jt_next; }
+        }
+        const bool block_done = kc_next == 0;      // the accumulators of (jt, half) are complete after this chunk
+        const bool more = jt_next >= 0;
+        const int st = n_use & 1;
+        mbar_wait_bounded(full + st, (n_use >> 1) & 1);
+        ++n_use;
+        const int ksteps = min(4, (jt * kJT + kJT - kc * kKC) / 32);   // k beyond the j tile's last row is zero
+        const uint32_t abase = smem_u32(ring + st * kStageBytes), bbase = abase + kDigits * kAPlaneBytes;
+        if (kc == 0) {                             // the epilogue of the previous block has read the accumulators
+          acc_fence(acc);
+          wgmma_fence();
+        }
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const double send = up ? v[c] : v[c + 4], keep = up ? v[c + 4] : v[c];
-              v[c] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-            }
+        for (int t = 0; t < kDigits; ++t) {
+          const uint64_t da = wgmma_desc_sw128(abase + t * kAPlaneBytes);
+#pragma unroll
+          for (int s = 0; s + t < kGroups; ++s) {     // digit pair (s+1, t+1): group g = s + t
+            const uint64_t db = wgmma_desc_sw128(bbase + s * kBPlaneBytes);
+            for (int kk = 0; kk < ksteps; ++kk)
+              wgmma_i8(acc[s + t], da + 2 * kk, db + 2 * kk, (kc > 0 || kk > 0 || t > 0) ? 1u : 0u);
           }
-          {
-            const bool up = lane & 8;
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                           // the previous chunk's wgmma are done: its stage can be refilled
+        if (more) load(jt_next, half_next, kc_next);
+        if (block_done) {
+          wgmma_wait<0>();
+          acc_fence(acc);
+          // accumulator i of this thread: Linv row 16 ew + lane / 4 + 8 ((i >> 1) & 1), candidate 8 (i >> 2) + 2 (lane % 4) + (i & 1)
+          const int j0 = jt * kJT + ew * 16 + (lane >> 2);
+          const double sc[2] = {__ldg(ia.lscale + j0), __ldg(ia.lscale + j0 + 8)};
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            double v[2];
 #pragma unroll
             for (int c = 0; c < 2; ++c) {
-              const double send = up ? v[c] : v[c + 2], keep = up ? v[c + 2] : v[c];
-              v[c] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+              v[c] = 0.0;
+#pragma unroll
+              for (int r = 0; r < 2; ++r) {
+                const int i = 4 * q + 2 * r + c;
+                // sum_g G_g 2^(-8(g+2)) = 2^-32 (hi + lo 2^-32),  hi = G0 2^16 + G1 2^8 + G2,  lo = G3 2^24 + ... + G6
+                const long long hi = ((long long)acc[0][i] << 16) + ((long long)acc[1][i] << 8) + (long long)acc[2][i];
+                const long long lo = ((long long)acc[3][i] << 24) + ((long long)acc[4][i] << 16) +
+                                     ((long long)acc[5][i] << 8) + (long long)acc[6][i];
+                const double w = sc[r] * fma((double)lo, 0x1p-32, (double)hi);
+                v[c] += w * w;
+              }
+              // sum over the 8 row lanes (fixed order)
+#pragma unroll
+              for (int o = 4; o < 32; o <<= 1) v[c] += __shfl_xor_sync(0xffffffffu, v[c], o);
+            }
+            if (lane < 4) {
+              double* red = s_red + ew * 64 + half * kCN + 8 * q + 2 * lane;
+              red[0] += v[0];
+              red[1] += v[1];
             }
           }
-          {
-            const bool up = lane & 4;
-            const double send = up ? v[0] : v[1], keep = up ? v[1] : v[0];
-            v[0] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+          if (can_discard && half == 1 && (jt & 1) == 0) {
+            // last use of k chunk jt / 2 of this tile's K* digits: drop its lines from L2 without a write-back
+            for (int i = etid; i < kDigits * kTM; i += kET)
+              asm volatile("discard.global.L2 [%0], 128;\n" ::"l"(kdt + (size_t)i * np + (size_t)(jt >> 1) * kKC) : "memory");
           }
-          v[0] += __shfl_xor_sync(0xffffffffu, v[0], 2);
-          v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
-          acc[grp] += v[0];
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(tempty)) : "memory");
-        if (can_discard) {
-          // All MMAs of j tile jt are done, and with the j tiles in descending order that was the last use of k chunk
-          // jt of this tile's K* digits: drop its lines from L2 without writing them back.  The scratch is written
-          // one tile ahead and exceeds L2 otherwise (2 x 68 MB at C2): every digit then went through HBM once, 0.7 GB
-          // out + 0.8 GB in per launch.  (Ordered before the next owner's stores by the release on kfree below.)
-          for (int i = etid; i < kDigits * kTM; i += kET)
-            asm volatile("discard.global.L2 [%0], 128;\n" ::"l"(kdt + (size_t)i * np + (size_t)jt * kKC) : "memory");
-        }
-        if (etid == 0) { VZ_I8T_ADD(2, t_b); }
+        if (!more) break;
+        jt = jt_next; half = half_next; kc = kc_next;
       }
-      if ((lane & 3) == 0) {
-        const int c = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-#pragma unroll
-        for (int grp = 0; grp < kEGroups; ++grp) s_red[quarter * 64 + cbase + grp * 8 + c] = acc[grp];
-      }
-      mbar_wait_bounded(kready + kb, (it / nbuf) & 1);     // mu / L-inf of this tile (long since complete)
       esync();
       if (etid < kTM) {
         const int r = etid, m = m0 + r;
@@ -599,9 +489,6 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
     }
     if (clamped) atomicAdd(a.clamp_count, clamped);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (is_mma) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "r"((uint32_t)kTmemCols));
 }
 
 // Linv (lower, fp64, [np x np]) -> 7 balanced base-256 digit planes relative to the row maximum, and the
@@ -631,30 +518,28 @@ __global__ void __launch_bounds__(128) k_slice_linv(const double* __restrict__ L
   if (tid == 0) lscale[j] = ldexp(1.0, ea + eb - 32);
 }
 
-// shared memory behind the operand ring: alpha, mu, L-inf, reduction, barriers, TMEM pointer, categorical rows, mask
+// shared memory behind the operand ring: alpha, mu, L-inf, reduction, barriers, categorical rows, mask
 size_t score_i8_misc_bytes(int dk) {
-  return sizeof(double) * (128 + 128 + 128 + 256) + sizeof(uint64_t) * (4 + 2 * kASlots + 2 + 4) + 16 +
-         sizeof(int32_t) * dk * 2 * kLD1 + kMaxDc;
+  return sizeof(double) * (128 + 128 + 128 + 256) + sizeof(uint64_t) * 6 + sizeof(int32_t) * dk * 2 * kLD1 + kMaxDc;
 }
 size_t score_i8_stage_bytes(int dc, int sb_bufs = 2) { return sizeof(double) * (1 + sb_bufs) * dc * kLD1; }
-size_t score_i8_smem_bytes(int dc, int dk, int nbuf, int n_aslots = kASlots, int sb_bufs = 2) {
-  return 1024 + 2 * kBBufBytes + (size_t)n_aslots * kASlotBytes + ((score_i8_misc_bytes(dk) + 15) & ~size_t(15)) +
+size_t score_i8_smem_bytes(int dc, int dk, int nbuf, int sb_bufs = 2) {
+  return 1024 + kRingBytes + ((score_i8_misc_bytes(dk) + 15) & ~size_t(15)) +
          (nbuf == 2 ? score_i8_stage_bytes(dc, sb_bufs) : 0);
 }
 // Shared-memory plan: overlap the phases (nbuf = 2) whenever the phase-1 staging fits next to the operand ring, giving
-// up Linv slots and the second trial buffer for large Dc; otherwise back to back with the staging aliased onto the ring.
-struct I8Plan { int nbuf, n_aslots, sb_bufs; };
+// up the second trial buffer for larger Dc; otherwise back to back with the staging aliased onto the ring.
+struct I8Plan { int nbuf, sb_bufs; };
 I8Plan score_i8_plan(int dc, int dk) {
-  const int tries[4][2] = {{4, 2}, {3, 2}, {3, 1}, {2, 1}};
-  for (const auto& t : tries)
-    if (score_i8_smem_bytes(dc, dk, 2, t[0], t[1]) <= 227 * 1024) return {2, t[0], t[1]};
-  return {1, kASlots, 2};
+  for (int sb_bufs = 2; sb_bufs >= 1; --sb_bufs)
+    if (score_i8_smem_bytes(dc, dk, 2, sb_bufs) <= 227 * 1024) return {2, sb_bufs};
+  return {1, 2};
 }
 
 }  // namespace
 
 bool score_i8_eligible(const vzgp_handle* h, int M) {
-  if (h->kp.use_linear || h->np < kJT || h->np > 4096 || h->dc < 1) return false;
+  if (h->kp.use_linear || h->np < kKC || h->np > 4096 || h->dc < 1) return false;
   if (score_i8_stage_bytes(h->dc) > (size_t)kRingBytes) return false;
   const int ntiles = (M + kTM - 1) / kTM;
   return ntiles >= h->sm_count;          // enough tiles for one CTA per SM (no column split on this path)
@@ -677,10 +562,6 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
   const I8Plan plan = score_i8_plan(h->dc, h->dk);
   const int nbuf = plan.nbuf;
   VZ_TRY(h->i8_kdig.reserve((size_t)grid * nbuf * kDigits * kTM * np));
-  // (A persisting L2 access-policy window over the digit scratch, as k_score uses for its fp64 scratch, changes
-  // nothing here: the two buffers are 136 MB at C2 against 126 MB of L2, the freshly written tile is the LRU victim
-  // while the current one is re-read, so every digit goes through HBM once - 0.7 GB written + 0.8 GB read per launch,
-  // 9 % of the HBM bandwidth, ncu: profiles/score_i8_kernel_ncu_r02.json.)
   I8Args ia;
   memset(&ia, 0, sizeof(ia));
   ScoreArgs& a = ia.s;
@@ -705,13 +586,12 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
   ia.lscale = h->i8_scale.as<double>();
   ia.kscale = ldexp(1.0, 56 - ea);
   ia.nbuf = nbuf;
-  ia.n_aslots = plan.n_aslots;
   ia.sb_bufs = plan.sb_bufs;
   ia.misc_bytes = (int)score_i8_misc_bytes(h->dk);
   {
     const uint64_t dims[2] = {(uint64_t)np, (uint64_t)grid * nbuf * kDigits * kTM};
     const uint64_t strides[1] = {(uint64_t)np};
-    const uint32_t box[2] = {(uint32_t)kKC, (uint32_t)kTM};
+    const uint32_t box[2] = {(uint32_t)kKC, (uint32_t)kCN};
     // 128-byte L2 promotion: a 256-byte one would pull the neighbouring k chunk's (already discarded) line back in
     VZ_TRY(make_tensor_map_u8(&ia.mapK, ia.kdig, 2, dims, strides, box, false));
   }
@@ -722,13 +602,13 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
     VZ_TRY(make_tensor_map_u8(&ia.mapL, h->i8_planes.as<uint8_t>(), 3, dims, strides, box));
   }
   const bool need_linf = (linf != nullptr) || (a.apply_tr && a.radius <= 0.5);
-  const size_t sm = score_i8_smem_bytes(h->dc, h->dk, nbuf, plan.n_aslots, plan.sb_bufs);
+  const size_t sm = score_i8_smem_bytes(h->dc, h->dk, nbuf, plan.sb_bufs);
   if (sm > 227 * 1024) { set_error("k_score_i8 needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
   if (need_linf) {
-    VZ_CUDA(cudaFuncSetAttribute(k_score_i8<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    VZ_TRY(raise_dyn_smem((const void*)k_score_i8<true>, sm));
     k_score_i8<true><<<grid, kI8Threads, sm, h->stream>>>(ia);
   } else {
-    VZ_CUDA(cudaFuncSetAttribute(k_score_i8<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    VZ_TRY(raise_dyn_smem((const void*)k_score_i8<false>, sm));
     k_score_i8<false><<<grid, kI8Threads, sm, h->stream>>>(ia);
   }
   VZ_CHECK_LAUNCH();
@@ -740,10 +620,8 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
 }  // namespace vzgp
 
 #ifdef VZ_I8_TIMING
-// Debug builds only (make EXTRA=-DVZ_I8_TIMING): clock64 sums of CTA 0.  [0] phase 1, [1] epilogue waiting for the
-// accumulators, [2] epilogue, [3] whole tile (worker), [4] MMA thread waiting for the epilogue, [5] ... for K* planes,
-// [6] ... for Linv planes, [7] MMA thread total, [8] / [9] producer waiting for a free B buffer / A slot, [10] producer
-// total, [15] tiles.  reset != 0 clears the counters.
+// Debug builds only (make EXTRA=-DVZ_I8_TIMING): clock64 sums of CTA 0.  [0] phase 1, [3] whole tile (consumer),
+// [12] K* warps waiting for a free digit buffer, [15] tiles.  reset != 0 clears the counters.
 extern "C" int vzgp_debug_i8_timing(long long* out, int reset) {
   if (cudaMemcpyFromSymbol(out, vzgp::g_i8_t, sizeof(long long) * 16) != cudaSuccess) return -2;
   if (reset) {

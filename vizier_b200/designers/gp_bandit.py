@@ -1,4 +1,4 @@
-"""`VizierGPBandit`: the GP-UCB designer, with the GP stack running in libvzgp (CUDA, sm_100a).
+"""`VizierGPBandit`: the GP-UCB designer, with the GP stack running in libvzgp (CUDA, sm_90a).
 
 Drop-in for vizier/_src/algorithms/designers/gp_bandit.py:88-641 on the single-metric default
 path: same constructor keywords, `update` / `suggest` / `predict` / `sample` / `from_problem`,
