@@ -1,4 +1,5 @@
-"""clock64 breakdown of k_score_i8 (CTA 0) - needs the library built with `make EXTRA=-DVZ_I8_TIMING`."""
+"""clock64 breakdown of k_score_i8 (CTA 0) - needs the instrumented library (`make -C vizier_b200/csrc timing`,
+then VZGP_LIB=vizier_b200/_lib/libvzgp_timing.so)."""
 import ctypes as C
 import json
 import sys

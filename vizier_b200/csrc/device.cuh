@@ -214,4 +214,14 @@ __device__ __forceinline__ void dmma_8x8x4(double& d0, double& d1, double a, dou
                : "d"(a), "d"(b));
 }
 
+// D[16x8] += A[16x8] B[8x8] (mma.sync m16n8k8 f64, sm_90).  Lane (g = lane/4, t = lane%4): a0 = A[g][t],
+// a1 = A[g+8][t], a2 = A[g][t+4], a3 = A[g+8][t+4]; b0 = B[t][g], b1 = B[t+4][g]; d0, d1 = D[g][2t, 2t+1],
+// d2, d3 = D[g+8][2t, 2t+1].
+__device__ __forceinline__ void dmma_16x8x8(double& d0, double& d1, double& d2, double& d3, double a0, double a1, double a2,
+                                            double a3, double b0, double b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+               : "+d"(d0), "+d"(d1), "+d"(d2), "+d"(d3)
+               : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
+}
+
 }  // namespace vzgp

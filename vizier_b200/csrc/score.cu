@@ -12,16 +12,20 @@
 //   phase 1  K* tile [64 x np] = Matern(x*, X) built 64 columns at a time from shared-memory
 //            staged rows; mu = K* alpha and the L-inf trust-region distance are reduced on the
 //            fly; the tile goes to a CTA-private scratch (L2 resident, never re-read by others).
-//   phase 2  W = K* . Linv^T in 64 x 128 blocks on the FP64 tensor pipe (mma.sync m8n8k4 f64;
-//            the only fp64 tensor-core instruction), operands streamed by a TMA producer warp (cp.async.bulk.tensor,
-//            128-byte swizzle) through a 4-stage ring with full/empty mbarriers, exploiting that
-//            Linv is lower triangular (k <= j, all-zero fragments skipped); each block is squared
-//            and row-summed in registers, W is never stored.
+//   phase 2  W = K* . Linv^T in 64 x 128 blocks on the FP64 tensor pipe (mma.sync m16n8k8 f64: on the
+//            H100 the m8n8k4 shape issues at half the rate), operands streamed by a TMA producer warp
+//            (cp.async.bulk.tensor, 128-byte swizzle) through a 4-stage ring with full/empty mbarriers,
+//            exploiting that Linv is lower triangular (k <= j, all-zero fragments skipped); each block
+//            is squared and row-summed in registers, W is never stored.  Large pools run in 2-CTA
+//            clusters that multicast each Linv box to both CTAs.
 //   epilogue var = sf2 + sn2 - sum W^2 (clamped at 0), sigma, UCB, trust region, outputs.
 #include <cuda.h>
 
 #include <climits>
 #include <cstring>
+#include <map>
+#include <mutex>
+#include <tuple>
 
 #include "launchers.h"
 #include "score_small.cuh"
@@ -45,6 +49,23 @@ constexpr int kAHalf = kTM * 16;                 // doubles
 constexpr int kBHalf = kBN * 16;
 constexpr int kStageDoubles = 2 * (kAHalf + kBHalf);   // 6144 doubles = 48 KB
 constexpr unsigned kStageBytes = kStageDoubles * sizeof(double);
+// Large pools run in clusters of kCluster CTAs on adjacent tiles.  They walk the same slab sequence, so
+// every Linv box is loaded from L2 once per cluster: the B operand of a stage is split into kBPieces
+// boxes of kBPieceRows rows, and each CTA multicasts its share into the same stage of all of them.
+constexpr int kCluster = 2;
+constexpr int kBPieces = kCluster < 2 ? 2 : kCluster;
+constexpr int kBPieceRows = 2 * kBN / kBPieces;
+static_assert(kBPieces % 2 == 0 && kBN % (kBPieces / 2) == 0, "B pieces tile the two halves of a stage");
+
+#ifdef VZ_SCORE_TIMING
+// Instrumented build only (make timing): clock64 sums over all CTAs, read by vzgp_debug_score_timing.
+// [0] tiles  [1] phase 1  [2] phase 2  [3] tile gate (barrier after phase 1)  [4] whole tile   (math warp 0)
+// [5] math warps waiting on full barriers (summed over the 16 warps)  [6] producer waiting on empty barriers
+__device__ unsigned long long g_score_t[8];
+#define VZ_ST(...) __VA_ARGS__
+#else
+#define VZ_ST(...)
+#endif
 
 template <bool WITH_LINF>
 __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constant__ ScoreArgs a) {
@@ -66,7 +87,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   double* s_linf = s_mu + 64;                            // [64]
   double* s_rowsq = s_linf + 64;                         // [4][64]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_rowsq + 256);  // [kStages] TMA bytes landed
-  uint64_t* empty_bar = full_bar + kStages;                         // [kStages] all 16 math warps released the stage
+  uint64_t* empty_bar = full_bar + kStages;                         // [kStages] all 16 math warps of every CTA in the cluster released the stage
   int32_t* za = reinterpret_cast<int32_t*>(full_bar + 8);  // [dk][LD]
   int32_t* zb = za + dk * LD;                            // [dk][LD]
   uint8_t* s_mask = reinterpret_cast<uint8_t*>(zb + dk * LD);  // [kMaxDc]
@@ -75,17 +96,30 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   const int ty = tid / 16, tx = tid % 16;      // phase-1 mapping (32 x 16 threads)
   const int wm = warp & 3, wn = warp >> 2;     // phase-2 warp grid 4 (M) x 4 (N)
   const int fr = lane >> 2, fk = lane & 3;     // fragment row / k within a DMMA tile
+  // Tile row (A: candidate, B: output column) that fragment row fr stands for within its 8-row group.
+  // An LDS.128 is served 8 lanes at a time; lanes 0-7 are fragment rows 0 and 1.  With the 128-byte
+  // swizzle rows r and r^1 keep their chunks in the same 64-byte half, a 2-way bank conflict on every
+  // operand load; rows r and r^4 land in opposite halves.  So fr = 2i, 2i+1 read rows i, i+4.  Row sums
+  // do not care which row a fragment row holds (the k mapping, which A and B must share, is unchanged).
+  const int pr = ((fr & 1) << 2) | (fr >> 1);
   double* scr = a.scratch + (size_t)blockIdx.x * kTM * np;
+  // Cluster of ncta CTAs (1 for medium pools, which split a tile's blocks between CTAs, else kCluster).
+  // The peers write into this CTA's ring and arrive on its empty barriers, so every gate that keeps the
+  // ring or the barriers untouched is cluster-wide when ncta > 1.
+  const unsigned crank = cluster_ctarank(), ncta = cluster_nctarank();
+  auto tile_gate = [&]() { if (ncta > 1) cluster_sync(); else __syncthreads(); };
   if (tid < kMaxDc) s_mask[tid] = a.tr_mask[tid];
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(full_bar + s, 1); mbar_init(empty_bar + s, kThreads / 32); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(full_bar + s, 1); mbar_init(empty_bar + s, ncta * (kThreads / 32)); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
-  __syncthreads();
+  tile_gate();   // barriers initialised in every CTA before any peer multicasts or arrives
   int clamped = 0;
   unsigned slab_n = 0;   // slabs issued (producer) / consumed (math warps) since kernel start: ring position and phase
   const bool is_producer = warp == kThreads / 32;
   auto consumer_sync = [&]() { asm volatile("bar.sync 1, %0;\n" ::"n"(kThreads) : "memory"); };
+  // Counters: sums over the tiles that hold candidates (the all-padding tile of a last round is left out).
+  VZ_ST(long long t_p1 = 0, t_gate = 0, t_p2 = 0, t_tile = 0, t_wait = 0, w_tile = 0, n_tiles = 0;)
 
   const int ntiles = (a.M + kTM - 1) / kTM;
   const int nblocks = (np + kBN - 1) / kBN;
@@ -93,7 +127,11 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   const double* XTs = a.XT;
   const double* XTu = a.XT + (size_t)dc * np;
 
-  for (int work = blockIdx.x; work < ntiles * nsplit; work += gridDim.x) {
+  // The CTAs of a cluster take adjacent work items and run the same number of rounds.  In the last
+  // round a CTA can be left without a tile (work >= ntiles, nsplit == 1): it scores an all-padding tile
+  // (m0 >= M, nothing emitted) so that its Linv pieces and stage releases still reach its peers.
+  for (int w0 = blockIdx.x - crank; w0 < ntiles * nsplit; w0 += gridDim.x) {
+    const int work = w0 + crank;
     const int tile = work / nsplit, split = work - tile * nsplit;
     const int m0 = tile * kTM;
     // Work split of this tile's phase 2 (identical for producer and consumers).
@@ -102,28 +140,39 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     auto slabs_in = [&](int jb) { int kend = (jb + 1) * kBN; if (kend > np) kend = np; return kend / kBK; };
     if (is_producer) {
       // ---- TMA producer warp: waits for phase 1 of this tile, then streams every slab of the
-      // tile through the ring, gated only by the per-stage empty barriers.
-      __syncthreads();
+      // tile through the ring, gated only by the per-stage empty barriers.  The gate also waits for
+      // phase 1 of the peers: their phase-1 staging aliases the ring this producer multicasts into.
+      tile_gate();
+      VZ_ST(w_tile = 0;)
       if (lane == 0) {
+        const uint16_t cmask = (uint16_t)((1u << ncta) - 1u);
         for (int q = 0; q < nq; ++q) {
           const int jb = block_of(q), nsl = slabs_in(jb);
           for (int ks = 0; ks < nsl; ++ks) {
             const int stage = slab_n % kStages;
+            VZ_ST(const long long t0 = clock64();)
             mbar_wait(empty_bar + stage, ((slab_n / kStages) & 1) ^ 1);
+            VZ_ST(w_tile += clock64() - t0;)
             double* base = ring + stage * kStageDoubles;
             const int k0 = ks * kBK;
-            mbar_expect_tx(full_bar + stage, kStageBytes);
+            mbar_expect_tx(full_bar + stage, kStageBytes);   // own A boxes + the B pieces of every CTA
             tma_load_2d(base, &a.mapA, k0, (int)blockIdx.x * kTM, full_bar + stage);
             tma_load_2d(base + kAHalf, &a.mapA, k0 + 16, (int)blockIdx.x * kTM, full_bar + stage);
-            tma_load_2d(base + 2 * kAHalf, &a.mapB, k0, jb * kBN, full_bar + stage);          // rows >= np: zero fill
-            tma_load_2d(base + 2 * kAHalf + kBHalf, &a.mapB, k0 + 16, jb * kBN, full_bar + stage);
+            for (int p = (int)crank; p < kBPieces; p += (int)ncta) {   // rows >= np: zero fill
+              const int half = p / (kBPieces / 2), r0 = (p % (kBPieces / 2)) * kBPieceRows;
+              double* dst = base + 2 * kAHalf + half * kBHalf + r0 * 16;
+              if (ncta > 1) tma_load_2d_multicast(dst, &a.mapB, k0 + 16 * half, jb * kBN + r0, full_bar + stage, cmask);
+              else tma_load_2d(dst, &a.mapB, k0 + 16 * half, jb * kBN + r0, full_bar + stage);
+            }
             ++slab_n;
           }
         }
       }
       __syncwarp();
+      VZ_ST(if (m0 < a.M) t_wait += w_tile;)
       continue;
     }
+    VZ_ST(const long long t_tile0 = clock64(); w_tile = 0;)
     consumer_sync();  // previous tile fully consumed by the math warps (sa, s_mu, s_rowsq, ring)
     // candidate tile, transposed; scaled by 1/ls like the reference's FeatureScaled kernel
     for (int e = tid; e < kTM * dc; e += kThreads) {
@@ -235,7 +284,9 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       }
     }
     fence_proxy_async();  // generic-proxy writes (scratch tile, aliased smem) before async-proxy (TMA) accesses
-    __syncthreads();      // this CTA's scratch tile is complete and visible
+    VZ_ST(const long long t1 = clock64();)
+    tile_gate();          // this CTA's scratch tile is complete and visible; the peers are done with their staging
+    VZ_ST(const long long t2 = clock64();)
 
     // ---------------- phase 2: row sums of (K* Linv^T)^2 on the DMMA pipe ----------------
     // Slab (jb, ks): A = scratch[0:64, ks*16 : +16], B = Linv[jb*128 : +128, ks*16 : +16];
@@ -254,14 +305,17 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       const int col_base = jb * kBN + wn * 32;   // first output column of this warp
       for (int ks = 0; ks < nsl; ++ks) {
         const int stage = slab_n % kStages;
+        VZ_ST(const long long tw = clock64();)
         mbar_wait(full_bar + stage, (slab_n / kStages) & 1);   // TMA bytes of this slab have landed
+        VZ_ST(w_tile += clock64() - tw;)
         ++slab_n;
         // Fragment loads are 16 bytes: lane (fr, fk) takes k = 8h + 2fk and 8h + 2fk + 1 of each
-        // 8-wide k group h, i.e. the operands of two DMMA k-steps (the k order inside a slab is
-        // irrelevant as long as A and B agree).  Row r = ... + fr, so the swizzle XOR is fr.
+        // 8-wide k group h as the k slots fk and fk + 4 of one m16n8k8 (rows fr and fr + 8 of A come
+        // from a0 and a1; the k order inside a slab is irrelevant as long as A and B agree).
+        // Fragment row fr reads tile row ... + pr, so the swizzle XOR is pr.
         const double* stg = ring + stage * kStageDoubles;
-        const double* Arow0 = stg + (wm * 16 + fr) * 16;            // + half*kAHalf + chunk*2
-        const double* Brow0 = stg + 2 * kAHalf + (wn * 32 + fr) * 16;
+        const double* Arow0 = stg + (wm * 16 + pr) * 16;            // + half*kAHalf + chunk*2
+        const double* Brow0 = stg + 2 * kAHalf + (wn * 32 + pr) * 16;
         const int k0 = ks * kBK;
         // Linv[c, k] = 0 for k > c.  k0 and col_base are multiples of 32: slabs right of this
         // warp's 32 columns contribute nothing; in the diagonal slab (k0 == col_base) the k group
@@ -269,42 +323,32 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
         if (k0 < col_base) {
 #pragma unroll
           for (int h = 0; h < 4; ++h) {
-            const int co = ((((h & 1) * 4 + fk) ^ fr) * 2);   // swizzled 16-byte chunk, in doubles
+            const int co = ((((h & 1) * 4 + fk) ^ pr) * 2);   // swizzled 16-byte chunk, in doubles
             const double2 a0 = *reinterpret_cast<const double2*>(Arow0 + (h >> 1) * kAHalf + co);
             const double2 a1 = *reinterpret_cast<const double2*>(Arow0 + (h >> 1) * kAHalf + 8 * 16 + co);
             double2 b[4];
 #pragma unroll
             for (int g = 0; g < 4; ++g) b[g] = *reinterpret_cast<const double2*>(Brow0 + (h >> 1) * kBHalf + g * 8 * 16 + co);
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              dmma_8x8x4(acc[0][g][0], acc[0][g][1], a0.x, b[g].x);
-              dmma_8x8x4(acc[1][g][0], acc[1][g][1], a1.x, b[g].x);
-            }
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              dmma_8x8x4(acc[0][g][0], acc[0][g][1], a0.y, b[g].y);
-              dmma_8x8x4(acc[1][g][0], acc[1][g][1], a1.y, b[g].y);
-            }
+            for (int g = 0; g < 4; ++g)
+              dmma_16x8x8(acc[0][g][0], acc[0][g][1], acc[1][g][0], acc[1][g][1], a0.x, a1.x, a0.y, a1.y, b[g].x, b[g].y);
           }
         } else if (k0 == col_base) {
 #pragma unroll
           for (int h = 0; h < 4; ++h) {
-            const int co = ((((h & 1) * 4 + fk) ^ fr) * 2);
+            const int co = ((((h & 1) * 4 + fk) ^ pr) * 2);
             const double2 a0 = *reinterpret_cast<const double2*>(Arow0 + (h >> 1) * kAHalf + co);
             const double2 a1 = *reinterpret_cast<const double2*>(Arow0 + (h >> 1) * kAHalf + 8 * 16 + co);
 #pragma unroll
             for (int g = 0; g < 4; ++g) {
               if (g < h) continue;  // compile-time: columns of fragment g lie left of k group h
               const double2 bg = *reinterpret_cast<const double2*>(Brow0 + (h >> 1) * kBHalf + g * 8 * 16 + co);
-              dmma_8x8x4(acc[0][g][0], acc[0][g][1], a0.x, bg.x);
-              dmma_8x8x4(acc[1][g][0], acc[1][g][1], a1.x, bg.x);
-              dmma_8x8x4(acc[0][g][0], acc[0][g][1], a0.y, bg.y);
-              dmma_8x8x4(acc[1][g][0], acc[1][g][1], a1.y, bg.y);
+              dmma_16x8x8(acc[0][g][0], acc[0][g][1], acc[1][g][0], acc[1][g][1], a0.x, a1.x, a0.y, a1.y, bg.x, bg.y);
             }
           }
         }
         __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(empty_bar + stage)) : "memory");
+        if ((unsigned)lane < ncta) mbar_arrive_cluster(empty_bar + stage, lane);   // the stage of every CTA it was multicast into
       }
 #pragma unroll
       for (int f = 0; f < 2; ++f)
@@ -314,13 +358,14 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
           rowsq[f] = fma(acc[f][g][1], acc[f][g][1], rowsq[f]);
         }
     }
+    VZ_ST(const long long t3 = clock64();)
     cp_async_wait<0>();
     // combine the 4 lanes that share a fragment row, then the four N-warps through smem
 #pragma unroll
     for (int f = 0; f < 2; ++f) {
       rowsq[f] += __shfl_xor_sync(0xffffffffu, rowsq[f], 1);
       rowsq[f] += __shfl_xor_sync(0xffffffffu, rowsq[f], 2);
-      if (fk == 0) s_rowsq[wn * 64 + wm * 16 + f * 8 + fr] = rowsq[f];
+      if (fk == 0) s_rowsq[wn * 64 + wm * 16 + f * 8 + pr] = rowsq[f];
     }
     consumer_sync();
     // ---------------- epilogue ----------------
@@ -339,8 +384,26 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
         }
       }
     }
+    VZ_ST(if (m0 < a.M) { t_p1 += t1 - t_tile0; t_gate += t2 - t1; t_p2 += t3 - t2; t_tile += clock64() - t_tile0; t_wait += w_tile; ++n_tiles; })
   }
   if (clamped) atomicAdd(a.clamp_count, clamped);
+#ifdef VZ_SCORE_TIMING
+  if (lane == 0) {
+    if (is_producer) {
+      atomicAdd(&g_score_t[6], (unsigned long long)t_wait);
+    } else {
+      atomicAdd(&g_score_t[5], (unsigned long long)t_wait);
+      if (warp == 0) {
+        atomicAdd(&g_score_t[0], (unsigned long long)n_tiles);
+        atomicAdd(&g_score_t[1], (unsigned long long)t_p1);
+        atomicAdd(&g_score_t[2], (unsigned long long)t_p2);
+        atomicAdd(&g_score_t[3], (unsigned long long)t_gate);
+        atomicAdd(&g_score_t[4], (unsigned long long)t_tile);
+      }
+    }
+  }
+#endif
+  if (ncta > 1) cluster_sync();   // no CTA exits while a peer can still multicast into it or arrive on its barriers
 }
 
 // nsplit > 1: sums the partial row sums in a fixed order and emits the scores.
@@ -470,6 +533,25 @@ static int ensure_scratch(vzgp_handle* h, size_t scratch_bytes) {
     }
     h->scratch_window = h->scratch.ptr;
   }
+  return 0;
+}
+
+// Clusters of cfg's shape that fit on the device at once (the GPCs decide it: not every SM count
+// divides into clusters).  Cached per device, kernel and shared-memory size.
+static int max_active_clusters(const void* kfn, const cudaLaunchConfig_t& cfg, int* out) {
+  static std::mutex mu;
+  static std::map<std::tuple<int, const void*, size_t>, int> cache;
+  int dev = 0;
+  VZ_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  int& n = cache[{dev, kfn, cfg.dynamicSmemBytes}];
+  if (n == 0) {
+    cudaLaunchConfig_t c = cfg;
+    c.gridDim = dim3(cfg.attrs[0].val.clusterDim.x);
+    VZ_CUDA(cudaOccupancyMaxActiveClusters(&n, kfn, &c));
+    if (n <= 0) { set_error("no cluster of the score kernel fits on device %d", dev); return VZGP_ERR_CUDA; }
+  }
+  *out = n;
   return 0;
 }
 
@@ -667,33 +749,43 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
     if (want && score_i8_eligible(h, M)) return launch_score_i8(h, Xs, Zs, M, acq, score, mu, sigma, linf);
   }
   // Medium pools cannot fill the GPU with one CTA per tile: share each tile's output column
-  // blocks between nsplit CTAs (each recomputes the cheap K* tile).
+  // blocks between nsplit CTAs (each recomputes the cheap K* tile).  Their CTAs walk different
+  // block sequences, so they run as clusters of one; large pools run as clusters of kCluster.
   int nsplit = 1;
   if (ntiles * 2 <= h->sm_count && nblocks >= 2) nsplit = (nblocks + 1) / 2;
   const int nwork = ntiles * nsplit;
-  const int grid = nwork < h->sm_count ? nwork : h->sm_count;
-  VZ_TRY(ensure_scratch(h, (size_t)grid * kTM * h->np * sizeof(double)));
-  fill_score_args(h, Xs, Zs, M, acq, score, mu, sigma, linf, &a);
-  VZ_TRY(make_map(&a.mapA, a.scratch, (uint64_t)grid * kTM, (uint64_t)h->np, (uint64_t)h->np, kTM));
-  VZ_TRY(make_map(&a.mapB, a.Linv, (uint64_t)h->np, (uint64_t)h->np, (uint64_t)h->np, kBN));
-  a.nsplit = nsplit;
-  if (nsplit > 1) {
-    VZ_TRY(h->Tws.reserve(sizeof(double) * (size_t)(nsplit + 2) * a.mpad));
-    a.part = h->Tws.as<double>();
-  }
-  const bool need_linf = (linf != nullptr) || (a.apply_tr && a.radius <= 0.5);
+  const int csize = nsplit == 1 ? kCluster : 1;
+  const bool need_linf = (linf != nullptr) || (acq->use_trust_region && acq->trust_radius <= 0.5);
   const size_t sm = score_smem_bytes(h->dc, h->dk, need_linf);
   if (sm > 227 * 1024) {
     set_error("score kernel needs %zu bytes of shared memory (Dc=%d with trust-region distance)", sm, h->dc);
     return VZGP_ERR_UNSUPPORTED;
   }
-  if (need_linf) {
-    VZ_TRY(raise_dyn_smem((const void*)k_score<true>, sm));
-    k_score<true><<<grid, kBlockThreads, sm, h->stream>>>(a);
-  } else {
-    VZ_TRY(raise_dyn_smem((const void*)k_score<false>, sm));
-    k_score<false><<<grid, kBlockThreads, sm, h->stream>>>(a);
+  const void* kfn = need_linf ? (const void*)k_score<true> : (const void*)k_score<false>;
+  VZ_TRY(raise_dyn_smem(kfn, sm));
+  cudaLaunchAttribute cattr[1];
+  cattr[0].id = cudaLaunchAttributeClusterDimension;
+  cattr[0].val.clusterDim.x = csize; cattr[0].val.clusterDim.y = 1; cattr[0].val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.blockDim = dim3(kBlockThreads); cfg.dynamicSmemBytes = sm; cfg.stream = h->stream;
+  cfg.attrs = cattr; cfg.numAttrs = 1;
+  // Persistent grid: as many clusters as can be co-resident, at most one per csize work items.
+  int slots = h->sm_count;
+  if (csize > 1) VZ_TRY(max_active_clusters(kfn, cfg, &slots));
+  const int want = (nwork + csize - 1) / csize;
+  const int grid = (want < slots ? want : slots) * csize;
+  cfg.gridDim = dim3(grid);
+  VZ_TRY(ensure_scratch(h, (size_t)grid * kTM * h->np * sizeof(double)));
+  fill_score_args(h, Xs, Zs, M, acq, score, mu, sigma, linf, &a);
+  VZ_TRY(make_map(&a.mapA, a.scratch, (uint64_t)grid * kTM, (uint64_t)h->np, (uint64_t)h->np, kTM));
+  VZ_TRY(make_map(&a.mapB, a.Linv, (uint64_t)h->np, (uint64_t)h->np, (uint64_t)h->np, kBPieceRows));
+  a.nsplit = nsplit;
+  if (nsplit > 1) {
+    VZ_TRY(h->Tws.reserve(sizeof(double) * (size_t)(nsplit + 2) * a.mpad));
+    a.part = h->Tws.as<double>();
   }
+  void* kargs[] = {&a};
+  VZ_CUDA(cudaLaunchKernelExC(&cfg, kfn, kargs));
   VZ_CHECK_LAUNCH();
   h->launches++;
   if (nsplit > 1) {
@@ -1105,3 +1197,15 @@ int launch_merge_topk(vzgp_handle* h, const double* rows, int n_rows, int width,
 
 
 }  // namespace vzgp
+
+#ifdef VZ_SCORE_TIMING
+// Instrumented build only: the k_score counters (slots listed at g_score_t).  reset != 0 clears them.
+extern "C" int vzgp_debug_score_timing(unsigned long long* out, int reset) {
+  if (cudaMemcpyFromSymbol(out, vzgp::g_score_t, sizeof(vzgp::g_score_t)) != cudaSuccess) return -2;
+  if (reset) {
+    unsigned long long z[8] = {};
+    if (cudaMemcpyToSymbol(vzgp::g_score_t, z, sizeof(z)) != cudaSuccess) return -2;
+  }
+  return 0;
+}
+#endif
