@@ -112,9 +112,26 @@ int64_t vzgp_launch_count(const vzgp_handle* h);
  * callers that run several handles concurrently, like the ARD restarts, give each an equal share).
  * "score_i8": 1 = large candidate pools (>= one 64-candidate tile per SM, 128 <= padded N <= 4096, no linear
  * kernel) are scored by the wgmma integer-split kernel, 0 = always the FP64 DMMA kernel, -1 = the process
- * default (environment VZGP_SCORE_I8, default 0). */
+ * default (environment VZGP_SCORE_I8, default 0).
+ * "small_tiles": pools of at most this many 64-candidate tiles take the small-pool kernels (0 = never), -1 = the
+ * process default (environment VZGP_SMALL_TILES, default 8). */
 int vzgp_set_int(vzgp_handle* h, const char* key, int value);
-/* Counters.  "launches" (= vzgp_launch_count), "score_i8_launches": launches of the integer-split scoring kernel. */
+
+/* Route the last scoring call on a handle took (vzgp_get_int key "score_route"; -1 before the first one).
+ * Every scoring entry point - vzgp_score, the host and top-k variants, GP-UCB-PE, ensemble, stack and
+ * multi-metric - records it on each handle it scores with. */
+typedef enum vzgp_score_route {
+  VZGP_ROUTE_SMALL = 0,    /* <= small_tiles tiles: k_cross_small, k_var_small, k_small_finalize */
+  VZGP_ROUTE_SPLIT = 1,    /* 2 * tiles <= SMs: k_score, score_nsplit CTAs per tile, then k_score_finalize */
+  VZGP_ROUTE_CLUSTER = 2,  /* every other pool: k_score in 2-CTA clusters */
+  VZGP_ROUTE_I8 = 3,       /* "score_i8" on and eligible: k_score_i8 */
+  VZGP_ROUTE_GENERAL = 4   /* linear_coef models: explicit K* and W, k_general_finalize */
+} vzgp_score_route;
+
+/* Counters.  "launches" (= vzgp_launch_count), "score_i8_launches": launches of the integer-split scoring kernel.
+ * "sm_count": multiprocessors of the handle's device.  Of the last scoring call: "score_route" (vzgp_score_route),
+ * "score_nsplit" (CTAs per 64-candidate tile: > 1 on the split route only, 1 on the cluster and i8 routes, 0
+ * otherwise), "score_grid" (CTAs of the k_score / k_score_i8 launch, 0 on the other routes). */
 int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value);
 
 /* ---- stage-wise entry points (parity tests call these one by one) -------- */

@@ -1,6 +1,6 @@
 """The dataflow factorisation (csrc/dataflow.cu) through its stage-wise entry point: L, L^-1 and the lower
 triangle of A^-1 against LAPACK (NumPy / SciPy) from two 64-blocks up to BASELINE C4's size (np = 2048:
-1549 tile tasks on 296 resident CTAs - more tasks than slots), alone and with several factorisations
+1549 tile tasks on 2 * SMs - 8 worker CTAs, 256 on a 132-SM H100 - more tasks than slots), alone and with several factorisations
 running concurrently on different handles / streams (partial residency of every kernel)."""
 import threading
 

@@ -580,21 +580,28 @@ def test_score_topk_pack_and_device_merge(dev):
 
 @pytest.mark.parametrize('n,d,m', [(1, 1, 1), (2, 3, 63), (64, 2, 65), (65, 7, 129), (127, 64, 40), (129, 33, 200)])
 def test_score_edge_shapes(dev, n, d, m):
-  """Ragged sizes around the 64-row tiles / 128-column blocks, D=1 and the D=64 maximum."""
+  """Ragged sizes around the 64-row tiles / 128-column blocks, D=1 and the D=64 maximum.  These pools have at
+  most 4 tiles: by default they take the small-pool kernels; with "small_tiles" = 0 the same pool runs k_score."""
   x, y, _ = _problem(n, d, 41)
   xs, _, _ = _problem(m, d, 42)
   po, pg = _params(d)
   pred = go.precompute_predictive(po, x, y)
   dev.fit(x, y, pg)
   acq = _gp().Acquisition(1.8, True, go.trust_radius(n, d, 0))
-  out = dev.score(xs, acq, with_aux=True)
-  dev.synchronize()
   want, aux = go.score_with_aux(pred, xs)
-  np.testing.assert_allclose(out['score'].cpu().numpy(), want, atol=TOL, rtol=0)
-  np.testing.assert_allclose(out['stddev'].cpu().numpy(), aux['stddev'], atol=TOL, rtol=0)
-  out2 = dev.score(xs, acq)
-  dev.synchronize()
-  np.testing.assert_allclose(out2['score'].cpu().numpy(), want, atol=TOL, rtol=0)
+  for small_tiles, small_route in ((-1, True), (0, False)):
+    dev.set_int('small_tiles', small_tiles)
+    try:
+      out = dev.score(xs, acq, with_aux=True)
+      route = dev.get_int('score_route')
+      out2 = dev.score(xs, acq)
+      dev.synchronize()
+    finally:
+      dev.set_int('small_tiles', -1)
+    assert (route == 0) == small_route, route
+    np.testing.assert_allclose(out['score'].cpu().numpy(), want, atol=TOL, rtol=0)
+    np.testing.assert_allclose(out['stddev'].cpu().numpy(), aux['stddev'], atol=TOL, rtol=0)
+    np.testing.assert_allclose(out2['score'].cpu().numpy(), want, atol=TOL, rtol=0)
 
 
 @pytest.mark.parametrize('n,d,m,radius', [(1000, 20, 25, None), (1000, 20, 512, 0.25), (960, 8, 64, 0.1),

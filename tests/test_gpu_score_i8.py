@@ -46,13 +46,18 @@ def _pool(dev, m, d, seed):
   return dev.random_pool(m, d, seed=seed)
 
 
+def _i8_tiles(dev):
+  """64-candidate tiles of a pool the integer-split kernel takes: at least one per SM (148 on a 132-SM H100)."""
+  return dev.get_int('sm_count') + 16
+
+
 @pytest.mark.parametrize('n,d,sf2', [(1000, 20, 1.0), (520, 7, 2.7), (192, 3, 0.31), (1030, 12, 1.0), (300, 40, 1.0),
                                      (2000, 50, 0.9999999), (300, 64, 1.0)])
 def test_i8_scores_match_oracle_and_dmma(dev, n, d, sf2):
   """np = 1024 / 576 (a half k chunk) / 192 / 1088; sf2 off a power of two; Dc = 40 and 50: one phase-1 trial
   buffer; Dc = 64: the phase-1 staging no longer fits next to the operand ring (nbuf = 1, phases back to back); C4's
   N = 2000 with sf2 just below a power of two (the balanced top digit needs the extra scale bit)."""
-  m = 148 * 64 + 37     # 149 tiles: more than one per SM on 132 SMs, so some CTAs reuse their digit buffers
+  m = _i8_tiles(dev) * 64 + 37     # one tile more than SMs + 16: some CTAs reuse their digit buffers
   x, y, _ = _problem(n, d, n)
   po, pg = _params(d, sf2=sf2)
   dev.fit(x, y, pg)
@@ -60,8 +65,10 @@ def test_i8_scores_match_oracle_and_dmma(dev, n, d, sf2):
   acq = _gp().Acquisition(1.8, True, go.trust_radius(n, d, 0))
   dev.set_int('score_i8', 0)
   ref = dev.score(xs, acq, with_aux=True)
+  assert dev.get_int('score_route') == 2
   dev.set_int('score_i8', 1)
   out = dev.score(xs, acq, with_aux=True)
+  assert dev.get_int('score_route') == 3 and dev.get_int('score_grid') == dev.get_int('sm_count')
   dev.synchronize()
   pred = go.precompute_predictive(po, x, y)
   sel = np.r_[0:256, m - 300:m]
@@ -81,7 +88,7 @@ def test_i8_scores_match_oracle_and_dmma(dev, n, d, sf2):
 
 def test_i8_ill_conditioned_and_categorical(dev):
   """sn2 = 1e-8 (Linv entries ~1e4, cancellation in W) and mixed continuous / categorical features."""
-  n, d, m = 600, 6, 148 * 64
+  n, d, m = 600, 6, _i8_tiles(dev) * 64
   x, y, _ = _problem(n, d, 3)
   po, pg = _params(d, sn2=1e-8, ls=0.05)
   dev.fit(x, y, pg)
@@ -118,7 +125,7 @@ def test_i8_ill_conditioned_and_categorical(dev):
 
 def test_i8_refit_invalidates_digit_planes(dev):
   """A second fit on the same handle (new Linv) must re-slice; a pool too small for the path falls back."""
-  n, d, m = 256, 4, 148 * 64
+  n, d, m = 256, 4, _i8_tiles(dev) * 64
   acq = _gp().Acquisition(1.8, False, 0.0)
   dev.set_int('score_i8', 1)
   for seed in (1, 2):
@@ -148,7 +155,7 @@ def test_i8_two_handles_on_two_streams_concurrently():
     dv = gp.DeviceGP(0)
     dv.set_int('score_i8', 1)
     dv.fit(x, y, pg)
-    xs = dv.random_pool(148 * 64 * 3, d, seed=k)
+    xs = dv.random_pool(_i8_tiles(dv) * 64 * 3, d, seed=k)
     ref = dv.score(xs, gp.Acquisition(1.8, False, 0.0), with_aux=True)
     dv.synchronize()
     devs.append(dv); pools.append(xs); want.append(ref['stddev'].clone())

@@ -484,6 +484,7 @@ int vzgp_set_int(vzgp_handle* h, const char* key, int value) {
   VZ_ARG(h && key, "handle / key");
   if (std::strcmp(key, "dataflow_ctas") == 0) { VZ_ARG(value >= 0, "value >= 0"); h->df_ctas = value; return 0; }
   if (std::strcmp(key, "score_i8") == 0) { VZ_ARG(value >= -1 && value <= 1, "value in {-1, 0, 1}"); h->score_i8 = value; return 0; }
+  if (std::strcmp(key, "small_tiles") == 0) { VZ_ARG(value >= -1, "value >= -1"); h->small_tiles = value; return 0; }
   set_error("vzgp_set_int: unknown key '%s'", key);
   return VZGP_ERR_ARG;
 }
@@ -492,6 +493,10 @@ int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value) {
   VZ_ARG(h && key && value, "handle / key / value");
   if (std::strcmp(key, "launches") == 0) { *value = h->launches; return 0; }
   if (std::strcmp(key, "score_i8_launches") == 0) { *value = h->i8_launches; return 0; }
+  if (std::strcmp(key, "sm_count") == 0) { *value = h->sm_count; return 0; }
+  if (std::strcmp(key, "score_route") == 0) { *value = h->score_route; return 0; }
+  if (std::strcmp(key, "score_nsplit") == 0) { *value = h->score_nsplit; return 0; }
+  if (std::strcmp(key, "score_grid") == 0) { *value = h->score_grid; return 0; }
   set_error("vzgp_get_int: unknown key '%s'", key);
   return VZGP_ERR_ARG;
 }

@@ -174,4 +174,11 @@ struct vzgp_handle {
   bool i8_ready = false;                        // the digit planes describe the current Linv
   int64_t i8_launches = 0;
   vzgp::DevBuf i8_planes, i8_scale, i8_kdig;
+
+  // Candidate scoring (score.cu): pools of at most small_tiles 64-candidate tiles take the small-pool kernels
+  // (-1: environment VZGP_SMALL_TILES, default 8).  The last launch_score on this handle records the route it
+  // took (vzgp_score_route), the CTAs sharing one tile (split route) and the grid of k_score / k_score_i8; tests
+  // read them through vzgp_get_int to check which kernel a case exercised.
+  int small_tiles = -1;
+  int score_route = -1, score_nsplit = 0, score_grid = 0;
 };

@@ -709,16 +709,22 @@ static int launch_score_general(vzgp_handle* h, const double* Xs, const int32_t*
 int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
                  double* score, double* mu, double* sigma, double* linf) {
   if (M <= 0) return 0;
-  if (h->kp.use_linear) return launch_score_general(h, Xs, Zs, M, acq, score, mu, sigma, linf);
+  auto record = [&](int route, int nsplit, int grid) { h->score_route = route; h->score_nsplit = nsplit; h->score_grid = grid; };
+  if (h->kp.use_linear) {
+    record(VZGP_ROUTE_GENERAL, 0, 0);
+    return launch_score_general(h, Xs, Zs, M, acq, score, mu, sigma, linf);
+  }
   const int ntiles = (M + kTM - 1) / kTM;
   const int nblocks = (h->np + kBN - 1) / kBN;
   // Pools of a few tiles (acquisition-optimiser batches) take the trial-axis decomposition.
-  static const int small_tiles_max = [] {
+  static const int env_small_tiles = [] {
     const char* e = getenv("VZGP_SMALL_TILES");   // tuning / test hook; 0 disables the small-pool path
     return e ? atoi(e) : 8;
   }();
+  const int small_tiles_max = h->small_tiles >= 0 ? h->small_tiles : env_small_tiles;
   ScoreArgs a;
   if (ntiles <= small_tiles_max) {
+    record(VZGP_ROUTE_SMALL, 0, 0);
     bool with_linf = false;
     VZ_TRY(prepare_small_score(h, Xs, Zs, M, acq, score, mu, sigma, linf, &a, &with_linf));
     const int nvb = h->np / kVarCols, nmb = h->np / 64;
@@ -746,7 +752,10 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
     // (C2 pool: 5.18 ms for k_score_i8 against 4.35 ms for k_score, H100 80GB HBM3 at a 700 W power limit).
     static const int env_i8 = [] { const char* e = getenv("VZGP_SCORE_I8"); return e ? atoi(e) : 0; }();
     const int want = h->score_i8 >= 0 ? h->score_i8 : env_i8;
-    if (want && score_i8_eligible(h, M)) return launch_score_i8(h, Xs, Zs, M, acq, score, mu, sigma, linf);
+    if (want && score_i8_eligible(h, M)) {
+      record(VZGP_ROUTE_I8, 1, 0);   // launch_score_i8 records its grid
+      return launch_score_i8(h, Xs, Zs, M, acq, score, mu, sigma, linf);
+    }
   }
   // Medium pools cannot fill the GPU with one CTA per tile: share each tile's output column
   // blocks between nsplit CTAs (each recomputes the cheap K* tile).  Their CTAs walk different
@@ -775,6 +784,7 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
   const int want = (nwork + csize - 1) / csize;
   const int grid = (want < slots ? want : slots) * csize;
   cfg.gridDim = dim3(grid);
+  record(nsplit > 1 ? VZGP_ROUTE_SPLIT : VZGP_ROUTE_CLUSTER, nsplit, grid);
   VZ_TRY(ensure_scratch(h, (size_t)grid * kTM * h->np * sizeof(double)));
   fill_score_args(h, Xs, Zs, M, acq, score, mu, sigma, linf, &a);
   VZ_TRY(make_map(&a.mapA, a.scratch, (uint64_t)grid * kTM, (uint64_t)h->np, (uint64_t)h->np, kTM));

@@ -614,6 +614,7 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
   VZ_CHECK_LAUNCH();
   h->launches++;
   h->i8_launches++;
+  h->score_grid = grid;
   return 0;
 }
 
