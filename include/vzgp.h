@@ -76,6 +76,37 @@ typedef struct vzgp_acq {
                                    1: inside if dist <  radius (gp_ucb_pe.py:236-241) */
 } vzgp_acq;
 
+/* Acquisition function of the single-model, ensemble and stack scoring calls (acquisitions.py:213-274,
+ * :368-492), evaluated on the posterior mean mu and stddev sd of each candidate before the trust region:
+ *   UCB  mu + coefficient * sd              (the default: vzgp_acq.ucb_coefficient)
+ *   LCB  mu - coefficient * sd
+ *   EI   imp * Phi(imp / sd) + sd * phi(imp / sd),  imp = mu - best_label - exploration  (TFP default 0.01)
+ *   PI   Phi((mu - best_label - exploration) / sd)                                     (exploration 0)
+ * With sd = 0 (a clamped variance) EI = max(imp, 0) and PI = (imp > 0).
+ * use_threshold (AcquisitionTrustRegion): where the `thresholding` value t is not >= threshold the score is
+ * bad_acq_value - t, elsewhere the `main` acquisition.  The caller resolves a NaN threshold and apply_tr_after by
+ * passing use_threshold = 0. */
+typedef enum vzgp_acq_kind { VZGP_ACQ_UCB = 0, VZGP_ACQ_LCB = 1, VZGP_ACQ_EI = 2, VZGP_ACQ_PI = 3 } vzgp_acq_kind;
+typedef struct vzgp_acq_term {
+  int kind;               /* vzgp_acq_kind */
+  double coefficient;     /* UCB / LCB */
+  double best_label;      /* EI / PI: finite */
+  double exploration;     /* EI / PI */
+} vzgp_acq_term;
+typedef struct vzgp_acq_fn {
+  vzgp_acq_term main;
+  int use_threshold;      /* AcquisitionTrustRegion: 0 = main only */
+  vzgp_acq_term thresholding;
+  double threshold, bad_acq_value;
+} vzgp_acq_fn;
+
+/* Sets the acquisition function of every later call on h that takes a vzgp_acq (vzgp_score and its host / top-k
+ * variants, vzgp_suggest_host, vzgp_random_search, vzgp_eagle_run and the host-stepped loop's scoring); fn = NULL
+ * restores UCB with vzgp_acq.ucb_coefficient (the default).  Multi-handle calls (ensemble, stack) use the setting
+ * of hs[0].  GP-UCB-PE, set-PE and multi-metric calls ignore it.  Unknown kinds and a non-finite best_label for EI
+ * or PI are rejected with VZGP_ERR_ARG. */
+int vzgp_set_acquisition(vzgp_handle* h, const vzgp_acq_fn* fn);
+
 /* GP-UCB-PE acquisition (vizier/_src/algorithms/designers/gp_ucb_pe.py:282-492) built from two
  * fitted models: A = completed trials (mean, stddev), B = completed + pending trials
  * (stddev_from_all; its labels are irrelevant).

@@ -53,6 +53,28 @@ class Acq(C.Structure):
   ]
 
 
+ACQ_UCB, ACQ_LCB, ACQ_EI, ACQ_PI = 0, 1, 2, 3   # vzgp_acq_kind
+
+
+class AcqTerm(C.Structure):
+  _fields_ = [
+      ('kind', C.c_int),
+      ('coefficient', C.c_double),
+      ('best_label', C.c_double),
+      ('exploration', C.c_double),
+  ]
+
+
+class AcqFn(C.Structure):
+  _fields_ = [
+      ('main', AcqTerm),
+      ('use_threshold', C.c_int),
+      ('thresholding', AcqTerm),
+      ('threshold', C.c_double),
+      ('bad_acq_value', C.c_double),
+  ]
+
+
 class PeParams(C.Structure):
   _fields_ = [
       ('mode', C.c_int),
@@ -133,6 +155,7 @@ SIGNATURES = {
     'vzgp_launch_count': (_i64, [_vp]),
     'vzgp_set_int': (_i, [_vp, C.c_char_p, _i]),
     'vzgp_get_int': (_i, [_vp, C.c_char_p, C.POINTER(C.c_int64)]),
+    'vzgp_set_acquisition': (_i, [_vp, C.POINTER(AcqFn)]),
     'vzgp_kernel_matrix': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _pP, _d, _vp, _i]),
     'vzgp_cross_kernel': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _pP, _vp, _i]),
     'vzgp_cholesky_retry': (_i, [_vp, _vp, _i, _i, _d, _i, _vp, _i, _pd]),

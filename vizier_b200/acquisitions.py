@@ -1,18 +1,186 @@
-"""Host-side acquisition parameters: UCB coefficient and the trust region's scalar state.
+"""Host-side acquisition parameters: the acquisition function and the trust region's scalar state.
 
-Mirrors vizier/_src/algorithms/designers/gp/acquisitions.py: `UCB` (:213-225, coefficient 1.8),
-`TrustRegion.__post_init__` (:734-749, which dimensions take part), `TrustRegion.trust_radius`
-(:757-777).  The per-candidate work (min L-inf distance, thresholding, -1e4 - distance penalty)
-runs inside the CUDA scoring kernel; only these O(D) scalars are computed here.
+Mirrors vizier/_src/algorithms/designers/gp/acquisitions.py: `UCB` / `LCB` / `EI` / `PI` (:213-274),
+`AcquisitionTrustRegion` (:390-492), `get_best_labels` (:92-109), `bayesian_scoring_function_factory`
+(:368-387), `TrustRegion.__post_init__` (:734-749, which dimensions take part), `TrustRegion.trust_radius`
+(:757-777).  The per-candidate work (the acquisition of (mean, stddev), its thresholding, the min L-inf distance
+and the -1e4 - distance penalty) runs inside the CUDA scoring kernels; `lower_acquisition` turns an acquisition
+object into the O(1) scalars they take.
 """
 
 from __future__ import annotations
 
-from typing import Optional, Sequence
+import dataclasses
+import warnings
+from typing import Any, Callable, Optional, Sequence
 
 import numpy as np
 
+from vizier_b200 import _lib
 from vizier_b200 import gp
+
+EI_EXPLORATION = 0.01      # tfp_bo GaussianProcessExpectedImprovement default exploration
+PI_EXPLORATION = 0.0       # tfp_bo GaussianProcessProbabilityOfImprovement default exploration
+
+
+class PaddedArray:
+  """The part of vizier's `types.PaddedArray` the acquisitions use.  Arrays here are never padded: every row is
+  an observation, so `replace_fill_value` has nothing to replace."""
+
+  def __init__(self, array, fill_value=np.nan):
+    self.padded_array = np.asarray(array, np.float64)
+    self.fill_value = fill_value
+    self._original_shape = self.padded_array.shape
+
+  @classmethod
+  def as_padded(cls, array) -> 'PaddedArray':
+    return cls(array)
+
+  def replace_fill_value(self, fill_value) -> 'PaddedArray':
+    return PaddedArray(self.padded_array, fill_value)
+
+
+@dataclasses.dataclass
+class ModelData:
+  """types.ModelData: `features` as the converter produces them, `labels` [num_observations, num_metrics]."""
+
+  features: Any
+  labels: PaddedArray
+
+
+def get_best_labels(labels: PaddedArray) -> np.ndarray:
+  """Maximum label per metric; -inf without observations (acquisitions.py:92-109)."""
+  if np.size(labels.padded_array) == 0:
+    return np.asarray(-np.inf)
+  return np.max(labels.replace_fill_value(-np.inf).padded_array, axis=-2)
+
+
+@dataclasses.dataclass
+class UCB:
+  coefficient: float = 1.8
+
+
+@dataclasses.dataclass
+class LCB:
+  coefficient: float = 1.8
+
+
+@dataclasses.dataclass
+class EI:
+  best_labels: Any
+
+
+@dataclasses.dataclass
+class PI:
+  best_labels: Any
+
+
+@dataclasses.dataclass
+class AcquisitionTrustRegion:
+  """`main_acquisition` where `thresholding_acquisition` >= threshold, else bad_acq_value - thresholding value.
+  threshold defaults to min(nanmean, nanmedian) of `labels`; with at most `apply_tr_after` labels the main
+  acquisition applies everywhere."""
+
+  main_acquisition: Any
+  thresholding_acquisition: Any
+  bad_acq_value: float = dataclasses.field(kw_only=True)
+  labels: Optional[PaddedArray] = dataclasses.field(kw_only=True)
+  threshold: Optional[float] = dataclasses.field(kw_only=True, default=None)
+  apply_tr_after: Optional[int] = dataclasses.field(kw_only=True, default=0)
+
+  @classmethod
+  def default_ucb_pi(cls, data: ModelData) -> 'AcquisitionTrustRegion':
+    return cls(UCB(1.8), PI(get_best_labels(data.labels)), bad_acq_value=-1e4, labels=data.labels, threshold=0.3,
+               apply_tr_after=0)
+
+  @classmethod
+  def default_ucb_lcb(cls, data: ModelData) -> 'AcquisitionTrustRegion':
+    return cls(UCB(1.8), LCB(1.8), labels=data.labels, bad_acq_value=-1e4, threshold=None, apply_tr_after=0)
+
+  @classmethod
+  def default_ucb_lcb_wide(cls, data: ModelData) -> 'AcquisitionTrustRegion':
+    return cls(UCB(1.8), LCB(2.5), labels=data.labels, bad_acq_value=-1e4, threshold=None, apply_tr_after=0)
+
+  @classmethod
+  def default_ucb_lcb_delay_tr(cls, data: ModelData) -> 'AcquisitionTrustRegion':
+    return cls(UCB(1.8), LCB(1.8), labels=data.labels, bad_acq_value=-1e4, threshold=None, apply_tr_after=5)
+
+
+@dataclasses.dataclass
+class BayesianScoringFunction:
+  """What a scoring-function factory returns: the acquisition function and whether the trust region applies.
+  The designer lowers `acquisition_fn` and scores on the device."""
+
+  predictive: Any
+  acquisition_fn: Any
+  use_trust_region: bool = False
+
+
+def bayesian_scoring_function_factory(acquisition_fn_factory: Callable[[ModelData], Any]) -> Callable:
+  """acquisitions.py:368-387: (data, predictive, continuous_feasible_values, use_trust_region) -> scoring function."""
+
+  def f(data: ModelData, predictive, continuous_feasible_values, use_trust_region: bool = False):
+    del continuous_feasible_values
+    return BayesianScoringFunction(predictive, acquisition_fn_factory(data), use_trust_region)
+
+  return f
+
+
+def _best_label(best_labels) -> float:
+  b = np.asarray(best_labels, np.float64).reshape(-1)
+  if b.size != 1:
+    raise NotImplementedError(f'EI / PI with {b.size} best labels (one metric only)')
+  return float(b[0])
+
+
+def _lower_term(fn) -> gp.AcqTermSpec:
+  if isinstance(fn, UCB):
+    return gp.AcqTermSpec(_lib.ACQ_UCB, coefficient=float(fn.coefficient))
+  if isinstance(fn, LCB):
+    return gp.AcqTermSpec(_lib.ACQ_LCB, coefficient=float(fn.coefficient))
+  if isinstance(fn, (EI, PI)):
+    best = _best_label(fn.best_labels)
+    if not np.isfinite(best):
+      # No observation yet (best label -inf): EI is +inf and PI is 1 everywhere.  Score the posterior mean
+      # instead, the order EI approaches as the best label goes to -inf.
+      return gp.AcqTermSpec(_lib.ACQ_UCB, coefficient=0.0)
+    if isinstance(fn, EI):
+      return gp.AcqTermSpec(_lib.ACQ_EI, best_label=best, exploration=EI_EXPLORATION)
+    return gp.AcqTermSpec(_lib.ACQ_PI, best_label=best, exploration=PI_EXPLORATION)
+  raise NotImplementedError(
+      f'acquisition function {type(fn).__name__} is not implemented on the device (UCB, LCB, EI, PI and '
+      'AcquisitionTrustRegion of those are)')
+
+
+def check_supported(fn) -> None:
+  """Raises NotImplementedError unless `lower_acquisition` can lower `fn` (any labels)."""
+  if isinstance(fn, AcquisitionTrustRegion):
+    check_supported(fn.main_acquisition)
+    check_supported(fn.thresholding_acquisition)
+  elif not isinstance(fn, (UCB, LCB, EI, PI)):
+    _lower_term(fn)
+
+
+def lower_acquisition(fn) -> gp.AcqFnSpec:
+  """An acquisition function object -> the `gp.AcqFnSpec` the scoring kernels evaluate.  AcquisitionTrustRegion:
+  threshold = its `threshold`, else min(nanmean, nanmedian) of its labels; a NaN threshold, or at most
+  `apply_tr_after` labels, leaves the main acquisition alone (acquisitions.py:466-492)."""
+  if not isinstance(fn, AcquisitionTrustRegion):
+    return gp.AcqFnSpec(_lower_term(fn))
+  main = _lower_term(fn.main_acquisition)
+  thr = _lower_term(fn.thresholding_acquisition)
+  threshold, main_only = -np.inf, False
+  if fn.labels is not None:
+    labels = fn.labels.replace_fill_value(np.nan).padded_array
+    with warnings.catch_warnings():           # all-NaN labels: NaN threshold, no warning
+      warnings.simplefilter('ignore', RuntimeWarning)
+      threshold = float(np.minimum(np.nanmean(labels), np.nanmedian(labels))) if labels.size else np.nan
+    main_only = fn.labels._original_shape[0] <= fn.apply_tr_after
+  if fn.threshold is not None:
+    threshold = float(fn.threshold)
+  if np.isnan(threshold) or main_only:
+    return gp.AcqFnSpec(main)
+  return gp.AcqFnSpec(main, thresholding=thr, threshold=threshold, bad_acq_value=float(fn.bad_acq_value))
 
 TR_MIN_RADIUS = 0.2        # TrustRegion.min_radius (acquisitions.py:751-754)
 TR_DIMENSION_FACTOR = 5.0  # acquisitions.py:760

@@ -394,6 +394,18 @@ static int ensure_pinned(vzgp_handle* h, size_t bytes) {
   return 0;
 }
 
+// The acquisition function the scoring calls on h evaluate (nullptr: UCB with the call's coefficient).
+static const AcqFn* handle_acq(const vzgp_handle* h) { return h->has_acq_fn ? &h->acq_fn : nullptr; }
+
+static int acq_term_from(const vzgp_acq_term& t, AcqTerm* out) {
+  VZ_ARG(t.kind >= VZGP_ACQ_UCB && t.kind <= VZGP_ACQ_PI, "unknown vzgp_acq_kind");
+  VZ_ARG(std::isfinite(t.coefficient) || t.kind == VZGP_ACQ_EI || t.kind == VZGP_ACQ_PI, "finite coefficient");
+  VZ_ARG((t.kind != VZGP_ACQ_EI && t.kind != VZGP_ACQ_PI) || (std::isfinite(t.best_label) && std::isfinite(t.exploration)),
+         "EI / PI need a finite best_label and exploration");
+  out->kind = t.kind; out->coefficient = t.coefficient; out->best_label = t.best_label; out->exploration = t.exploration;
+  return 0;
+}
+
 }  // namespace vzgp
 
 using namespace vzgp;
@@ -487,6 +499,24 @@ int vzgp_set_int(vzgp_handle* h, const char* key, int value) {
   if (std::strcmp(key, "small_tiles") == 0) { VZ_ARG(value >= -1, "value >= -1"); h->small_tiles = value; return 0; }
   set_error("vzgp_set_int: unknown key '%s'", key);
   return VZGP_ERR_ARG;
+}
+
+int vzgp_set_acquisition(vzgp_handle* h, const vzgp_acq_fn* fn) {
+  VZ_ARG(h != nullptr, "handle");
+  if (fn == nullptr) { h->has_acq_fn = false; return 0; }
+  AcqFn f = ucb_acq_fn(0.0);
+  VZ_TRY(acq_term_from(fn->main, &f.main));
+  f.use_thr = fn->use_threshold ? 1 : 0;
+  if (f.use_thr) {
+    VZ_TRY(acq_term_from(fn->thresholding, &f.thr));
+    VZ_ARG(!std::isnan(fn->threshold), "threshold is NaN (pass use_threshold = 0)");
+    VZ_ARG(std::isfinite(fn->bad_acq_value), "finite bad_acq_value");
+    f.threshold = fn->threshold;
+    f.bad_value = fn->bad_acq_value;
+  }
+  h->acq_fn = f;
+  h->has_acq_fn = true;
+  return 0;
 }
 
 int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value) {
@@ -726,7 +756,7 @@ int vzgp_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const
   if (h != nullptr && h->fitted && M == 0) return 0;  // empty pool: nothing to do
   VZ_TRY(check_scoring(h, Xs, Zs, M, acq, score));
   Guard g(h->device);
-  return launch_score(h, Xs, Zs, M, acq, score, mu, sigma, linf);
+  return launch_score(h, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(h));
 }
 
 int vzgp_clamped_count(vzgp_handle* h, int64_t* count_out) {
@@ -781,7 +811,7 @@ static int score_host_enqueue(vzgp_handle* h, const double* Xs, const int32_t* Z
     const int n = bounds[c + 1] - bounds[c];
     VZ_CUDA(cudaStreamWaitEvent(h->stream, h->copy_ev[c], 0));
     VZ_TRY(launch_score(h, dX + lo * h->dc, h->dk > 0 ? dZ + lo * h->dk : nullptr, n, acq, o + lo, mu ? o + M + lo : nullptr,
-                        sigma ? o + 2 * (size_t)M + lo : nullptr, linf ? o + 3 * (size_t)M + lo : nullptr));
+                        sigma ? o + 2 * (size_t)M + lo : nullptr, linf ? o + 3 * (size_t)M + lo : nullptr, handle_acq(h)));
   }
   *dX_out = dX;
   *o_out = o;
@@ -886,7 +916,7 @@ int vzgp_random_search(vzgp_handle* h, int64_t M, int64_t index_base, const vzgp
   int32_t* dBestZ = reinterpret_cast<int32_t*>(dBest + (size_t)kMaxTopk * (dc > 0 ? dc : 1));
   if (dc > 0) VZ_TRY(launch_random_fill(h, dX, M * dc, index_base * dc, seed, 3u, 0u));
   if (dk > 0) VZ_TRY(launch_random_fill_cat(h, dZ, M, dk, sizes, index_base, seed, 8u));
-  VZ_TRY(launch_score(h, dX, dk > 0 ? dZ : nullptr, (int)M, acq, dS, nullptr, nullptr, nullptr));
+  VZ_TRY(launch_score(h, dX, dk > 0 ? dZ : nullptr, (int)M, acq, dS, nullptr, nullptr, nullptr, handle_acq(h)));
   long long* d_idx; double* d_val;
   VZ_TRY(topk_to_device(h, dS, M, count, &d_idx, &d_val));
   if (dc > 0) VZ_TRY(launch_gather_rows(h, dX, dc, d_idx, count, M, dBest));
@@ -967,12 +997,13 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
                           double* best_score, vzgp_handle* const* ens = nullptr, int n_ens = 0,
                           const vzgp_scalarization* scal = nullptr, const double* stack_alphas = nullptr) {
   VZ_ARG(h && cfg && (acq || pe || scal) && best_score, "handle / pointers");
+  const AcqFn* fn = (pe || scal) ? nullptr : handle_acq(ens ? ens[0] : h);   // multi-handle calls: the setting of hs[0]
   auto score_batch = [&](const double* xs, const int32_t* zs, int m, double* out) -> int {
     if (scal) return launch_score_multi(h, xs, zs, m, out, nullptr, nullptr);
     if (pe) return launch_score_pe(h, hB, xs, zs, m, pe, out, nullptr, nullptr, nullptr);
-    if (stack_alphas) return launch_score_stack(ens, n_ens, stack_alphas, xs, zs, m, acq, out, nullptr, nullptr, nullptr);
-    if (n_ens > 1) return launch_score_ensemble(ens, n_ens, xs, zs, m, acq, out, nullptr, nullptr, nullptr);
-    return launch_score(h, xs, zs, m, acq, out, nullptr, nullptr, nullptr);
+    if (stack_alphas) return launch_score_stack(ens, n_ens, stack_alphas, xs, zs, m, acq, out, nullptr, nullptr, nullptr, fn);
+    if (n_ens > 1) return launch_score_ensemble(ens, n_ens, xs, zs, m, acq, out, nullptr, nullptr, nullptr, fn);
+    return launch_score(h, xs, zs, m, acq, out, nullptr, nullptr, nullptr, fn);
   };
   if (!h->fitted) { set_error("vzgp_eagle_run before vzgp_fit"); return VZGP_ERR_STATE; }
   VZ_ARG(best_x != nullptr || h->dc == 0, "best_x");
@@ -1009,12 +1040,12 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
   bool done = false;
   if (n_ens <= 1 && !scal && !stack_alphas && eagle_persistent_eligible(h, pe ? hB : nullptr, e)) {
     // small study: the whole loop is one persistent single-CTA kernel
-    VZ_TRY(launch_eagle_persistent64(h, pe ? hB : nullptr, e, acq, pe, steps));
+    VZ_TRY(launch_eagle_persistent64(h, pe ? hB : nullptr, e, acq, pe, steps, fn));
     done = true;
   } else if (n_ens <= 1 && !scal && !stack_alphas && eagle_grid_eligible(h, pe ? hB : nullptr, e)) {
     // mid-size study: one cooperative launch, phases separated by grid barriers.  If the cooperative
     // launch is refused (nothing has run then) the launch-per-phase loop below takes over.
-    done = launch_eagle_grid(h, pe ? hB : nullptr, e, acq, pe, steps) == 0;
+    done = launch_eagle_grid(h, pe ? hB : nullptr, e, acq, pe, steps, fn) == 0;
     if (!done) cudaGetLastError();
   }
   if (!done) {
@@ -1250,7 +1281,7 @@ int vzgp_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const i
   VZ_ARG(M == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
   VZ_ARG(M == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
   Guard g(hs[0]->device);
-  return launch_score_ensemble(hs, E, Xs, Zs, M, acq, score, mu, sigma, linf);
+  return launch_score_ensemble(hs, E, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(hs[0]));
 }
 
 int vzgp_eagle_run_ensemble(vzgp_handle* const* hs, int E, const vzgp_eagle_config* cfg, const vzgp_acq* acq,
@@ -1282,7 +1313,7 @@ int vzgp_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const 
   VZ_ARG(M == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
   VZ_ARG(M == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
   Guard g(hs[0]->device);
-  return launch_score_stack(hs, E, alphas, Xs, Zs, M, acq, score, mu, sigma, linf);
+  return launch_score_stack(hs, E, alphas, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(hs[0]));
 }
 
 int vzgp_eagle_run_stack(vzgp_handle* const* hs, int E, const double* alphas, const vzgp_eagle_config* cfg,
@@ -1505,7 +1536,7 @@ int vzgp_score_topk(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
   VZ_TRY(check_scoring(h, Xs, Zs, M, acq, dS));
   VZ_ARG(h->dk == 0, "continuous features only");
   VZ_TRY(h->xs_dev.reserve(0));
-  VZ_TRY(launch_score(h, Xs, Zs, M, acq, dS, nullptr, nullptr, nullptr));
+  VZ_TRY(launch_score(h, Xs, Zs, M, acq, dS, nullptr, nullptr, nullptr, handle_acq(h)));
   long long* d_idx; double* d_val;
   VZ_TRY(topk_to_device(h, dS, M, count, &d_idx, &d_val));
   double* dBest = reinterpret_cast<double*>(h->small.as<char>() + kOffRows);
@@ -1536,7 +1567,7 @@ int vzgp_score_topk_pack(vzgp_handle* h, const double* Xs, const int32_t* Zs, in
   }
   VZ_TRY(check_scoring(h, Xs, Zs, M, acq, dS));
   VZ_ARG(h->dk == 0, "continuous features only");
-  VZ_TRY(launch_score(h, Xs, Zs, M, acq, dS, nullptr, nullptr, nullptr));
+  VZ_TRY(launch_score(h, Xs, Zs, M, acq, dS, nullptr, nullptr, nullptr, handle_acq(h)));
   long long* d_idx; double* d_val;
   VZ_TRY(topk_to_device(h, dS, M, count, &d_idx, &d_val));
   return launch_pack_topk(h, Xs, dc, d_idx, d_val, count, M, index_base, payload_dev);

@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/vzgp.h"
+#include "acq_fn.cuh"
 
 namespace vzgp {
 
@@ -181,4 +182,9 @@ struct vzgp_handle {
   // read them through vzgp_get_int to check which kernel a case exercised.
   int small_tiles = -1;
   int score_route = -1, score_nsplit = 0, score_grid = 0;
+
+  // Acquisition function set by vzgp_set_acquisition (c_abi.cu); without one the calls score UCB with their
+  // vzgp_acq.ucb_coefficient.  Read at every call: no launch state is built from it.
+  bool has_acq_fn = false;
+  vzgp::AcqFn acq_fn;
 };

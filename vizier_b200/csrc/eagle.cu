@@ -279,8 +279,9 @@ __device__ __forceinline__ void posterior_tile64(const SmallModel& m, const Mode
   __syncthreads();
 }
 
-// Acquisition of the batch from the staged model(s): UCB + trust region (acquisitions.py:152-225) or the
+// Acquisition of the batch from the staged model(s): acquisition function (acq_fn.cuh) + trust region (acquisitions.py:152-225) or the
 // GP-UCB-PE combination of models a (completed trials) and b (completed + pending), gp_ucb_pe.py:344-492.
+template <bool GENERIC>
 __device__ __forceinline__ void score_batch64(const SmallModel& ma, const SmallModel& mb, const SmallAcq& q,
                                               const PersistSmem& sm, const double* cand, const int32_t* candz, int B,
                                               double* out_score, int* clamp_count) {
@@ -289,7 +290,7 @@ __device__ __forceinline__ void score_batch64(const SmallModel& ma, const SmallM
   if (q.pe_mode < 0) {
     posterior_tile64(ma, sm.a, sm, B, q, sm.mu, sm.sd, q.want_linf ? sm.linf : nullptr, clamp_count);
     if (tid < B) {
-      double sc = fma(q.coef, sm.sd[tid], sm.mu[tid]);
+      double sc = acq_eval<GENERIC>(q.fn, sm.mu[tid], sm.sd[tid]);
       if (q.apply_tr) {
         const double dist = sm.linf[tid];
         const bool inside = (q.tr_strict ? (dist < q.radius) : (dist <= q.radius)) || (q.radius > 0.5);
@@ -319,6 +320,7 @@ __device__ __forceinline__ void score_batch64(const SmallModel& ma, const SmallM
   __syncthreads();
 }
 
+template <bool GENERIC>
 __global__ void __launch_bounds__(kPThreads) k_eagle_persistent64(const EagleDev eg, SmallModel m, SmallModel mb,
                                                                   SmallAcq q, int steps, size_t eagle_scratch_doubles,
                                                                   int* clamp_count) {
@@ -386,7 +388,7 @@ __global__ void __launch_bounds__(kPThreads) k_eagle_persistent64(const EagleDev
     for (int vb = 0; vb < nvb; ++vb) eagle_suggest_block<kW>(e, vb, sm.eagle);
     __syncthreads();
     VZ_ET(c_s);
-    score_batch64(m, mb, q, sm, e.batch, e.batch_z, e.B, e.batch_r, clamp_count);
+    score_batch64<GENERIC>(m, mb, q, sm, e.batch, e.batch_z, e.B, e.batch_r, clamp_count);
     VZ_ET(c_c);
     if (tid < 256) eagle_update_block<true>(e, sm.eagle);
     __syncthreads();
@@ -485,7 +487,7 @@ static SmallModel small_model_of(const vzgp_handle* h) {
 
 // acq (UCB on h) or pe (GP-UCB-PE on h = model A and hB = model B): exactly one is non-null.
 int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const vzgp_acq* acq,
-                              const vzgp_pe_params* pe, int steps) {
+                              const vzgp_pe_params* pe, int steps, const AcqFn* fn) {
   const SmallModel m = small_model_of(h);
   const SmallModel mb = hB ? small_model_of(hB) : m;
   const vzgp_handle* ht = pe ? hB : h;     // the trust region is measured on this model's trials
@@ -499,7 +501,7 @@ int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e
     q.radius = pe->trust_radius; q.apply_tr = pe->use_trust_region ? 1 : 0; q.tr_strict = 1;
     mask = pe->tr_dim_mask; tr_rows = pe->tr_rows;
   } else {
-    q.pe_mode = -1; q.coef = acq->ucb_coefficient;
+    q.pe_mode = -1; q.fn = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
     q.radius = acq->trust_radius; q.apply_tr = acq->use_trust_region ? 1 : 0; q.tr_strict = acq->tr_strict ? 1 : 0;
     mask = acq->tr_dim_mask; tr_rows = acq->tr_rows;
   }
@@ -514,8 +516,13 @@ int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e
                                       (size_t)nm * 64 + 128 + 128 + 64 + 256) +
                     sizeof(int32_t) * ((size_t)(nm + 1) * h->dk * kPXLD + 2) + eagle_persistent_state_bytes(e);
   if (sm > 227 * 1024) { set_error("persistent eagle kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
-  VZ_TRY(raise_dyn_smem((const void*)k_eagle_persistent64, sm));
-  k_eagle_persistent64<<<1, kPThreads, sm, h->stream>>>(e, m, mb, q, steps, scratch, h->small.as<int>());
+  if (q.pe_mode < 0 && !acq_fn_is_ucb(q.fn)) {
+    VZ_TRY(raise_dyn_smem((const void*)k_eagle_persistent64<true>, sm));
+    k_eagle_persistent64<true><<<1, kPThreads, sm, h->stream>>>(e, m, mb, q, steps, scratch, h->small.as<int>());
+  } else {
+    VZ_TRY(raise_dyn_smem((const void*)k_eagle_persistent64<false>, sm));
+    k_eagle_persistent64<false><<<1, kPThreads, sm, h->stream>>>(e, m, mb, q, steps, scratch, h->small.as<int>());
+  }
   VZ_CHECK_LAUNCH();
   h->launches++;
   return 0;

@@ -44,6 +44,7 @@ __device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned nblocks
   __syncthreads();
 }
 
+template <bool GENERIC>
 __global__ void __launch_bounds__(kSmallThreads) k_eagle_grid(const __grid_constant__ GridArgs g) {
   extern __shared__ double smem[];
   const EagleDev& e = g.e;
@@ -98,9 +99,11 @@ __global__ void __launch_bounds__(kSmallThreads) k_eagle_grid(const __grid_const
       for (int m0 = 0; m0 < e.B; m0 += kSmallThreads / 8) {
         const int m = m0 + (tid >> 3);
         const bool act = m < e.B;
-        if (g.wl_a) small_finalize_8<true>(g.a, m, p8, act, clamped); else small_finalize_8<false>(g.a, m, p8, act, clamped);
+        if (g.wl_a) small_finalize_8<true, GENERIC>(g.a, m, p8, act, clamped);
+        else small_finalize_8<false, GENERIC>(g.a, m, p8, act, clamped);
         if (two) {
-          if (g.wl_b) small_finalize_8<true>(g.b, m, p8, act, clamped); else small_finalize_8<false>(g.b, m, p8, act, clamped);
+          if (g.wl_b) small_finalize_8<true, false>(g.b, m, p8, act, clamped);
+          else small_finalize_8<false, false>(g.b, m, p8, act, clamped);
           __syncwarp();
           if (act && p8 == 0) {
             double acq;
@@ -148,7 +151,7 @@ bool eagle_grid_eligible(const vzgp_handle* h, const vzgp_handle* hB, const Eagl
 
 // acq (UCB on h) or pe (GP-UCB-PE on h = model A and hB = model B): exactly one is non-null.
 int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const vzgp_acq* acq,
-                      const vzgp_pe_params* pe, int steps) {
+                      const vzgp_pe_params* pe, int steps, const AcqFn* fn) {
   static thread_local GridArgs G;   // several KB (descriptors, parameter tables): kept off the stack
   G.e = e;
   G.steps = steps;
@@ -156,7 +159,7 @@ int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const 
   const int32_t* zs = h->dk > 0 ? e.batch_z : nullptr;
   bool wl = false;
   if (!pe) {
-    VZ_TRY(prepare_small_score(h, xs, zs, e.B, acq, e.batch_r, nullptr, nullptr, nullptr, &G.a, &wl));
+    VZ_TRY(prepare_small_score(h, xs, zs, e.B, acq, e.batch_r, nullptr, nullptr, nullptr, &G.a, &wl, fn));
     G.b = G.a;
     G.pe_mode = -1; G.wl_a = wl ? 1 : 0; G.wl_b = 0;
     G.ucb = G.explore = G.penalty = G.threshold = G.radius = 0.0; G.apply_tr = 0;
@@ -187,9 +190,10 @@ int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const 
   if (s_c > sm) sm = s_c;
   if (s_v > sm) sm = s_v;
   if (sm > 227 * 1024) { set_error("eagle grid kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
-  VZ_TRY(raise_dyn_smem((const void*)k_eagle_grid, sm));
+  const void* kfn = (!pe && !acq_fn_is_ucb(G.a.acq)) ? (const void*)k_eagle_grid<true> : (const void*)k_eagle_grid<false>;
+  VZ_TRY(raise_dyn_smem(kfn, sm));
   int occ = 0;
-  VZ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_eagle_grid, kSmallThreads, sm));
+  VZ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, kSmallThreads, sm));
   if (occ < 1) { set_error("eagle grid kernel does not fit on an SM"); return VZGP_ERR_UNSUPPORTED; }
   const int ntiles = (e.B + kTM - 1) / kTM;
   int want = (G.a.np / kVarCols) * ntiles + (pe ? (G.b.np / kVarCols) * ntiles : 0);   // W items >= K* items
@@ -199,7 +203,7 @@ int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const 
   VZ_CUDA(cudaMemsetAsync(bar, 0, sizeof(unsigned), h->stream));
   G.barrier = bar;
   void* params[] = {&G};
-  VZ_CUDA(cudaLaunchCooperativeKernel((const void*)k_eagle_grid, dim3(grid), dim3(kSmallThreads), params, sm, h->stream));
+  VZ_CUDA(cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(kSmallThreads), params, sm, h->stream));
   h->launches++;
   return 0;
 }

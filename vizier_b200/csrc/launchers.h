@@ -3,6 +3,7 @@
 #include <tuple>
 #include <type_traits>
 
+#include "acq_fn.cuh"
 #include "common.cuh"
 
 namespace vzgp {
@@ -73,19 +74,22 @@ int chol_dataflow(vzgp_handle* h, double* L, double* Linv, double* LinvT, double
 int chol_dataflow_prepare(vzgp_handle* h, int np, bool want_kinv);
 int chol_dataflow_timed_out(vzgp_handle* h, int* out);
 
+// The scoring launchers take the acquisition function as `fn`; nullptr means UCB with acq->ucb_coefficient (the
+// per-member scorings inside the ensemble, stack and GP-UCB-PE launchers rely on that).
 int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                 double* score, double* mu, double* sigma, double* linf);
+                 double* score, double* mu, double* sigma, double* linf, const AcqFn* fn = nullptr);
 // wgmma integer-split variant of the large-pool scoring kernel (score_i8.cu).
 bool score_i8_eligible(const vzgp_handle* h, int M);
 int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                    double* score, double* mu, double* sigma, double* linf);
+                    double* score, double* mu, double* sigma, double* linf, const AcqFn* fn = nullptr);
 // CUtensorMap (void*) of a u8 tensor of `rank` <= 3 dims (innermost first), byte strides of dims 1.., 128-byte swizzle.
 int make_tensor_map_u8(void* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                        const uint32_t* box, bool promote_256 = true);
 int launch_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
                     const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all);
 int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const double* Xs, const int32_t* Zs, int M,
-                       const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf);
+                       const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf,
+                       const AcqFn* fn = nullptr);
 int launch_set_pe_combine(vzgp_handle* h, int n_sets, int q, const vzgp_pe_params* pe, const double* cov, int ldc,
                           const double* mu_a, const double* sd_a, const double* linf, double* score, double* sd_all);
 int prepare_scalarization(vzgp_handle* h, const vzgp_scalarization* sc);
@@ -105,7 +109,8 @@ int launch_gather_rows(vzgp_handle* h, const double* X, int dc, const long long*
 int launch_nll_grad_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int n_valid,
                           const KernelParams& kp, double sn2, double jitter0, int max_iters, double* out);
 int launch_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int M,
-                          const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf);
+                          const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf,
+                          const AcqFn* fn = nullptr);
 int launch_pack_topk(vzgp_handle* h, const double* X, int dc, const long long* idx, const double* val,
                      int count, int64_t M, int64_t index_base, double* payload);
 int launch_merge_topk(vzgp_handle* h, const double* rows, int n_rows, int width, int count, double* out);
@@ -148,7 +153,8 @@ struct SmallModel {
   int n_valid;
 };
 struct SmallAcq {
-  double coef, radius;
+  AcqFn fn;                             // pe_mode < 0: acquisition function of (mean, stddev)
+  double coef, radius;                  // coef: GP-UCB-PE mode 0
   double explore, penalty, threshold;   // GP-UCB-PE
   int pe_mode;                          // -1: UCB on one model; 0 / 1: GP-UCB-PE modes (vzgp_pe_params.mode)
   int apply_tr, tr_rows, tr_strict, want_linf;
@@ -156,11 +162,11 @@ struct SmallAcq {
 };
 bool eagle_persistent_eligible(const vzgp_handle* h, const vzgp_handle* hB, const EagleDev& e);
 int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const vzgp_acq* acq,
-                              const vzgp_pe_params* pe, int steps);
+                              const vzgp_pe_params* pe, int steps, const AcqFn* fn = nullptr);
 // Multi-CTA persistent Eagle loop (eagle_grid.cu): cooperative launch, batch <= 512 candidates.
 bool eagle_grid_eligible(const vzgp_handle* h, const vzgp_handle* hB, const EagleDev& e);
 int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const vzgp_acq* acq,
-                      const vzgp_pe_params* pe, int steps);
+                      const vzgp_pe_params* pe, int steps, const AcqFn* fn = nullptr);
 size_t eagle_suggest_smem(const EagleDev& e);
 size_t eagle_update_smem(const EagleDev& e);
 size_t eagle_suggest_cta_smem(const EagleDev& e);

@@ -67,7 +67,7 @@ __device__ unsigned long long g_score_t[8];
 #define VZ_ST(...)
 #endif
 
-template <bool WITH_LINF>
+template <bool WITH_LINF, bool GENERIC>
 __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constant__ ScoreArgs a) {
   extern __shared__ double smem_raw[];
   // the swizzled TMA boxes need a 1024-byte aligned base
@@ -374,7 +374,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       if (m < a.M) {
         const double rs = (s_rowsq[r] + s_rowsq[64 + r]) + (s_rowsq[128 + r] + s_rowsq[192 + r]);
         if (nsplit == 1) {
-          emit_score(a, m, rs, s_mu[r], s_linf[r], clamped);
+          emit_score<GENERIC>(a, m, rs, s_mu[r], s_linf[r], clamped);
         } else {
           a.part[(size_t)split * a.mpad + m] = rs;
           if (split == 0) {
@@ -556,7 +556,7 @@ static int max_active_clusters(const void* kfn, const cudaLaunchConfig_t& cfg, i
 }
 
 static void fill_score_args(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                            double* score, double* mu, double* sigma, double* linf, ScoreArgs* pa) {
+                            const AcqFn* fn, double* score, double* mu, double* sigma, double* linf, ScoreArgs* pa) {
   ScoreArgs& a = *pa;
   const int ntiles = (M + kTM - 1) / kTM;
   a.Xs = Xs; a.Zs = Zs; a.M = M;
@@ -565,7 +565,7 @@ static void fill_score_args(vzgp_handle* h, const double* Xs, const int32_t* Zs,
   a.Linv = h->Linv.as<double>(); a.ldi = h->np;
   a.alpha = h->alpha.as<double>();
   a.kp = h->kp; a.sn2 = h->sn2;
-  a.coef = acq->ucb_coefficient;
+  a.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
   a.apply_tr = acq->use_trust_region ? 1 : 0;
   a.tr_rows = (acq->tr_rows > 0 && acq->tr_rows < h->n_valid) ? acq->tr_rows : h->n_valid;
   a.tr_strict = acq->tr_strict ? 1 : 0;
@@ -584,10 +584,11 @@ static void fill_score_args(vzgp_handle* h, const double* Xs, const int32_t* Zs,
 }
 
 int prepare_small_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                        double* score, double* mu, double* sigma, double* linf, ScoreArgs* a, bool* with_linf) {
+                        double* score, double* mu, double* sigma, double* linf, ScoreArgs* a, bool* with_linf,
+                        const AcqFn* fn) {
   const int ntiles = (M + kTM - 1) / kTM;
   VZ_TRY(ensure_scratch(h, (size_t)ntiles * kTM * h->np * sizeof(double)));
-  fill_score_args(h, Xs, Zs, M, acq, score, mu, sigma, linf, a);
+  fill_score_args(h, Xs, Zs, M, acq, fn, score, mu, sigma, linf, a);
   const int nvb = h->np / kVarCols, nmb = h->np / 64;
   VZ_TRY(h->Tws.reserve(sizeof(double) * (size_t)(nvb + 2 * nmb) * a->mpad));
   a->part_rs = h->Tws.as<double>();
@@ -615,7 +616,8 @@ struct GeneralArgs {
   const double* alpha;
   int mc, np, n_valid, dc;
   KernelParams kp;
-  double sn2, mean_const, coef, radius;
+  double sn2, mean_const, radius;
+  AcqFn acq;
   int apply_tr, tr_rows, tr_strict, want_linf;
   uint8_t tr_mask[kMaxDc];
   double* score; double* mu; double* sigma; double* linf;
@@ -659,7 +661,7 @@ __global__ void __launch_bounds__(256) k_general_finalize(GeneralArgs a) {
   double var = kss - rs + a.sn2;
   if (var < 0.0) { var = 0.0; atomicAdd(a.clamp_count, 1); }
   const double sd = sqrt(var);
-  double sc = fma(a.coef, sd, mean);
+  double sc = acq_value(a.acq, mean, sd);
   if (a.apply_tr) {
     const bool inside = (a.tr_strict ? (dist < a.radius) : (dist <= a.radius)) || (a.radius > 0.5);
     sc = inside ? sc : (-1e4 - dist);
@@ -671,7 +673,7 @@ __global__ void __launch_bounds__(256) k_general_finalize(GeneralArgs a) {
 }
 
 static int launch_score_general(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                                double* score, double* mu, double* sigma, double* linf) {
+                                const AcqFn* fn, double* score, double* mu, double* sigma, double* linf) {
   const int np = h->np, dc = h->dc, dk = h->dk;
   constexpr int kChunk = 4096;
   const size_t nks = (size_t)kChunk * np, nx = (size_t)kChunk * (dc > 0 ? dc : 1);
@@ -683,7 +685,7 @@ static int launch_score_general(vzgp_handle* h, const double* Xs, const int32_t*
   GeneralArgs a;
   a.Ks = Ks; a.W = W; a.Xs = Xp; a.X = h->X.as<double>(); a.alpha = h->alpha.as<double>();
   a.np = np; a.n_valid = h->n_valid; a.dc = dc; a.kp = h->kp; a.sn2 = h->sn2; a.mean_const = h->mean_const;
-  a.coef = acq->ucb_coefficient; a.radius = acq->trust_radius;
+  a.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient); a.radius = acq->trust_radius;
   a.apply_tr = acq->use_trust_region ? 1 : 0;
   a.tr_rows = (acq->tr_rows > 0 && acq->tr_rows < h->n_valid) ? acq->tr_rows : h->n_valid;
   a.tr_strict = acq->tr_strict ? 1 : 0;
@@ -707,12 +709,12 @@ static int launch_score_general(vzgp_handle* h, const double* Xs, const int32_t*
 }
 
 int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                 double* score, double* mu, double* sigma, double* linf) {
+                 double* score, double* mu, double* sigma, double* linf, const AcqFn* fn) {
   if (M <= 0) return 0;
   auto record = [&](int route, int nsplit, int grid) { h->score_route = route; h->score_nsplit = nsplit; h->score_grid = grid; };
   if (h->kp.use_linear) {
     record(VZGP_ROUTE_GENERAL, 0, 0);
-    return launch_score_general(h, Xs, Zs, M, acq, score, mu, sigma, linf);
+    return launch_score_general(h, Xs, Zs, M, acq, fn, score, mu, sigma, linf);
   }
   const int ntiles = (M + kTM - 1) / kTM;
   const int nblocks = (h->np + kBN - 1) / kBN;
@@ -726,7 +728,7 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
   if (ntiles <= small_tiles_max) {
     record(VZGP_ROUTE_SMALL, 0, 0);
     bool with_linf = false;
-    VZ_TRY(prepare_small_score(h, Xs, Zs, M, acq, score, mu, sigma, linf, &a, &with_linf));
+    VZ_TRY(prepare_small_score(h, Xs, Zs, M, acq, score, mu, sigma, linf, &a, &with_linf, fn));
     const int nvb = h->np / kVarCols, nmb = h->np / 64;
     const size_t sm1 = cross_small_smem_bytes(h->dc, h->dk), sm2 = var_small_smem_bytes();
     const dim3 g1(nmb, ntiles * 4), g2(nvb, ntiles);
@@ -754,7 +756,7 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
     const int want = h->score_i8 >= 0 ? h->score_i8 : env_i8;
     if (want && score_i8_eligible(h, M)) {
       record(VZGP_ROUTE_I8, 1, 0);   // launch_score_i8 records its grid
-      return launch_score_i8(h, Xs, Zs, M, acq, score, mu, sigma, linf);
+      return launch_score_i8(h, Xs, Zs, M, acq, score, mu, sigma, linf, fn);
     }
   }
   // Medium pools cannot fill the GPU with one CTA per tile: share each tile's output column
@@ -770,7 +772,9 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
     set_error("score kernel needs %zu bytes of shared memory (Dc=%d with trust-region distance)", sm, h->dc);
     return VZGP_ERR_UNSUPPORTED;
   }
-  const void* kfn = need_linf ? (const void*)k_score<true> : (const void*)k_score<false>;
+  const bool generic = !acq_fn_is_ucb(fn ? *fn : ucb_acq_fn(0.0));
+  const void* kfn = generic ? (need_linf ? (const void*)k_score<true, true> : (const void*)k_score<false, true>)
+                            : (need_linf ? (const void*)k_score<true, false> : (const void*)k_score<false, false>);
   VZ_TRY(raise_dyn_smem(kfn, sm));
   cudaLaunchAttribute cattr[1];
   cattr[0].id = cudaLaunchAttributeClusterDimension;
@@ -786,7 +790,7 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
   cfg.gridDim = dim3(grid);
   record(nsplit > 1 ? VZGP_ROUTE_SPLIT : VZGP_ROUTE_CLUSTER, nsplit, grid);
   VZ_TRY(ensure_scratch(h, (size_t)grid * kTM * h->np * sizeof(double)));
-  fill_score_args(h, Xs, Zs, M, acq, score, mu, sigma, linf, &a);
+  fill_score_args(h, Xs, Zs, M, acq, fn, score, mu, sigma, linf, &a);
   VZ_TRY(make_map(&a.mapA, a.scratch, (uint64_t)grid * kTM, (uint64_t)h->np, (uint64_t)h->np, kTM));
   VZ_TRY(make_map(&a.mapB, a.Linv, (uint64_t)h->np, (uint64_t)h->np, (uint64_t)h->np, kBPieceRows));
   a.nsplit = nsplit;
@@ -876,7 +880,7 @@ int launch_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const in
 struct StackCombine {
   int E;
   double alpha[16];
-  double coef;
+  AcqFn acq;
   int apply_tr, tr_strict;
   double radius;
 };
@@ -890,7 +894,7 @@ __global__ void k_stack_combine(int M, StackCombine p, const double* __restrict_
     mean += mu_e[(size_t)e * M + m];
     sd = pow(sd_e[(size_t)e * M + m], p.alpha[e]) * pow(sd, 1.0 - p.alpha[e]);
   }
-  double sc = fma(p.coef, sd, mean);
+  double sc = acq_value(p.acq, mean, sd);
   if (p.apply_tr) {
     const double dist = linf[m];
     const bool inside = (p.tr_strict ? (dist < p.radius) : (dist <= p.radius)) || (p.radius > 0.5);
@@ -902,7 +906,7 @@ __global__ void k_stack_combine(int M, StackCombine p, const double* __restrict_
 }
 
 int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const double* Xs, const int32_t* Zs, int M,
-                       const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf) {
+                       const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf, const AcqFn* fn) {
   if (M <= 0) return 0;
   vzgp_handle* top = hs[E - 1];
   VZ_TRY(top->pe_tmp.reserve(sizeof(double) * (2 * (size_t)E + 2) * (size_t)M));
@@ -920,7 +924,8 @@ int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, cons
     VZ_TRY(launch_score(hs[e], Xs, Zs, M, &none, dummy, mu_e + (size_t)e * M, sd_e + (size_t)e * M,
                         (e == E - 1 && want_linf) ? linf_buf : nullptr));
   StackCombine p;
-  p.E = E; p.coef = acq->ucb_coefficient; p.apply_tr = want_tr ? 1 : 0; p.tr_strict = acq->tr_strict ? 1 : 0;
+  p.E = E; p.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
+  p.apply_tr = want_tr ? 1 : 0; p.tr_strict = acq->tr_strict ? 1 : 0;
   p.radius = acq->trust_radius;
   for (int e = 0; e < 16; ++e) p.alpha[e] = e < E ? alphas[e] : 0.0;
   k_stack_combine<<<(M + 255) / 256, 256, 0, top->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma);
@@ -998,7 +1003,7 @@ int launch_set_pe_combine(vzgp_handle* h, int n_sets, int q, const vzgp_pe_param
 // ---------------------------------------------------------------------------
 struct EnsCombine {
   int E;
-  double coef;
+  AcqFn acq;
   int apply_tr, tr_strict;
   double radius;
 };
@@ -1017,7 +1022,7 @@ __global__ void k_ensemble_combine(int M, EnsCombine p, const double* __restrict
   double var = s2 / p.E - mean * mean;
   if (var < 0.0) { var = 0.0; atomicAdd(clamp_count, 1); }
   const double sd = sqrt(var);
-  double sc = fma(p.coef, sd, mean);
+  double sc = acq_value(p.acq, mean, sd);
   if (p.apply_tr) {
     const double dist = linf[m];
     const bool inside = (p.tr_strict ? (dist < p.radius) : (dist <= p.radius)) || (p.radius > 0.5);
@@ -1029,7 +1034,7 @@ __global__ void k_ensemble_combine(int M, EnsCombine p, const double* __restrict
 }
 
 int launch_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int M,
-                          const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf) {
+                          const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf, const AcqFn* fn) {
   if (M <= 0) return 0;
   vzgp_handle* h0 = hs[0];
   VZ_TRY(h0->pe_tmp.reserve(sizeof(double) * (2 * (size_t)E + 2) * (size_t)M));
@@ -1047,7 +1052,8 @@ int launch_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const
     VZ_TRY(launch_score(hs[e], Xs, Zs, M, &none, dummy, mu_e + (size_t)e * M, sd_e + (size_t)e * M,
                         (e == 0 && want_linf) ? linf_buf : nullptr));
   EnsCombine p;
-  p.E = E; p.coef = acq->ucb_coefficient; p.apply_tr = want_tr ? 1 : 0; p.tr_strict = acq->tr_strict ? 1 : 0;
+  p.E = E; p.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
+  p.apply_tr = want_tr ? 1 : 0; p.tr_strict = acq->tr_strict ? 1 : 0;
   p.radius = acq->trust_radius;
   k_ensemble_combine<<<(M + 255) / 256, 256, 0, h0->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma, h0->small.as<int>());
   VZ_CHECK_LAUNCH();

@@ -154,7 +154,7 @@ __device__ __forceinline__ void g_i8_t_tiles() {
 //   full[s]    TMA -> consumer: operand stage s has landed
 // nbuf = 2 overlaps the phases (digit scratch and phase-1 staging have their own memory); nbuf = 1 (large Dc:
 // the staging does not fit next to the operand ring) runs them back to back with the staging aliased onto the ring.
-template <bool WITH_LINF>
+template <bool WITH_LINF, bool GENERIC>
 __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constant__ I8Args ia) {
   const ScoreArgs& a = ia.s;
   extern __shared__ double smem_raw[];
@@ -480,7 +480,7 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
         const int r = etid, m = m0 + r;
         if (m < a.M) {
           const double rs = (s_red[r] + s_red[64 + r]) + (s_red[128 + r] + s_red[192 + r]);
-          emit_score(a, m, rs, s_mu[kb * 64 + r], s_linf[kb * 64 + r], clamped);
+          emit_score<GENERIC>(a, m, rs, s_mu[kb * 64 + r], s_linf[kb * 64 + r], clamped);
         }
       }
       esync();             // s_red and s_mu[kb] are consumed
@@ -546,7 +546,7 @@ bool score_i8_eligible(const vzgp_handle* h, int M) {
 }
 
 int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                    double* score, double* mu, double* sigma, double* linf) {
+                    double* score, double* mu, double* sigma, double* linf, const AcqFn* fn) {
   const int np = h->np;
   const int ntiles = (M + kTM - 1) / kTM;
   const int grid = ntiles < h->sm_count ? ntiles : h->sm_count;
@@ -571,7 +571,7 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
   a.Linv = h->Linv.as<double>(); a.ldi = np;
   a.alpha = h->alpha.as<double>();
   a.kp = h->kp; a.sn2 = h->sn2;
-  a.coef = acq->ucb_coefficient;
+  a.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
   a.apply_tr = acq->use_trust_region ? 1 : 0;
   a.tr_rows = (acq->tr_rows > 0 && acq->tr_rows < h->n_valid) ? acq->tr_rows : h->n_valid;
   a.tr_strict = acq->tr_strict ? 1 : 0;
@@ -604,13 +604,12 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
   const bool need_linf = (linf != nullptr) || (a.apply_tr && a.radius <= 0.5);
   const size_t sm = score_i8_smem_bytes(h->dc, h->dk, nbuf, plan.sb_bufs);
   if (sm > 227 * 1024) { set_error("k_score_i8 needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
-  if (need_linf) {
-    VZ_TRY(raise_dyn_smem((const void*)k_score_i8<true>, sm));
-    k_score_i8<true><<<grid, kI8Threads, sm, h->stream>>>(ia);
-  } else {
-    VZ_TRY(raise_dyn_smem((const void*)k_score_i8<false>, sm));
-    k_score_i8<false><<<grid, kI8Threads, sm, h->stream>>>(ia);
-  }
+  const bool generic = !acq_fn_is_ucb(a.acq);
+  const void* kfn = generic ? (need_linf ? (const void*)k_score_i8<true, true> : (const void*)k_score_i8<false, true>)
+                            : (need_linf ? (const void*)k_score_i8<true, false> : (const void*)k_score_i8<false, false>);
+  VZ_TRY(raise_dyn_smem(kfn, sm));
+  void* kargs[] = {&ia};
+  VZ_CUDA(cudaLaunchKernel(kfn, dim3(grid), dim3(kI8Threads), kargs, sm, h->stream));
   VZ_CHECK_LAUNCH();
   h->launches++;
   h->i8_launches++;

@@ -4,6 +4,7 @@
 #pragma once
 #include <cuda.h>
 
+#include "acq_fn.cuh"
 #include "async.cuh"
 #include "launchers.h"
 #include "tiles.cuh"
@@ -29,7 +30,6 @@ struct ScoreArgs {
   const double* alpha;
   KernelParams kp;
   double sn2;
-  double coef;
   int apply_tr;     // trust region modifies the score
   int tr_rows;      // trusted points = first tr_rows rows of X
   int tr_strict;    // inside test: dist < radius instead of <=
@@ -50,15 +50,17 @@ struct ScoreArgs {
   double* sigma;
   double* linf;
   int* clamp_count;
+  AcqFn acq;          // acquisition function of (mean, stddev)
 };
 
 // Final score from the reduced pieces (shared by the fused epilogue and the split finalize kernel).
+template <bool GENERIC = true>
 __device__ __forceinline__ void emit_score(const ScoreArgs& a, int m, double rs, double mean, double dist,
                                            int& clamped) {
   double var = a.kp.sf2 - rs + a.sn2;
   if (var < 0.0) { var = 0.0; ++clamped; }
   const double sd = sqrt(var);
-  double sc = fma(a.coef, sd, mean);
+  double sc = acq_eval<GENERIC>(a.acq, mean, sd);
   if (a.apply_tr) {
     const bool inside = (a.tr_strict ? (dist < a.radius) : (dist <= a.radius)) || (a.radius > 0.5);
     sc = inside ? sc : (-1e4 - dist);
@@ -76,7 +78,7 @@ __device__ __forceinline__ void emit_score(const ScoreArgs& a, int m, double rs,
 //   k_cross_small  grid (np/64, tiles): K* block [64 cand x 64 trials] -> scratch, partial mean / L-inf
 //   k_var_small    grid (np/16, tiles): W[:, 16 cols] = K*[:, 0:kext] Linv[16 rows, 0:kext]^T on the
 //                  DMMA pipe (cp.async ring), partial row sums of W^2
-//   k_small_finalize: fixed-order sums of the partials -> variance, UCB, trust region.
+//   k_small_finalize: fixed-order sums of the partials -> variance, acquisition, trust region.
 // All reductions have a fixed order: results are reproducible run to run.
 // ---------------------------------------------------------------------------
 constexpr int kSmallThreads = 256;
@@ -360,7 +362,7 @@ __device__ __forceinline__ void var_small_dispatch(const ScoreArgs& a, int b, in
 
 // EIGHT lanes per candidate m (lane group p = 0..7 sums partials p, p + 8, ... then a fixed shuffle tree):
 // deterministic, and a 25-candidate batch finalises in one pass of 200 threads.
-template <bool WITH_LINF>
+template <bool WITH_LINF, bool GENERIC = true>
 __device__ __forceinline__ void small_finalize_8(const ScoreArgs& a, int m, int p, bool active, int& clamped) {
   const int nvb = a.np / kVarCols, nmb = a.np / 64;
   double rs = 0.0, mean = 0.0, dist = INFINITY;
@@ -377,12 +379,14 @@ __device__ __forceinline__ void small_finalize_8(const ScoreArgs& a, int m, int 
     mean += __shfl_xor_sync(0xffffffffu, mean, o);
     if (WITH_LINF) dist = fmin(dist, __shfl_xor_sync(0xffffffffu, dist, o));
   }
-  if (active && p == 0) emit_score(a, m, rs, mean, dist, clamped);
+  if (active && p == 0) emit_score<GENERIC>(a, m, rs, mean, dist, clamped);
 }
 
 // Host side (score.cu): argument block + workspaces of the small-pool path for M candidates on `h`.
+// fn: the acquisition function (nullptr: UCB with acq->ucb_coefficient).
 int prepare_small_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                        double* score, double* mu, double* sigma, double* linf, ScoreArgs* a, bool* with_linf);
+                        double* score, double* mu, double* sigma, double* linf, ScoreArgs* a, bool* with_linf,
+                        const AcqFn* fn = nullptr);
 size_t cross_small_smem_bytes(int dc, int dk);
 size_t var_small_smem_bytes();
 

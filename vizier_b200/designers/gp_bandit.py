@@ -18,8 +18,11 @@ hyper-volume scalarisations, without a trust region.
 (general launch sequences: no captured graph, explicit K* for the scoring).
 `set_priors` trains a stack of residual GPs, one level per prior study plus the current study on top (gp_bandit.py:289-318;
 gp/gp_models.py:91-140, :245-300; gp/transfer_learning.py), scored through `vzgp_score_stack` (`gp.StackedGP`).
-Not implemented (the reference supports them; SURVEY 8f "next"): parallel (q-) acquisitions / custom scoring functions,
-non-independent multi-task kernels, priors for multi-metric or ensemble models; each raises NotImplementedError
+`scoring_function_factory` (e.g. `acquisitions.bayesian_scoring_function_factory(lambda d: EI(get_best_labels(d.labels)))`
+or `AcquisitionTrustRegion.default_ucb_pi`) selects UCB, LCB, EI, PI or a thresholded pair of those; the device
+scoring kernels evaluate it (`acquisitions.lower_acquisition`).  Multi-metric problems keep their scalarised UCB.
+Not implemented (the reference supports them; SURVEY 8f "next"): parallel (q-) acquisitions, other acquisition
+functions (MaxValueEntropySearch, Sample, user callables), non-independent multi-task kernels, priors for multi-metric or ensemble models; each raises NotImplementedError
 instead of silently doing something else.  Categorical parameters ARE supported
 end to end.  `padding_schedule` is accepted and has no numerical effect here: the kernels take
 explicit sizes (`n_valid`, Dc, Dk) instead of padded shapes + masks, which is what the reference's
@@ -108,8 +111,8 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     self._ensemble_size = int(ensemble_size or 1)
     if self._ensemble_size < 1 or self._ensemble_size > ard_random_restarts:
       raise ValueError('ensemble_size must be in [1, ard_random_restarts].')
-    if scoring_function_is_parallel or scoring_function_factory is not None:
-      raise NotImplementedError('custom / parallel scoring functions are not implemented (UCB only).')
+    if scoring_function_is_parallel:
+      raise NotImplementedError('parallel (q-) scoring functions are not implemented.')
     if self._n_metrics > 1 and self._ensemble_size > 1:
       raise NotImplementedError('ensembles of multi-metric models are not implemented.')
     del padding_schedule, multitask_type
@@ -121,12 +124,18 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     self._ard_random_restarts = ard_random_restarts
     self._num_seed_trials = num_seed_trials
     self._use_trust_region = use_trust_region and self._n_metrics == 1   # gp_bandit.py:241
+    # gp_bandit.py:206-260: multi-metric problems override the factory with scalarised UCB; a single-metric one is
+    # validated now on empty data, so an acquisition the device cannot evaluate fails at construction.
+    self._scoring_function_factory = scoring_function_factory if self._n_metrics == 1 else None
     self._ucb_coefficient = ucb_coefficient
     self._metadata_ns = 'oss_gp_bandit'
     self._output_warper = output_warper or output_warpers.create_default_warper()
     self._rng = np.random.default_rng(_seed_from(rng))
     self._converter = converters.TrialToModelInputConverter.from_problem(problem)
     self._acquisition_optimizer = acquisition_optimizer_factory(self._converter)
+    if self._scoring_function_factory is not None:
+      empty = acq_lib.ModelData(features=None, labels=acq_lib.PaddedArray.as_padded(np.zeros((0, self._n_metrics))))
+      acq_lib.check_supported(self._scoring_function(empty).acquisition_fn)
     # Scalarisation weights are drawn once per designer (gp_bandit.py:217-222: one weights_rng): |N(0,1)|,
     # rows normalised to unit L2 norm (acquisitions.py:585-589).
     self._scal_weights = None
@@ -255,17 +264,31 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
       dev.fit(cont, y, self._last_params, z=z)
     return dev
 
-  def _acquisition(self, n_obs: int, labels: Optional[np.ndarray] = None):
+  def _scoring_function(self, data):
+    sf = self._scoring_function_factory(
+        data, None, self._converter.continuous_feasible_values(_MAX_NUM_FEASIBLE_VALUES_FOR_TRUST_REGION),
+        self._use_trust_region)
+    if not isinstance(sf, acq_lib.BayesianScoringFunction):
+      raise NotImplementedError(f'scoring function {type(sf).__name__} is not implemented on the device '
+                                '(use acquisitions.bayesian_scoring_function_factory)')
+    return sf
+
+  def _acquisition(self, n_obs: int, labels: Optional[np.ndarray] = None, features=None):
     if self._n_metrics > 1:
       # gp_bandit.py:217-239: HV scalarisation around the reference point of the (warped) labels, floored
       # at the best scalarised value observed so far
       ref = acq_lib.hv_reference_point(labels, self._ref_scaling)
       best = acq_lib.hv_scalarize(labels, self._scal_weights, ref).max(axis=-1)
       return gp.ScalarizedUcbAcquisition(self._scal_weights, ref, best, self._ucb_coefficient)
-    return acq_lib.make_acquisition(
+    acq = acq_lib.make_acquisition(
         n_obs, self._converter.continuous_feasible_values(_MAX_NUM_FEASIBLE_VALUES_FOR_TRUST_REGION),
         self._converter.n_continuous, self._converter.n_categorical, use_trust_region=self._use_trust_region,
         ucb_coefficient=self._ucb_coefficient)
+    if self._scoring_function_factory is not None:
+      # gp_bandit.py:497-505: the factory sees the (warped) labels of this suggest
+      data = acq_lib.ModelData(features=features, labels=acq_lib.PaddedArray.as_padded(labels))
+      acq.acq_fn = acq_lib.lower_acquisition(self._scoring_function(data).acquisition_fn)
+    return acq
 
   @profiler.record_runtime
   def _optimize_acquisition(self, dev: gp.DeviceGP, acq: gp.Acquisition, count: int, features=None):
@@ -302,7 +325,7 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     start = datetime.datetime.now()
     cont, cat, labels = self._trials_to_data(self._trials)
     dev = self._update_gp(cont, cat, labels)
-    acq = self._acquisition(cont.shape[0], labels)
+    acq = self._acquisition(cont.shape[0], labels, features=(cont, cat))
     best = self._optimize_acquisition(dev, acq, count, features=(cont, cat))
     out = []
     for t in best:

@@ -101,9 +101,43 @@ def param_bounds(dc: int, dk: int, linear: bool = False) -> tuple[np.ndarray, np
   return lo, hi
 
 
+@dataclasses.dataclass(frozen=True)
+class AcqTermSpec:
+  """One pointwise acquisition of (mean, stddev); see vzgp_acq_term in include/vzgp.h."""
+
+  kind: int                    # _lib.ACQ_UCB / ACQ_LCB / ACQ_EI / ACQ_PI
+  coefficient: float = 0.0     # UCB / LCB
+  best_label: float = 0.0      # EI / PI
+  exploration: float = 0.0     # EI / PI
+
+  def _c(self) -> '_lib.AcqTerm':
+    return _lib.AcqTerm(int(self.kind), float(self.coefficient), float(self.best_label), float(self.exploration))
+
+
+@dataclasses.dataclass(frozen=True)
+class AcqFnSpec:
+  """Acquisition function a handle scores with (vzgp_set_acquisition): `main`, or with `thresholding` set the
+  AcquisitionTrustRegion rule (acquisitions.py:466-492): bad_acq_value - t where t = thresholding < threshold."""
+
+  main: AcqTermSpec
+  thresholding: Optional[AcqTermSpec] = None
+  threshold: float = 0.0
+  bad_acq_value: float = -1e4
+
+  def _c(self) -> '_lib.AcqFn':
+    f = _lib.AcqFn()
+    f.main = self.main._c()
+    f.use_threshold = 1 if self.thresholding is not None else 0
+    f.thresholding = (self.thresholding or self.main)._c()
+    f.threshold = float(self.threshold)
+    f.bad_acq_value = float(self.bad_acq_value)
+    return f
+
+
 @dataclasses.dataclass
 class Acquisition:
-  """UCB coefficient + trust region (acquisitions.py:213-225, :691-820)."""
+  """UCB coefficient + trust region (acquisitions.py:213-225, :691-820).  `acq_fn` (acquisitions.lower_acquisition)
+  replaces UCB by another acquisition function of (mean, stddev); None scores UCB with `ucb_coefficient`."""
 
   ucb_coefficient: float = 1.8
   use_trust_region: bool = True
@@ -111,6 +145,7 @@ class Acquisition:
   tr_dim_mask: Optional[np.ndarray] = None  # bool [Dc]
   tr_rows: int = 0          # trusted points = first tr_rows rows of the model's X (0 = all)
   tr_strict: bool = False   # dist < radius (gp_ucb_pe.py) instead of dist <= radius (acquisitions.py)
+  acq_fn: Optional[AcqFnSpec] = None
 
   def _c(self):
     a = _lib.Acq()
@@ -206,6 +241,18 @@ class DeviceGP:
     self.dc = self.dk = self.n = 0
     self.n_metrics = 1
     self.cholesky_failed = False
+    self._acq_fn: Optional[AcqFnSpec] = None   # what vzgp_set_acquisition last gave the handle
+
+  def set_acquisition(self, fn: Optional[AcqFnSpec]) -> None:
+    """Acquisition function of the later scoring and Eagle calls on this handle (None: UCB)."""
+    c = fn._c() if fn is not None else None
+    _lib.check('vzgp_set_acquisition', self._lib.vzgp_set_acquisition(self._h, C.byref(c) if c is not None else None))
+    self._acq_fn = fn
+
+  def _use_acq(self, acq) -> None:
+    fn = acq.acq_fn if isinstance(acq, Acquisition) else None
+    if fn != self._acq_fn:
+      self.set_acquisition(fn)
 
   def close(self):
     if getattr(self, '_h', None):
@@ -483,6 +530,7 @@ class DeviceGP:
         for k in ('mean', 'stddev', 'linf_distance'):
           res[k] = torch.empty((m,), dtype=torch.float64, device=self.device)
       self._stream.wait_stream(torch.cuda.current_stream(self.device))
+    self._use_acq(acq)
     a, keep = acq._c()
     _lib.check('vzgp_score', self._lib.vzgp_score(
         self._h, _ptr(xst), _ptr(zst), m, C.byref(a), _ptr(res['score']), _ptr(res.get('mean')),
@@ -513,6 +561,7 @@ class DeviceGP:
   def score_host(self, xs: np.ndarray, acq: Acquisition, *, score_out: np.ndarray,
                  zs: Optional[np.ndarray] = None, mean_out=None, stddev_out=None, linf_out=None):
     """HOST buffers in, HOST buffers out (pinned memory recommended).  Synchronous."""
+    self._use_acq(acq)
     a, keep = acq._c()
     m = xs.shape[0]
 
@@ -550,6 +599,7 @@ class DeviceGP:
 
   def score_topk(self, xs: torch.Tensor, acq: Acquisition, count: int, score_out: Optional[torch.Tensor] = None):
     """Score device candidates, select the top `count`, return (features, scores, indices) on the host."""
+    self._use_acq(acq)
     a, keep = acq._c()
     m = xs.shape[0]
     bx = np.zeros((count, self.dc), np.float64)
@@ -569,6 +619,7 @@ class DeviceGP:
     a NumPy array) in one synchronous C call; `exchange` is a `multi_gpu.PeerExchange` (None = this rank
     alone).  Returns (global indices [count] i64, scores [count], features [count, Dc]) - the same on
     every rank."""
+    self._use_acq(acq)
     a, keep = acq._c()
     m = xs_host.shape[0]
     rows = np.zeros((count, self.dc + 2), np.float64)
@@ -589,6 +640,7 @@ class DeviceGP:
                       payload: torch.Tensor, score_out: Optional[torch.Tensor] = None) -> None:
     """Asynchronous shard step: score, local top-`count`, rows [score, global index, features] into the
     device tensor `payload` [count, Dc+2].  No host synchronisation (multi_gpu.TopkExchange)."""
+    self._use_acq(acq)
     a, keep = acq._c()
     assert payload.is_cuda and payload.dtype == torch.float64 and payload.shape == (count, self.dc + 2)
     self._stream.wait_stream(torch.cuda.current_stream(self.device))
@@ -625,6 +677,7 @@ class DeviceGP:
 
   def random_search(self, m: int, acq: Acquisition, count: int, seed: int, index_base: int = 0, cat_sizes=None):
     """Returns (best_x [count,Dc], best_z [count,Dk], best_score [count], best_index [count])."""
+    self._use_acq(acq)
     a, keep = acq._c()
     bx = np.zeros((count, self.dc), np.float64)
     bz = np.zeros((count, self.dk), np.int32)
@@ -680,6 +733,8 @@ class DeviceGP:
     if isinstance(acq, UcbPeAcquisition):
       return self._eagle_run_pe(cfg, acq, count, seed, prior, prior_z, cat_sizes, other)
     multi = isinstance(acq, ScalarizedUcbAcquisition)
+    if not multi:
+      self._use_acq(acq)
     a, keep = acq._c()
     n_prior = 0 if prior is None else len(prior)
     pt = self._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
@@ -804,6 +859,7 @@ class StackedGP:
       for k in ('mean', 'stddev', 'linf_distance'):
         res[k] = torch.empty((m,), dtype=torch.float64, device=f.device)
     f._stream.wait_stream(torch.cuda.current_stream(f.device))
+    self.levels[0]._use_acq(acq)          # multi-handle calls take the acquisition of hs[0]
     a, keep = acq._c()
     _lib.check('vzgp_score_stack', f._lib.vzgp_score_stack(
         self._handles(), len(self.levels), self._alphas(), _ptr(xst), _ptr(zst), m, C.byref(a), _ptr(res['score']),
@@ -814,6 +870,7 @@ class StackedGP:
   def eagle_run(self, cfg, acq: Acquisition, count: int, seed: int, prior=None, prior_z=None, cat_sizes=None, other=None):
     assert other is None
     f = self.levels[-1]
+    self.levels[0]._use_acq(acq)
     a, keep = acq._c()
     n_prior = 0 if prior is None else len(prior)
     pt = f._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
@@ -954,6 +1011,7 @@ class EnsembleGP:
     if with_aux:
       for k in ('mean', 'stddev', 'linf_distance'):
         res[k] = torch.empty((m,), dtype=torch.float64, device=self.device)
+    f._use_acq(acq)                       # multi-handle calls take the acquisition of hs[0]
     a, keep = acq._c()
     _lib.check('vzgp_score_ensemble', self._lib.vzgp_score_ensemble(
         self._handles(), len(self.members), _ptr(xst), _ptr(zst), m, C.byref(a), _ptr(res['score']),
@@ -965,6 +1023,7 @@ class EnsembleGP:
                 other=None):
     assert other is None
     f = self.members[0]
+    f._use_acq(acq)
     a, keep = acq._c()
     n_prior = 0 if prior is None else len(prior)
     pt = f._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None

@@ -231,9 +231,12 @@ class VectorizedOptimizer:
         'linf_distance': out['linf_distance'].cpu().numpy(),
         'radius': np.full(count, acq.trust_radius),
     }
-    aux['raw_acquisition'] = aux['mean'] + acq.ucb_coefficient * aux['stddev']
     if not acq.use_trust_region:
-      aux = {}
+      return VectorizedStrategyResults(bx, bs, {}, categorical=bz)
+    # the acquisition before the trust region, evaluated by the same device epilogue as the scores
+    raw = dev.score(bx, dataclasses.replace(acq, use_trust_region=False), zs=bz if self.n_categorical else None)
+    dev.synchronize()
+    aux['raw_acquisition'] = raw['score'].cpu().numpy()
     return VectorizedStrategyResults(bx, bs, aux, categorical=bz)
 
 
