@@ -7,7 +7,8 @@ runs the k_score<true> instance (L-inf distance); bench.py times that instance a
 Counters are summed over all CTAs and reported per tile: phase 1 (K* tile), the gate after it, phase 2
 (DMMA slab stream), the whole tile (all of math warp 0), the average math warp's wait on the full
 barriers (ring starved: operand feed too slow) and the producer's wait on the empty barriers (ring full:
-the math warps are the limit)."""
+the math warps are the limit).  Phase 1 is split into the d2 loop, Matern + mu, the scratch stores and
+the barrier / cp.async waits (math warp 0)."""
 import ctypes as C
 import json
 import sys
@@ -18,6 +19,7 @@ sys.path.insert(0, '.')
 from vizier_b200 import _lib, gp  # noqa: E402
 
 MATH_WARPS = 16
+COUNTERS = 11
 
 
 def main():
@@ -35,7 +37,7 @@ def main():
   acq = gp.Acquisition(1.8, True, 0.3) if '--trust-region' in sys.argv else gp.Acquisition(1.8, False, 0.0)
   lib = _lib.load()
   lib.vzgp_debug_score_timing.restype = C.c_int
-  buf = (C.c_ulonglong * 8)()
+  buf = (C.c_ulonglong * COUNTERS)()
   out = None
   for p in pools[:2]:
     out = dev.score(p, acq, out=out)
@@ -52,7 +54,9 @@ def main():
   t = np.array(buf[:], dtype=np.float64)
   tiles = max(t[0], 1.0)
   per_tile = {'phase1': t[1] / tiles, 'gate': t[3] / tiles, 'phase2': t[2] / tiles, 'tile': t[4] / tiles,
-              'full_wait_per_math_warp': t[5] / MATH_WARPS / tiles, 'empty_wait_producer': t[6] / tiles}
+              'full_wait_per_math_warp': t[5] / MATH_WARPS / tiles, 'empty_wait_producer': t[6] / tiles,
+              'phase1_d2': t[7] / tiles, 'phase1_matern_mu': t[8] / tiles, 'phase1_stores': t[9] / tiles,
+              'phase1_waits': t[10] / tiles}
   res = {'ms_per_pass': e0.elapsed_time(e1) / passes, 'tiles_per_pass': tiles / passes,
          'cycles_per_tile': {k: int(round(v)) for k, v in per_tile.items()},
          'full_wait_share_of_phase2': round(per_tile['full_wait_per_math_warp'] / max(per_tile['phase2'], 1.0), 4),

@@ -28,6 +28,7 @@
 #include <tuple>
 
 #include "launchers.h"
+#include "matern_fast.cuh"
 #include "score_small.cuh"
 #include "topk_merge.cuh"
 #include "tiles.cuh"
@@ -61,7 +62,9 @@ static_assert(kBPieces % 2 == 0 && kBN % (kBPieces / 2) == 0, "B pieces tile the
 // Instrumented build only (make timing): clock64 sums over all CTAs, read by vzgp_debug_score_timing.
 // [0] tiles  [1] phase 1  [2] phase 2  [3] tile gate (barrier after phase 1)  [4] whole tile   (math warp 0)
 // [5] math warps waiting on full barriers (summed over the 16 warps)  [6] producer waiting on empty barriers
-__device__ unsigned long long g_score_t[8];
+// phase 1, math warp 0: [7] d2 loop  [8] Matern + mu  [9] scratch stores  [10] barrier and cp.async waits
+constexpr int kScoreCounters = 11;
+__device__ unsigned long long g_score_t[kScoreCounters];
 #define VZ_ST(...) __VA_ARGS__
 #else
 #define VZ_ST(...)
@@ -120,6 +123,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   auto consumer_sync = [&]() { asm volatile("bar.sync 1, %0;\n" ::"n"(kThreads) : "memory"); };
   // Counters: sums over the tiles that hold candidates (the all-padding tile of a last round is left out).
   VZ_ST(long long t_p1 = 0, t_gate = 0, t_p2 = 0, t_tile = 0, t_wait = 0, w_tile = 0, n_tiles = 0;)
+  VZ_ST(long long t_d2 = 0, t_mat = 0, t_st = 0, t_sync = 0;)
 
   const int ntiles = (a.M + kTM - 1) / kTM;
   const int nblocks = (np + kBN - 1) / kBN;
@@ -202,6 +206,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     stage_trials(0, 0);
     cp_async_commit();
     for (int jb = 0; jb < nj; ++jb) {
+      VZ_ST(long long tc = clock64();)
       const int buf = jb & 1;
       if (jb + 1 < nj) stage_trials(jb + 1, buf ^ 1);   // buffer buf^1 was released by the barrier below
       cp_async_commit();
@@ -211,6 +216,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
         stage_rows_T_i32(a.Z, np, dk, jb * 64, 64, zb, LD, kThreads);
         consumer_sync();
       }
+      VZ_ST(t_sync += clock64() - tc; tc = clock64();)
       const double* sbj = sb + buf * dc * LD;
       const double* alj = s_alpha + buf * 64;
       double d2[2][4], lf[2][4];
@@ -253,22 +259,34 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
           for (int j = 0; j < 4; ++j) d2[i][j] += (avz != zb[k * LD + GP1::col_of(tx, j)]) ? w : 0.0;
         }
       }
+      VZ_ST(t_d2 += clock64() - tc; tc = clock64();)
+      // The eight kernel values as one straight-line block of the branch-free Matern (independent chains
+      // the scheduler can interleave); columns at or past n_valid are zeroed by a select.
+      double kv[2][4];
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        double kv[4];
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) kv[i][j] = matern52_fast(d2[i][j], a.kp.sf2);
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const int cj = GP1::col_of(tx, j);
-          const bool valid = (jb * 64 + cj) < a.n_valid;
-          kv[j] = valid ? matern52(d2[i][j], a.kp.sf2) : 0.0;
-          mu_part[i] = fma(kv[j], alj[cj], mu_part[i]);
+          kv[i][j] = (jb * 64 + cj) < a.n_valid ? kv[i][j] : 0.0;
+          mu_part[i] = fma(kv[i][j], alj[cj], mu_part[i]);
           if (WITH_LINF && (jb * 64 + cj) < a.tr_rows) lmin[i] = fmin(lmin[i], lf[i][j]);
         }
+      VZ_ST(t_mat += clock64() - tc; tc = clock64();)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
         double* dst = scr + (size_t)GP1::row_of(ty, i) * np + jb * 64;
-        *reinterpret_cast<double2*>(dst + GP1::col_of(tx, 0)) = make_double2(kv[0], kv[1]);
-        *reinterpret_cast<double2*>(dst + GP1::col_of(tx, 2)) = make_double2(kv[2], kv[3]);
+        *reinterpret_cast<double2*>(dst + GP1::col_of(tx, 0)) = make_double2(kv[i][0], kv[i][1]);
+        *reinterpret_cast<double2*>(dst + GP1::col_of(tx, 2)) = make_double2(kv[i][2], kv[i][3]);
       }
+      VZ_ST(t_st += clock64() - tc;)
+      VZ_ST(tc = clock64();)
       consumer_sync();  // everyone is done with buffer `buf` (and zb) before it is refilled
+      VZ_ST(t_sync += clock64() - tc;)
     }
     cp_async_wait<0>();
 #pragma unroll
@@ -399,6 +417,10 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
         atomicAdd(&g_score_t[2], (unsigned long long)t_p2);
         atomicAdd(&g_score_t[3], (unsigned long long)t_gate);
         atomicAdd(&g_score_t[4], (unsigned long long)t_tile);
+        atomicAdd(&g_score_t[7], (unsigned long long)t_d2);
+        atomicAdd(&g_score_t[8], (unsigned long long)t_mat);
+        atomicAdd(&g_score_t[9], (unsigned long long)t_st);
+        atomicAdd(&g_score_t[10], (unsigned long long)t_sync);
       }
     }
   }
@@ -1219,7 +1241,7 @@ int launch_merge_topk(vzgp_handle* h, const double* rows, int n_rows, int width,
 extern "C" int vzgp_debug_score_timing(unsigned long long* out, int reset) {
   if (cudaMemcpyFromSymbol(out, vzgp::g_score_t, sizeof(vzgp::g_score_t)) != cudaSuccess) return -2;
   if (reset) {
-    unsigned long long z[8] = {};
+    unsigned long long z[vzgp::kScoreCounters] = {};
     if (cudaMemcpyToSymbol(vzgp::g_score_t, z, sizeof(z)) != cudaSuccess) return -2;
   }
   return 0;
