@@ -18,7 +18,7 @@ import torch
 sys.path.insert(0, '.')
 from vizier_b200 import _lib, gp  # noqa: E402
 
-MATH_WARPS = 16
+MATH_WARPS = 8
 COUNTERS = 11
 
 

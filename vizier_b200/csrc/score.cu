@@ -18,6 +18,10 @@
 //            exploiting that Linv is lower triangular (k <= j, all-zero fragments skipped); each block
 //            is squared and row-summed in registers, W is never stored.  Large pools run in 2-CTA
 //            clusters that multicast each Linv box to both CTAs.
+//            Eight math warps (2 (M) x 4 (N), a 32 x 32 block each) and the producer warp: 288 threads.
+//            One SM sub-partition holds 3 of the 9 warps, which caps the kernel at 168 registers; the
+//            64 accumulator registers of a warp tile fit without spills because K* is stored in row-pair
+//            order (no register moves to form the A fragments) and the k-group loop is not unrolled.
 //   epilogue var = sf2 + sn2 - sum W^2 (clamped at 0), sigma, UCB, trust region, outputs.
 #include <cuda.h>
 
@@ -35,20 +39,29 @@
 
 namespace vzgp {
 
-using GP1 = GemmCfg<64, 64, 16, 2, 4>;  // phase-1 thread mapping: 512 threads, 2x4 outputs each
-constexpr int kThreads = 512;        // consumer threads (16 math warps)
-constexpr int kBlockThreads = 544;   // + one TMA producer warp
+using GP1 = GemmCfg<64, 64, 16, 4, 4>;  // phase-1 thread mapping: 256 threads, 4x4 outputs each
+constexpr int kThreads = 256;        // consumer threads (8 math warps)
+constexpr int kBlockThreads = 288;   // + one TMA producer warp
+static_assert(GP1::kThreads == kThreads, "phase 1 maps one d2 block to every math thread");
 
 // Phase-2 tiling: 64 candidates x 128 output columns per pass, k-slabs of 32, 4-stage TMA ring.
-// 16 warps as 4 (M) x 4 (N): each warp owns a 16 x 32 block = 2 x 4 DMMA tiles.
+// 8 warps as 2 (M) x 4 (N): each warp owns a 32 x 32 block = 2 x 4 m16n8 DMMA tiles.
 constexpr int kBN = 128;         // output columns per pass
-constexpr int kBK = 32;          // k-slab = two TMA boxes of 16 doubles (one 128-byte swizzle atom per row)
+constexpr int kBK = 32;          // k-slab = 32 columns of K* and Linv
 constexpr int kStages = 4;
-// One stage: A half0 | A half1 | B half0 | B half1, each a dense [rows][16] box written by TMA with
-// the 128-byte swizzle (16-byte chunk c of row r lands at chunk c ^ (r & 7)).
-constexpr int kAHalf = kTM * 16;                 // doubles
+// K* is stored in row-pair order so that one 16-byte load gives two A-fragment registers in the order
+// m16n8k8 wants them.  Pair p of a tile holds rows 16 (p / 8) + p % 8 and that + 8 (rows fr and fr + 8
+// of one A fragment); in the scratch a pair is one row of 2 np doubles, [k][2 rows], and in shared memory
+// pair position 2p + e stands for row pair_row(2p + e).
+__host__ __device__ constexpr int pair_pos(int r) { return (((r >> 4) * 8 + (r & 7)) << 1) | ((r >> 3) & 1); }
+__host__ __device__ constexpr int pair_row(int pos) { return ((pos >> 4) << 4) + ((pos >> 1) & 7) + ((pos & 1) << 3); }
+static_assert(pair_row(pair_pos(13)) == 13 && pair_row(pair_pos(58)) == 58 && pair_pos(8) == 1, "pair order round trip");
+// One stage: A box 0..3 | B half0 | B half1, each a dense [rows][16] box written by TMA with the 128-byte
+// swizzle (16-byte chunk c of row r lands at chunk c ^ (r & 7)).  A box h: k group h of the slab, 32 row
+// pairs x 8 k x 2 rows.  B half: 128 Linv rows x 16 k.
+constexpr int kABox = (kTM / 2) * 16;            // doubles
 constexpr int kBHalf = kBN * 16;
-constexpr int kStageDoubles = 2 * (kAHalf + kBHalf);   // 6144 doubles = 48 KB
+constexpr int kStageDoubles = 4 * kABox + 2 * kBHalf;   // 6144 doubles = 48 KB
 constexpr unsigned kStageBytes = kStageDoubles * sizeof(double);
 // Large pools run in clusters of kCluster CTAs on adjacent tiles.  They walk the same slab sequence, so
 // every Linv box is loaded from L2 once per cluster: the B operand of a stage is split into kBPieces
@@ -61,7 +74,7 @@ static_assert(kBPieces % 2 == 0 && kBN % (kBPieces / 2) == 0, "B pieces tile the
 #ifdef VZ_SCORE_TIMING
 // Instrumented build only (make timing): clock64 sums over all CTAs, read by vzgp_debug_score_timing.
 // [0] tiles  [1] phase 1  [2] phase 2  [3] tile gate (barrier after phase 1)  [4] whole tile   (math warp 0)
-// [5] math warps waiting on full barriers (summed over the 16 warps)  [6] producer waiting on empty barriers
+// [5] math warps waiting on full barriers (summed over the 8 warps)  [6] producer waiting on empty barriers
 // phase 1, math warp 0: [7] d2 loop  [8] Matern + mu  [9] scratch stores  [10] barrier and cp.async waits
 constexpr int kScoreCounters = 11;
 __device__ unsigned long long g_score_t[kScoreCounters];
@@ -90,20 +103,20 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   double* s_linf = s_mu + 64;                            // [64]
   double* s_rowsq = s_linf + 64;                         // [4][64]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_rowsq + 256);  // [kStages] TMA bytes landed
-  uint64_t* empty_bar = full_bar + kStages;                         // [kStages] all 16 math warps of every CTA in the cluster released the stage
+  uint64_t* empty_bar = full_bar + kStages;                         // [kStages] all 8 math warps of every CTA in the cluster released the stage
   int32_t* za = reinterpret_cast<int32_t*>(full_bar + 8);  // [dk][LD]
   int32_t* zb = za + dk * LD;                            // [dk][LD]
   uint8_t* s_mask = reinterpret_cast<uint8_t*>(zb + dk * LD);  // [kMaxDc]
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int ty = tid / 16, tx = tid % 16;      // phase-1 mapping (32 x 16 threads)
-  const int wm = warp & 3, wn = warp >> 2;     // phase-2 warp grid 4 (M) x 4 (N)
+  const int ty = tid / 16, tx = tid % 16;      // phase-1 mapping (16 x 16 threads)
+  const int wm = warp & 1, wn = warp >> 1;     // phase-2 warp grid 2 (M) x 4 (N)
   const int fr = lane >> 2, fk = lane & 3;     // fragment row / k within a DMMA tile
-  // Tile row (A: candidate, B: output column) that fragment row fr stands for within its 8-row group.
-  // An LDS.128 is served 8 lanes at a time; lanes 0-7 are fragment rows 0 and 1.  With the 128-byte
-  // swizzle rows r and r^1 keep their chunks in the same 64-byte half, a 2-way bank conflict on every
-  // operand load; rows r and r^4 land in opposite halves.  So fr = 2i, 2i+1 read rows i, i+4.  Row sums
-  // do not care which row a fragment row holds (the k mapping, which A and B must share, is unchanged).
+  // Linv row (output column) that B fragment row fr stands for within its 8-row group.  An LDS.128 is
+  // served 8 lanes at a time; lanes 0-7 are fragment rows 0 and 1.  With the 128-byte swizzle rows r and
+  // r^1 keep their chunks in the same 64-byte half, a 2-way bank conflict on every operand load; rows r
+  // and r^4 land in opposite halves.  So fr = 2i, 2i+1 read rows i, i+4.  Row sums do not care which
+  // column a fragment row holds.  (A, in pair order, reads even and odd chunks and needs no remapping.)
   const int pr = ((fr & 1) << 2) | (fr >> 1);
   double* scr = a.scratch + (size_t)blockIdx.x * kTM * np;
   // Cluster of ncta CTAs (1 for medium pools, which split a tile's blocks between CTAs, else kCluster).
@@ -160,11 +173,11 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
             double* base = ring + stage * kStageDoubles;
             const int k0 = ks * kBK;
             mbar_expect_tx(full_bar + stage, kStageBytes);   // own A boxes + the B pieces of every CTA
-            tma_load_2d(base, &a.mapA, k0, (int)blockIdx.x * kTM, full_bar + stage);
-            tma_load_2d(base + kAHalf, &a.mapA, k0 + 16, (int)blockIdx.x * kTM, full_bar + stage);
+            for (int h = 0; h < 4; ++h)
+              tma_load_2d(base + h * kABox, &a.mapA, 2 * k0 + 16 * h, (int)blockIdx.x * (kTM / 2), full_bar + stage);
             for (int p = (int)crank; p < kBPieces; p += (int)ncta) {   // rows >= np: zero fill
               const int half = p / (kBPieces / 2), r0 = (p % (kBPieces / 2)) * kBPieceRows;
-              double* dst = base + 2 * kAHalf + half * kBHalf + r0 * 16;
+              double* dst = base + 4 * kABox + half * kBHalf + r0 * 16;
               if (ncta > 1) tma_load_2d_multicast(dst, &a.mapB, k0 + 16 * half, jb * kBN + r0, full_bar + stage, cmask);
               else tma_load_2d(dst, &a.mapB, k0 + 16 * half, jb * kBN + r0, full_bar + stage);
             }
@@ -178,12 +191,12 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     }
     VZ_ST(const long long t_tile0 = clock64(); w_tile = 0;)
     consumer_sync();  // previous tile fully consumed by the math warps (sa, s_mu, s_rowsq, ring)
-    // candidate tile, transposed; scaled by 1/ls like the reference's FeatureScaled kernel
+    // candidate tile, transposed and in pair order; scaled by 1/ls like the reference's FeatureScaled kernel
     for (int e = tid; e < kTM * dc; e += kThreads) {
       const int r = e / dc, d = e - r * dc;
       const int gr = m0 + r;
       const double v = gr < a.M ? __ldg(a.Xs + (size_t)gr * dc + d) : 0.0;
-      sa[d * LD + r] = WITH_LINF ? v : v * a.kp.inv_ls_c[d];
+      sa[d * LD + pair_pos(r)] = WITH_LINF ? v : v * a.kp.inv_ls_c[d];
     }
     if (dk > 0) stage_rows_T_i32(a.Zs, a.M, dk, m0, kTM, za, LD, kThreads);
 
@@ -199,9 +212,9 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       }
       if (tid < 32) cp_async16(s_alpha + buf * 64 + tid * 2, a.alpha + jb * 64 + tid * 2, true);
     };
-    double mu_part[2], lmin[2];
+    double mu_part[4], lmin[4];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) { mu_part[i] = 0.0; lmin[i] = INFINITY; }
+    for (int i = 0; i < 4; ++i) { mu_part[i] = 0.0; lmin[i] = INFINITY; }
     const int nj = np / 64;
     stage_trials(0, 0);
     cp_async_commit();
@@ -219,21 +232,22 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       VZ_ST(t_sync += clock64() - tc; tc = clock64();)
       const double* sbj = sb + buf * dc * LD;
       const double* alj = s_alpha + buf * 64;
-      double d2[2][4], lf[2][4];
+      double d2[4][4], lf[4][4];
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
+      for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) { d2[i][j] = 0.0; lf[i][j] = 0.0; }
       for (int d = 0; d < dc; ++d) {
-        const double2 av = *reinterpret_cast<const double2*>(sa + d * LD + GP1::row_of(ty, 0));
+        const double2 a0 = *reinterpret_cast<const double2*>(sa + d * LD + GP1::row_of(ty, 0));
+        const double2 a1 = *reinterpret_cast<const double2*>(sa + d * LD + GP1::row_of(ty, 2));
         const double2 b0 = *reinterpret_cast<const double2*>(sbj + d * LD + GP1::col_of(tx, 0));
         const double2 b1 = *reinterpret_cast<const double2*>(sbj + d * LD + GP1::col_of(tx, 2));
-        const double aa[2] = {av.x, av.y}, bb[4] = {b0.x, b0.y, b1.x, b1.y};
+        const double aa[4] = {a0.x, a0.y, a1.x, a1.y}, bb[4] = {b0.x, b0.y, b1.x, b1.y};
         if (WITH_LINF) {
           const double w = a.kp.inv_ls2_c[d];
           const bool in_tr = s_mask[d] != 0;
 #pragma unroll
-          for (int i = 0; i < 2; ++i)
+          for (int i = 0; i < 4; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
               const double df = aa[i] - bb[j];
@@ -242,7 +256,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
             }
         } else {
 #pragma unroll
-          for (int i = 0; i < 2; ++i)
+          for (int i = 0; i < 4; ++i)
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
               const double df = aa[i] - bb[j];
@@ -253,35 +267,44 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       for (int k = 0; k < dk; ++k) {
         const double w = a.kp.inv_ls2_k[k];
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int avz = za[k * LD + GP1::row_of(ty, i)];
+        for (int i = 0; i < 4; ++i) {
+          const int avz = za[k * LD + pair_row(GP1::row_of(ty, i))];   // za is staged in row order
 #pragma unroll
           for (int j = 0; j < 4; ++j) d2[i][j] += (avz != zb[k * LD + GP1::col_of(tx, j)]) ? w : 0.0;
         }
       }
       VZ_ST(t_d2 += clock64() - tc; tc = clock64();)
-      // The eight kernel values as one straight-line block of the branch-free Matern (independent chains
-      // the scheduler can interleave); columns at or past n_valid are zeroed by a select.
-      double kv[2][4];
+      // The L-inf distances are folded before the Matern block so that they are not live across it.
+      if (WITH_LINF) {
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            if ((jb * 64 + GP1::col_of(tx, j)) < a.tr_rows) lmin[i] = fmin(lmin[i], lf[i][j]);
+      }
+      // The sixteen kernel values as one straight-line block of the branch-free Matern (independent chains
+      // the scheduler can interleave); columns at or past n_valid are zeroed by a select.
+      double kv[4][4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) kv[i][j] = matern52_fast(d2[i][j], a.kp.sf2);
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
+      for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const int cj = GP1::col_of(tx, j);
           kv[i][j] = (jb * 64 + cj) < a.n_valid ? kv[i][j] : 0.0;
           mu_part[i] = fma(kv[i][j], alj[cj], mu_part[i]);
-          if (WITH_LINF && (jb * 64 + cj) < a.tr_rows) lmin[i] = fmin(lmin[i], lf[i][j]);
         }
       VZ_ST(t_mat += clock64() - tc; tc = clock64();)
+      // rows i = 2 ip, 2 ip + 1 of this thread are pair positions 2p, 2p + 1: one 16-byte store per column
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        double* dst = scr + (size_t)GP1::row_of(ty, i) * np + jb * 64;
-        *reinterpret_cast<double2*>(dst + GP1::col_of(tx, 0)) = make_double2(kv[i][0], kv[i][1]);
-        *reinterpret_cast<double2*>(dst + GP1::col_of(tx, 2)) = make_double2(kv[i][2], kv[i][3]);
+      for (int ip = 0; ip < 2; ++ip) {
+        double* dst = scr + (size_t)(GP1::row_of(ty, 2 * ip) >> 1) * (2 * np) + 2 * jb * 64;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          *reinterpret_cast<double2*>(dst + 2 * GP1::col_of(tx, j)) = make_double2(kv[2 * ip][j], kv[2 * ip + 1][j]);
       }
       VZ_ST(t_st += clock64() - tc;)
       VZ_ST(tc = clock64();)
@@ -290,15 +313,15 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     }
     cp_async_wait<0>();
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < 4; ++i) {
 #pragma unroll
       for (int o = 8; o > 0; o >>= 1) {
         mu_part[i] += __shfl_xor_sync(0xffffffffu, mu_part[i], o);
         if (WITH_LINF) lmin[i] = fmin(lmin[i], __shfl_xor_sync(0xffffffffu, lmin[i], o));
       }
       if (tx == 0) {
-        s_mu[GP1::row_of(ty, i)] = mu_part[i];
-        s_linf[GP1::row_of(ty, i)] = lmin[i];
+        s_mu[pair_row(GP1::row_of(ty, i))] = mu_part[i];
+        s_linf[pair_row(GP1::row_of(ty, i))] = lmin[i];
       }
     }
     fence_proxy_async();  // generic-proxy writes (scratch tile, aliased smem) before async-proxy (TMA) accesses
@@ -307,18 +330,21 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     VZ_ST(const long long t2 = clock64();)
 
     // ---------------- phase 2: row sums of (K* Linv^T)^2 on the DMMA pipe ----------------
-    // Slab (jb, ks): A = scratch[0:64, ks*16 : +16], B = Linv[jb*128 : +128, ks*16 : +16];
-    // block jb needs ks < min(np, (jb+1)*128)/16 because Linv is lower triangular.  The slab
+    // Slab (jb, ks): A = K*[0:64, ks*32 : +32] (four pair-order boxes), B = Linv[jb*128 : +128, ks*32 : +32];
+    // block jb needs ks < min(np, (jb+1)*128)/32 because Linv is lower triangular.  The slab
     // stream is flattened over blocks so the TMA ring never drains between blocks.
     // With nsplit > 1 this CTA takes blocks {split, nblocks-1-split} (balanced triangular work).
-    double rowsq[2] = {0.0, 0.0};
+    // acc[mf][f][g][c]: M fragment mf (tile rows wm*32 + mf*16 + ...), fragment row fr + 8f, column fragment g.
+    double rowsq[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
     for (int q = 0; q < nq; ++q) {
       const int jb = block_of(q);
-      double acc[2][4][2];
+      double acc[2][2][4][2];
 #pragma unroll
-      for (int f = 0; f < 2; ++f)
+      for (int mf = 0; mf < 2; ++mf)
 #pragma unroll
-        for (int g = 0; g < 4; ++g) { acc[f][g][0] = 0.0; acc[f][g][1] = 0.0; }
+        for (int f = 0; f < 2; ++f)
+#pragma unroll
+          for (int g = 0; g < 4; ++g) { acc[mf][f][g][0] = 0.0; acc[mf][f][g][1] = 0.0; }
       const int nsl = slabs_in(jb);
       const int col_base = jb * kBN + wn * 32;   // first output column of this warp
       for (int ks = 0; ks < nsl; ++ks) {
@@ -328,63 +354,73 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
         VZ_ST(w_tile += clock64() - tw;)
         ++slab_n;
         // Fragment loads are 16 bytes: lane (fr, fk) takes k = 8h + 2fk and 8h + 2fk + 1 of each
-        // 8-wide k group h as the k slots fk and fk + 4 of one m16n8k8 (rows fr and fr + 8 of A come
-        // from a0 and a1; the k order inside a slab is irrelevant as long as A and B agree).
-        // Fragment row fr reads tile row ... + pr, so the swizzle XOR is pr.
+        // 8-wide k group h as the k slots fk and fk + 4 of one m16n8k8 (the k order inside a slab is
+        // irrelevant as long as A and B agree).  A: one load per k gives rows fr and fr + 8 of M fragment
+        // mf (pair row (wm*2 + mf)*8 + fr of box h, chunk k % 8), i.e. a0, a1 or a2, a3 in register order.
+        // B: one load gives both k of column fr, which reads Linv row ... + pr.  Every row base is a
+        // multiple of 8, so the swizzle XOR is fr for A and pr for B; both are conflict-free.
         const double* stg = ring + stage * kStageDoubles;
-        const double* Arow0 = stg + (wm * 16 + pr) * 16;            // + half*kAHalf + chunk*2
-        const double* Brow0 = stg + 2 * kAHalf + (wn * 32 + pr) * 16;
+        const double* Arow0 = stg + (wm * 16 + fr) * 16;            // + h*kABox + mf*8*16 + chunk*2
+        const double* Brow0 = stg + 4 * kABox + (wn * 32 + pr) * 16;
         const int k0 = ks * kBK;
         // Linv[c, k] = 0 for k > c.  k0 and col_base are multiples of 32: slabs right of this
         // warp's 32 columns contribute nothing; in the diagonal slab (k0 == col_base) the k group
-        // h only reaches column fragments g >= h (static pattern, no predication).
-        if (k0 < col_base) {
+        // h only reaches column fragments g >= h.
+        // k group h of the slab: 4 B and 4 A fragment loads, then 8 DMMAs (fewer in the diagonal slab).
+        auto group = [&](int h, bool diag) {
+          const int co = ((((h & 1) * 4 + fk) ^ pr) * 2);   // swizzled 16-byte B chunk, in doubles
+          auto live = [&](int g) { return !(diag && g < h); };   // columns of fragment g < h lie left of k group h
+          double2 b[4];
 #pragma unroll
-          for (int h = 0; h < 4; ++h) {
-            const int co = ((((h & 1) * 4 + fk) ^ pr) * 2);   // swizzled 16-byte chunk, in doubles
-            const double2 a0 = *reinterpret_cast<const double2*>(Arow0 + (h >> 1) * kAHalf + co);
-            const double2 a1 = *reinterpret_cast<const double2*>(Arow0 + (h >> 1) * kAHalf + 8 * 16 + co);
-            double2 b[4];
+          for (int g = 0; g < 4; ++g)
+            if (live(g)) b[g] = *reinterpret_cast<const double2*>(Brow0 + (h >> 1) * kBHalf + g * 8 * 16 + co);
 #pragma unroll
-            for (int g = 0; g < 4; ++g) b[g] = *reinterpret_cast<const double2*>(Brow0 + (h >> 1) * kBHalf + g * 8 * 16 + co);
+          for (int mf = 0; mf < 2; ++mf) {
+            const double* Ah = Arow0 + h * kABox + mf * 8 * 16;
+            const double2 a01 = *reinterpret_cast<const double2*>(Ah + (((2 * fk) ^ fr) * 2));       // k = 8h + 2fk
+            const double2 a23 = *reinterpret_cast<const double2*>(Ah + (((2 * fk + 1) ^ fr) * 2));   // k = 8h + 2fk + 1
 #pragma unroll
             for (int g = 0; g < 4; ++g)
-              dmma_16x8x8(acc[0][g][0], acc[0][g][1], acc[1][g][0], acc[1][g][1], a0.x, a1.x, a0.y, a1.y, b[g].x, b[g].y);
+              if (live(g))
+                dmma_16x8x8(acc[mf][0][g][0], acc[mf][0][g][1], acc[mf][1][g][0], acc[mf][1][g][1],
+                            a01.x, a01.y, a23.x, a23.y, b[g].x, b[g].y);
           }
+        };
+        // The group loops are not unrolled: unrolled, ptxas hoists the loads of all four groups and runs
+        // out of registers.  A group's eight DMMAs keep the pipe busy while the other warp of the SM
+        // sub-partition waits for its loads.  The full slab has no predicate; the diagonal slab (one in
+        // every nsl of a warp) predicates its DMMAs on g >= h.
+        if (k0 < col_base) {
+#pragma unroll 1
+          for (int h = 0; h < 4; ++h) group(h, false);
         } else if (k0 == col_base) {
-#pragma unroll
-          for (int h = 0; h < 4; ++h) {
-            const int co = ((((h & 1) * 4 + fk) ^ pr) * 2);
-            const double2 a0 = *reinterpret_cast<const double2*>(Arow0 + (h >> 1) * kAHalf + co);
-            const double2 a1 = *reinterpret_cast<const double2*>(Arow0 + (h >> 1) * kAHalf + 8 * 16 + co);
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              if (g < h) continue;  // compile-time: columns of fragment g lie left of k group h
-              const double2 bg = *reinterpret_cast<const double2*>(Brow0 + (h >> 1) * kBHalf + g * 8 * 16 + co);
-              dmma_16x8x8(acc[0][g][0], acc[0][g][1], acc[1][g][0], acc[1][g][1], a0.x, a1.x, a0.y, a1.y, bg.x, bg.y);
-            }
-          }
+#pragma unroll 1
+          for (int h = 0; h < 4; ++h) group(h, true);
         }
         __syncwarp();
         if ((unsigned)lane < ncta) mbar_arrive_cluster(empty_bar + stage, lane);   // the stage of every CTA it was multicast into
       }
 #pragma unroll
-      for (int f = 0; f < 2; ++f)
+      for (int mf = 0; mf < 2; ++mf)
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          rowsq[f] = fma(acc[f][g][0], acc[f][g][0], rowsq[f]);
-          rowsq[f] = fma(acc[f][g][1], acc[f][g][1], rowsq[f]);
-        }
+        for (int f = 0; f < 2; ++f)
+#pragma unroll
+          for (int g = 0; g < 4; ++g) {
+            rowsq[mf][f] = fma(acc[mf][f][g][0], acc[mf][f][g][0], rowsq[mf][f]);
+            rowsq[mf][f] = fma(acc[mf][f][g][1], acc[mf][f][g][1], rowsq[mf][f]);
+          }
     }
     VZ_ST(const long long t3 = clock64();)
     cp_async_wait<0>();
     // combine the 4 lanes that share a fragment row, then the four N-warps through smem
 #pragma unroll
-    for (int f = 0; f < 2; ++f) {
-      rowsq[f] += __shfl_xor_sync(0xffffffffu, rowsq[f], 1);
-      rowsq[f] += __shfl_xor_sync(0xffffffffu, rowsq[f], 2);
-      if (fk == 0) s_rowsq[wn * 64 + wm * 16 + f * 8 + pr] = rowsq[f];
-    }
+    for (int mf = 0; mf < 2; ++mf)
+#pragma unroll
+      for (int f = 0; f < 2; ++f) {
+        rowsq[mf][f] += __shfl_xor_sync(0xffffffffu, rowsq[mf][f], 1);
+        rowsq[mf][f] += __shfl_xor_sync(0xffffffffu, rowsq[mf][f], 2);
+        if (fk == 0) s_rowsq[wn * 64 + wm * 32 + mf * 16 + f * 8 + fr] = rowsq[mf][f];
+      }
     consumer_sync();
     // ---------------- epilogue ----------------
     if (tid < kTM) {
@@ -813,7 +849,9 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
   record(nsplit > 1 ? VZGP_ROUTE_SPLIT : VZGP_ROUTE_CLUSTER, nsplit, grid);
   VZ_TRY(ensure_scratch(h, (size_t)grid * kTM * h->np * sizeof(double)));
   fill_score_args(h, Xs, Zs, M, acq, fn, score, mu, sigma, linf, &a);
-  VZ_TRY(make_map(&a.mapA, a.scratch, (uint64_t)grid * kTM, (uint64_t)h->np, (uint64_t)h->np, kTM));
+  // K* in pair order: grid * 32 row pairs of 2 np doubles; a box is one k group (32 pairs x 8 k x 2 rows)
+  VZ_TRY(make_map(&a.mapA, a.scratch, (uint64_t)grid * (kTM / 2), 2 * (uint64_t)h->np, 2 * (uint64_t)h->np, kTM / 2));
+  static_assert(4 * kABox == kTM * kBK, "four A boxes hold one slab of K*");
   VZ_TRY(make_map(&a.mapB, a.Linv, (uint64_t)h->np, (uint64_t)h->np, (uint64_t)h->np, kBPieceRows));
   a.nsplit = nsplit;
   if (nsplit > 1) {
