@@ -159,10 +159,29 @@ typedef enum vzgp_score_route {
   VZGP_ROUTE_GENERAL = 4   /* linear_coef models: explicit K* and W, k_general_finalize */
 } vzgp_score_route;
 
+/* Route the last NLL + gradient evaluation on a handle took (vzgp_get_int key "nll_route"; -1 before the first).
+ * vzgp_nll_grad, vzgp_nll_grad_multi and vzgp_nll_grad_batch record it on every handle they evaluate with. */
+typedef enum vzgp_nll_route {
+  VZGP_NLL_SMALL = 0,      /* N <= 64, one metric, no linear_coef: k_nll_grad_small (retry loop inside the kernel) */
+  VZGP_NLL_GRAPH = 1,      /* the replayed single-evaluation CUDA graph, no pivot flagged */
+  VZGP_NLL_EAGER = 2,      /* eager launches with the host retry loop: a pivot flagged in a graph, linear_coef or
+                              VZGP_NLL_GRAPH=0; also a restart of vzgp_nll_grad_batch that fell back */
+  VZGP_NLL_BATCH = 3       /* vzgp_nll_grad_batch, no pivot flagged for this restart */
+} vzgp_nll_route;
+
+/* Factorisation route of the last fit, NLL evaluation, vzgp_cholesky_retry or vzgp_factor_inverse on a handle
+ * (vzgp_get_int key "factor_route"; -1 before the first).  A retry ladder records its last attempt. */
+typedef enum vzgp_factor_route {
+  VZGP_FACTOR_PANEL = 0,   /* 64-wide panel kernels (potrf_blocked; k_nll_grad_small factors its 64 x 64 block in
+                              the same way) */
+  VZGP_FACTOR_DATAFLOW = 1 /* k_chol_dataflow: factor, L^-1, L^-T (and K_y^-1 for the NLL) in one launch */
+} vzgp_factor_route;
+
 /* Counters.  "launches" (= vzgp_launch_count), "score_i8_launches": launches of the integer-split scoring kernel.
  * "sm_count": multiprocessors of the handle's device.  Of the last scoring call: "score_route" (vzgp_score_route),
  * "score_nsplit" (CTAs per 64-candidate tile: > 1 on the split route only, 1 on the cluster and i8 routes, 0
- * otherwise), "score_grid" (CTAs of the k_score / k_score_i8 launch, 0 on the other routes). */
+ * otherwise), "score_grid" (CTAs of the k_score / k_score_i8 launch, 0 on the other routes).  Of the last NLL
+ * evaluation and factorisation: "nll_route" (vzgp_nll_route), "factor_route" (vzgp_factor_route). */
 int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value);
 
 /* ---- stage-wise entry points (parity tests call these one by one) -------- */

@@ -103,7 +103,8 @@ def test_cholesky_retry_semantics(dev):
   assert retries == 6 and np.isnan(l.cpu().numpy()).any()
 
 
-@pytest.mark.parametrize('n,d,dk,nv', [(50, 4, 0, 50), (200, 6, 0, 200), (150, 5, 2, 140), (333, 20, 0, 333)])
+@pytest.mark.parametrize('n,d,dk,nv', [(50, 4, 0, 50), (200, 6, 0, 200), (150, 5, 2, 140), (333, 20, 0, 333), (63, 3, 0, 63),
+                                        (64, 4, 0, 64), (65, 4, 0, 65), (127, 5, 0, 64), (128, 5, 2, 65), (129, 6, 0, 1)])
 def test_fit_factor_and_alpha(dev, n, d, dk, nv):
   x, y, z = _problem(n, d, 5, dk)
   po, pg = _params(d, dk)
@@ -169,7 +170,8 @@ def test_score_hard_conditioning_scaled_tolerance(dev):
   np.testing.assert_allclose(out['stddev'].cpu().numpy(), sd_w, atol=1e-7, rtol=0)
 
 
-@pytest.mark.parametrize('n,d,dk,nv', [(40, 3, 0, 40), (130, 6, 2, 120), (256, 20, 0, 256)])
+@pytest.mark.parametrize('n,d,dk,nv', [(40, 3, 0, 40), (130, 6, 2, 120), (256, 20, 0, 256), (65, 4, 0, 64), (127, 5, 0, 127),
+                                        (128, 5, 1, 65), (129, 6, 2, 1), (129, 3, 0, 129)])
 def test_nll_grad(dev, n, d, dk, nv):
   x, y, z = _problem(n, d, 10, dk)
   po, pg = _params(d, dk, sf2=0.7, sn2=2e-3)
@@ -183,7 +185,8 @@ def test_nll_grad(dev, n, d, dk, nv):
   np.testing.assert_allclose(grad, want_g, atol=1e-8 * max(1.0, np.max(np.abs(want_g))), rtol=0)
 
 
-@pytest.mark.parametrize('n,d,dk,nv', [(1, 1, 0, 1), (7, 2, 1, 7), (50, 4, 0, 50), (64, 20, 3, 64), (64, 64, 0, 57), (33, 5, 2, 20)])
+@pytest.mark.parametrize('n,d,dk,nv', [(1, 1, 0, 1), (7, 2, 1, 7), (50, 4, 0, 50), (64, 20, 3, 64), (64, 64, 0, 57), (33, 5, 2, 20),
+                                        (63, 3, 0, 63), (64, 4, 1, 1)])
 def test_nll_grad_small_fused_kernel(dev, n, d, dk, nv):
   """N <= 64 takes the single-launch kernel (k_nll_grad_small): same oracle, same tolerances, and the
   make_loss_fn closure the ARD driver uses returns the same numbers; the fitted model is untouched."""

@@ -84,8 +84,9 @@ static int factor_invert(vzgp_handle* h, double* L, double* Linv, double* LinvT,
   if (LinvT != nullptr) {
     const int st = chol_dataflow(h, L, Linv, LinvT, Kinv, np, flag);
     if (st < 0) return st;
-    if (st == 0) { *used_dataflow = true; return 0; }
+    if (st == 0) { *used_dataflow = true; h->factor_route = VZGP_FACTOR_DATAFLOW; return 0; }
   }
+  h->factor_route = VZGP_FACTOR_PANEL;
   VZ_TRY(potrf_blocked(h, L, np, Linv, np, np, flag));
   VZ_TRY(h->Tws.reserve(sizeof(double) * (size_t)np * np));
   VZ_TRY(trtri_doubling(h, L, np, Linv, np, h->Tws.as<double>(), np, np));
@@ -211,10 +212,11 @@ static int nll_sequence(vzgp_handle* h, const double* X, const int32_t* Z, const
   VZ_TRY(launch_copy_lower_shift(h, h->Kws.as<double>(), np, np, np, 0.0, h->L.as<double>(), np));
   bool df = false;   // dataflow kernel: factor, both inverses and K_y^-1 (one plane) in one launch
   VZ_TRY(factor_invert(h, h->L.as<double>(), h->Linv.as<double>(), h->LinvT.as<double>(), h->Kinv.as<double>(), np, flag, &df));
+  h->nll_factor_route = h->factor_route;
   VZ_TRY(solve_alphas(h, y, N, n_valid, np, n_metrics, 0.0, df));
   double* out2 = reinterpret_cast<double*>(h->small.as<char>() + kOffLogdet);
   double* gout = reinterpret_cast<double*>(h->small.as<char>() + kOffGrad);
-  VZ_TRY(launch_logdet_quad(h, h->L.as<double>(), np, n_valid, h->ypad.as<double>() + np, out2, 4 * np, n_metrics));
+  VZ_TRY(launch_logdet_quad(h, h->L.as<double>(), np, N, n_valid, h->ypad.as<double>() + np, out2, 4 * np, n_metrics));
   if (!df) VZ_TRY(launch_lauum(h, h->Linv.as<double>(), np, h->Kinv.as<double>(), np, np));
   VZ_TRY(launch_nll_grad_tiles(h, h->X.as<double>(), h->Z.as<int32_t>(), np, n_valid, kp, h->Kinv.as<double>(), np,
                                h->alpha.as<double>(), h->Tws.as<double>(), gout, df ? np : 0, n_metrics));
@@ -259,6 +261,7 @@ static int nll_graph_eval(vzgp_handle* h, const double* X, const int32_t* Z, con
     VZ_TRY(chol_dataflow_prepare(h, np, true));   // task list + flags: not capturable
     bufs(cur);
     h->n = N; h->np = np; h->dc = dc; h->dk = dk; h->n_valid = n_valid; h->n_metrics = n_metrics;
+    h->mean_const = 0.0;   // the label-padding node captures it: a linear_coef fit before must not leak its prior mean in
     const int64_t l0 = h->launches;
     if (cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeRelaxed) != cudaSuccess) { cudaGetLastError(); return 1; }
     const int st = nll_sequence(h, X, Z, y, N, dc, dk, n_valid, kp, sn2, n_metrics);
@@ -314,6 +317,7 @@ static int nll_graph_eval(vzgp_handle* h, const double* X, const int32_t* Z, con
   VZ_CUDA(cudaMemcpyAsync(hostg, h->small.as<char>() + kOffGrad, sizeof(double) * nq, cudaMemcpyDeviceToHost, h->stream));
   VZ_CUDA(cudaMemcpyAsync(&bad, h->small.as<char>() + kOffFlag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   VZ_CUDA(cudaStreamSynchronize(h->stream));
+  h->nll_route = VZGP_NLL_GRAPH; h->factor_route = h->nll_factor_route;
   return bad ? 1 : 0;
 }
 
@@ -527,6 +531,8 @@ int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value) {
   if (std::strcmp(key, "score_route") == 0) { *value = h->score_route; return 0; }
   if (std::strcmp(key, "score_nsplit") == 0) { *value = h->score_nsplit; return 0; }
   if (std::strcmp(key, "score_grid") == 0) { *value = h->score_grid; return 0; }
+  if (std::strcmp(key, "nll_route") == 0) { *value = h->nll_route; return 0; }
+  if (std::strcmp(key, "factor_route") == 0) { *value = h->factor_route; return 0; }
   set_error("vzgp_get_int: unknown key '%s'", key);
   return VZGP_ERR_ARG;
 }
@@ -700,6 +706,7 @@ int vzgp_nll_grad_multi(vzgp_handle* h, const double* X, const int32_t* Z, const
     double host[4 + kMaxGrad];
     VZ_CUDA(cudaMemcpyAsync(host, dout, sizeof(double) * (4 + nq), cudaMemcpyDeviceToHost, h->stream));
     VZ_CUDA(cudaStreamSynchronize(h->stream));
+    h->nll_route = VZGP_NLL_SMALL; h->factor_route = VZGP_FACTOR_PANEL;
     finish(host[0] + host[1], host + 4);
     return (int)host[3];
   }
@@ -721,12 +728,13 @@ int vzgp_nll_grad_multi(vzgp_handle* h, const double* X, const int32_t* Z, const
   double shift = 0.0;
   int retries = fit_common(h, X, Z, y, N, Dc, Dk, n_valid, p, &shift, n_metrics);
   if (retries < 0) return retries;
+  h->nll_route = VZGP_NLL_EAGER;
   const int np = h->np, nq = Dc + Dk + 2 + (lin ? Dc + 2 : 0);
   VZ_TRY(h->Kinv.reserve(sizeof(double) * (size_t)np * np * kLauumSplit));   // partial planes of K_y^-1
   double* out2 = reinterpret_cast<double*>(h->small.as<char>() + kOffLogdet);
   double* gout = reinterpret_cast<double*>(h->small.as<char>() + kOffGrad);
   double* w = h->ypad.as<double>() + np;
-  VZ_TRY(launch_logdet_quad(h, h->L.as<double>(), np, n_valid, w, out2, 4 * np, n_metrics, h->alpha.as<double>()));
+  VZ_TRY(launch_logdet_quad(h, h->L.as<double>(), np, N, n_valid, w, out2, 4 * np, n_metrics, h->alpha.as<double>()));
   VZ_TRY(launch_lauum(h, h->Linv.as<double>(), np, h->Kinv.as<double>(), np, np));
   VZ_TRY(launch_nll_grad_tiles(h, h->X.as<double>(), h->Z.as<int32_t>(), np, n_valid, h->kp,
                                h->Kinv.as<double>(), np, h->alpha.as<double>(), h->Tws.as<double>(), gout, 0, n_metrics));
@@ -1375,6 +1383,7 @@ int vzgp_nll_grad_batch(vzgp_handle* const* hs, int R, const double* X, const in
       VZ_TRY(ensure_pinned(h, res_bytes));
       h->fitted = false; h->i8_ready = false;
       h->n = N; h->np = np; h->dc = Dc; h->dk = Dk; h->n_valid = n_valid; h->n_metrics = n_metrics;
+      h->mean_const = 0.0;   // captured by the label-padding node (see nll_graph_eval)
       VZ_CUDA(cudaStreamSynchronize(h->stream));
     }
     const int64_t l0[kMaxBatch] = {};
@@ -1471,6 +1480,7 @@ int vzgp_nll_grad_batch(vzgp_handle* const* hs, int R, const double* X, const in
     const double* hg = reinterpret_cast<const double*>(pin + 16);
     const int bad = *reinterpret_cast<const int*>(pin + 16 + sizeof(double) * nq);
     if (!bad) {
+      hs[r]->nll_route = VZGP_NLL_BATCH; hs[r]->factor_route = hs[r]->nll_factor_route;
       finish_loss(&ps[r], Dc, Dk, n_valid, n_metrics, h2[1] + h2[0], hg, loss_out + r, grad_out + (size_t)r * nq);
     } else {
       // a pivot failed without jitter: this restart alone takes the path with the retry loop

@@ -163,7 +163,12 @@ struct vzgp_handle {
   int nll_key_dims[5] = {0, 0, 0, 0, 0};                         // N, dc, dk, n_valid, n_metrics
   const void* nll_bufs[kNllBufsDecl] = {};                                 // handle buffers the graph points into (a growth reallocates them)
   int nll_launches = 0;
+  int nll_factor_route = 0;   // factor route of the captured sequence (fixed by np and VZGP_DATAFLOW)
   void* batch = nullptr;   // BatchGraph (c_abi.cu): this handle leads a batch of concurrent evaluations
+
+  // Route of the last NLL + gradient evaluation on this handle (vzgp_nll_route) and of its last factorisation
+  // (vzgp_factor_route); -1 before the first.  Tests read them through vzgp_get_int.
+  int nll_route = -1, factor_route = -1;
 
   // Dataflow factorisation (dataflow.cu): task list for the current nb, flags, chain partial sums.
   vzgp::DevBuf df_tasks[2], df_flags, df_S;     // task lists without / with the K_y^-1 tasks

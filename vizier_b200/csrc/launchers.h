@@ -51,7 +51,7 @@ int launch_pad_vector(vzgp_handle* h, const double* src, int n, int n_valid, int
 int launch_pad_rows(vzgp_handle* h, const double* src, int n, int d, int np, double* dst);
 int launch_transpose_scale(vzgp_handle* h, const double* X, int np, int dc, const KernelParams& kp, double* XT);
 int launch_pad_rows_i32(vzgp_handle* h, const int32_t* src, int n, int d, int np, int32_t* dst);
-int launch_logdet_quad(vzgp_handle* h, const double* L, int ld, int n_valid, const double* w, double* out,
+int launch_logdet_quad(vzgp_handle* h, const double* L, int ld, int n, int n_valid, const double* w, double* out,
                        int wstride = 0, int n_metrics = 1, const double* alpha = nullptr);
 
 int launch_gemm_nt_tri(vzgp_handle* h, const double* A, int lda, int mp, const double* B, int ldb, int np,

@@ -437,16 +437,19 @@ __global__ void k_pad_rows_i32(const int32_t* __restrict__ src, int n, int d, in
   dst[e] = e < (size_t)n * d ? src[e] : -1;
 }
 
-// n_metrics * sum_i log L_ii over i < n_valid and  0.5 * sum_m sum_i w_m[i]^2  ->  out[0], out[1]
+// n_metrics * sum_i log L_ii over i < n and  0.5 * sum_m sum_i w_m[i]^2 over i < n_valid  ->  out[0], out[1]
 // (single block; w_m = w + m * wstride: the independent multi-task GP shares one factor).
 // out[2] = sum_i alpha[i] over the valid rows (gradient of the constant mean of the linear_coef model).
-__global__ void k_logdet_quad(const double* __restrict__ L, int ld, int n_valid,
+// The log-det runs over all n observations, masked ones included: a masked row is an identity row, so it adds
+// log(1 + shift) once the jitter fires, as in TFP's masked GaussianProcess (DESIGN.md, deviations).
+__global__ void k_logdet_quad(const double* __restrict__ L, int ld, int n, int n_valid,
                               const double* __restrict__ w, int wstride, int n_metrics, double* __restrict__ out,
                               const double* __restrict__ alpha) {
   __shared__ double red[32];
   double a = 0.0, b = 0.0, c = 0.0;
-  for (int i = threadIdx.x; i < n_valid; i += blockDim.x) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
     a += log(L[(size_t)i * ld + i]);
+    if (i >= n_valid) continue;
     for (int m = 0; m < n_metrics; ++m) { const double v = w[(size_t)m * wstride + i]; b = fma(v, v, b); }
     if (alpha) c += alpha[i];
   }
@@ -691,9 +694,9 @@ int launch_pad_rows_i32(vzgp_handle* h, const int32_t* src, int n, int d, int np
   h->launches++;
   return 0;
 }
-int launch_logdet_quad(vzgp_handle* h, const double* L, int ld, int n_valid, const double* w,
+int launch_logdet_quad(vzgp_handle* h, const double* L, int ld, int n, int n_valid, const double* w,
                        double* out, int wstride, int n_metrics, const double* alpha) {
-  k_logdet_quad<<<1, 256, 0, h->stream>>>(L, ld, n_valid, w, wstride, n_metrics, out, alpha);
+  k_logdet_quad<<<1, 256, 0, h->stream>>>(L, ld, n, n_valid, w, wstride, n_metrics, out, alpha);
   VZ_CHECK_LAUNCH();
   h->launches++;
   return 0;

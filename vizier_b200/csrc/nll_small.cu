@@ -24,7 +24,7 @@ __device__ __forceinline__ double warp_sum(double v) {
 }
 }  // namespace
 
-// out: [0] = sum_i log L_ii (valid rows), [1] = 0.5 * |L^-1 y|^2, [2] = shift used, [3] = retries
+// out: [0] = sum_i log L_ii (i < N), [1] = 0.5 * |L^-1 y|^2, [2] = shift used, [3] = retries
 //      (max_iters + 1 = never succeeded), [4 .. 4 + nq) = raw gradient sums in the order
 //      categorical (G E neq_k), continuous (G E diff_d^2), trace(G), sum(G K).
 __global__ void __launch_bounds__(256) k_nll_grad_small(const double* __restrict__ X, const int32_t* __restrict__ Z,
@@ -128,7 +128,11 @@ __global__ void __launch_bounds__(256) k_nll_grad_small(const double* __restrict
   // ---- log-det and quadratic form ----
   if (warp == 0) {
     double lg = 0.0, q = 0.0;
-    for (int i = lane; i < n_valid; i += 32) { lg += log(a[i * kLD + i]); q = fma(wv[i], wv[i], q); }
+    // log-det over all N rows: a masked (identity) row adds log(1 + shift) once the jitter fires (k_logdet_quad)
+    for (int i = lane; i < N; i += 32) {
+      lg += log(a[i * kLD + i]);
+      if (i < n_valid) q = fma(wv[i], wv[i], q);
+    }
     lg = warp_sum(lg); q = warp_sum(q);
     if (lane == 0) { out[0] = lg; out[1] = 0.5 * q; out[2] = shift; out[3] = (double)attempt; }
   }

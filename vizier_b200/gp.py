@@ -517,6 +517,7 @@ class DeviceGP:
       return out_l, out_g
 
     f.n_restarts = r_all
+    f.status = status   # per restart, of the last call: Cholesky retries of a restart that took the retry path
     return f
 
   def score(self, xs, acq: Acquisition, zs=None, with_aux: bool = False, out: Optional[dict] = None) -> dict:
