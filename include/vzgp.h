@@ -156,7 +156,7 @@ typedef enum vzgp_score_route {
   VZGP_ROUTE_SPLIT = 1,    /* 2 * tiles <= SMs: k_score, score_nsplit CTAs per tile, then k_score_finalize */
   VZGP_ROUTE_CLUSTER = 2,  /* every other pool: k_score in 2-CTA clusters */
   VZGP_ROUTE_I8 = 3,       /* "score_i8" on and eligible: k_score_i8 */
-  VZGP_ROUTE_GENERAL = 4   /* linear_coef models: explicit K* and W, k_general_finalize */
+  VZGP_ROUTE_GENERAL = 4   /* linear_coef models: explicit K* and W, k_general_finalize; every vzgp_score_qsets call */
 } vzgp_score_route;
 
 /* Route the last NLL + gradient evaluation on a handle took (vzgp_get_int key "nll_route"; -1 before the first).
@@ -469,6 +469,45 @@ int vzgp_eagle_run_stack(vzgp_handle* const* hs, int E, const double* alphas, co
  * mu / sigma (model A) and sigma_all (sqrt of the diagonal of B's covariance), each [n_sets * q], are optional. */
 int vzgp_score_set_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, int n_sets, int q, const vzgp_pe_params* pe,
                       double* score, double* mu, double* sigma, double* sigma_all);
+
+/* Parallel (q-) acquisitions (acquisitions.py:495-568): Monte Carlo estimates over the joint posterior predictive of
+ * a set of q points.  Per set, with mean mu [q] and covariance Sigma [q x q] (observation noise on the diagonal),
+ * L = Cholesky of Sigma (unshifted, then shifts 1e-4 * 10^k, k < 5; a set whose factor still fails scores NaN) and
+ * S draws f_s = mu + L z_s:
+ *   QEI   mean_s max_j max(f_sj - best_label - 0.01, 0)
+ *   QPI   mean_s [max_j f_sj - best_label > 0]
+ *   QUCB  mean_s max_j (mu_j + coefficient * |f_sj - mu_j|)
+ * A non-finite best_label (no observation) makes QEI and QPI score mean_s max_j f_sj.  Ensembles (E members) are
+ * the uniform mixture: each (set, sample) draws one member and samples all q points from it; QUCB's mu is the
+ * mixture mean.  Draws depend on the set's position p = set index mod period (common random numbers across the
+ * batches of an optimiser run): z for (p, s, j) from Philox stream 12, elements 2e and 2e + 1 with e = (p S + s) q + j
+ * (Box-Muller), the member from stream 13, element p S + s.  With the trust region on and trust_radius <= 0.5, each
+ * point farther than the radius (L-inf, over tr_dim_mask) from the first tr_rows trials adds -1e4 - distance
+ * (gp_ucb_pe.py:245-269). */
+typedef enum vzgp_qacq_kind { VZGP_QACQ_QEI = 0, VZGP_QACQ_QPI = 1, VZGP_QACQ_QUCB = 2 } vzgp_qacq_kind;
+typedef struct vzgp_qacq {
+  int kind;                     /* vzgp_qacq_kind */
+  double best_label;            /* QEI / QPI */
+  double coefficient;           /* QUCB */
+  int num_samples;              /* S, 1 .. 8192 */
+  int period;                   /* positions repeat every `period` sets; <= 0: n_sets */
+  int use_trust_region;
+  double trust_radius;
+  const uint8_t* tr_dim_mask;   /* host [Dc] or NULL (all dimensions) */
+  int tr_rows;                  /* 0 = all valid trials */
+  double* cov_out;              /* optional device [E][n_sets][q][q]: the covariance blocks */
+} vzgp_qacq;
+
+/* Scores n_sets sets of q points (Xs [n_sets * q x Dc], Zs [n_sets * q x Dk], device) under the E models hs (E = 1: a
+ * single model; members must be fitted on the same trials and share device and stream).  1 <= q <= 16, E <= 16.
+ * Device outputs: score [n_sets]; optional mu (mixture mean), sigma (mixture stddev) and linf (L-inf distance to the
+ * trusted trials), each [n_sets * q].  K* and W = K* L^-T go through the general route in chunks of whole sets. */
+int vzgp_score_qsets(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int n_sets, int q,
+                     const vzgp_qacq* qa, uint64_t seed, double* score, double* mu, double* sigma, double* linf);
+/* The Monte Carlo stage alone on given moments: mean [E][n_sets * q], cov [E][n_sets][q][q] (device).  The trust
+ * region fields are ignored. */
+int vzgp_qacq_from_moments(vzgp_handle* h, int n_sets, int q, int E, const double* mean, const double* cov,
+                           const vzgp_qacq* qa, uint64_t seed, double* score);
 
 /* Host-stepped form of the same optimiser: identical device-resident state and kernels, but the CALLER scores every
  * batch - for acquisitions libvzgp cannot evaluate by itself, e.g. one with a user-supplied `prior_acquisition` term

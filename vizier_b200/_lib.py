@@ -75,6 +75,24 @@ class AcqFn(C.Structure):
   ]
 
 
+QACQ_QEI, QACQ_QPI, QACQ_QUCB = 0, 1, 2   # vzgp_qacq_kind
+
+
+class QAcq(C.Structure):
+  _fields_ = [
+      ('kind', C.c_int),
+      ('best_label', C.c_double),
+      ('coefficient', C.c_double),
+      ('num_samples', C.c_int),
+      ('period', C.c_int),
+      ('use_trust_region', C.c_int),
+      ('trust_radius', C.c_double),
+      ('tr_dim_mask', C.POINTER(C.c_uint8)),
+      ('tr_rows', C.c_int),
+      ('cov_out', C.c_void_p),
+  ]
+
+
 class PeParams(C.Structure):
   _fields_ = [
       ('mode', C.c_int),
@@ -198,6 +216,8 @@ SIGNATURES = {
     'vzgp_score_stack': (_i, [C.POINTER(C.c_void_p), _i, _pd, _vp, _vp, _i, _pA, _vp, _vp, _vp, _vp]),
     'vzgp_eagle_run_stack': (_i, [C.POINTER(C.c_void_p), _i, _pd, _pE, _pA, _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32, _pd]),
     'vzgp_score_set_pe': (_i, [_vp, _vp, _vp, _i, _i, _pPE, _vp, _vp, _vp, _vp]),
+    'vzgp_score_qsets': (_i, [C.POINTER(_vp), _i, _vp, _vp, _i, _i, C.POINTER(QAcq), _u64, _vp, _vp, _vp, _vp]),
+    'vzgp_qacq_from_moments': (_i, [_vp, _i, _i, _i, _vp, _vp, C.POINTER(QAcq), _u64, _vp]),
     'vzgp_eagle_begin': (_i, [_vp, _pE, _pi32, _i, _u64, _i, C.POINTER(C.c_void_p)]),
     'vzgp_eagle_seed': (_i, [_vp, _vp, _vp]),
     'vzgp_eagle_ask': (_i, [_vp, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),

@@ -5,7 +5,8 @@ Mirrors vizier/_src/algorithms/designers/gp/acquisitions.py: `UCB` / `LCB` / `EI
 (:368-387), `TrustRegion.__post_init__` (:734-749, which dimensions take part), `TrustRegion.trust_radius`
 (:757-777).  The per-candidate work (the acquisition of (mean, stddev), its thresholding, the min L-inf distance
 and the -1e4 - distance penalty) runs inside the CUDA scoring kernels; `lower_acquisition` turns an acquisition
-object into the O(1) scalars they take.
+object into the O(1) scalars they take.  The parallel acquisitions `QEI` / `QPI` / `QUCB` (:495-568) score sets of
+points; `lower_parallel_acquisition` turns them into the `gp.QAcquisition` of the set scorer (csrc/score_q.cu).
 """
 
 from __future__ import annotations
@@ -73,6 +74,34 @@ class EI:
 @dataclasses.dataclass
 class PI:
   best_labels: Any
+
+
+@dataclasses.dataclass
+class QEI:
+  """Parallel expected improvement of a set of points (acquisitions.py:495-518), estimated from `num_samples`
+  joint posterior draws."""
+
+  best_labels: Any
+  num_samples: int = 100
+
+
+@dataclasses.dataclass
+class QPI:
+  """Parallel probability of improvement (acquisitions.py:521-544)."""
+
+  best_labels: Any
+  num_samples: int = 100
+
+
+@dataclasses.dataclass
+class QUCB:
+  """Parallel upper confidence bound (acquisitions.py:547-568); QUCB(c * sqrt(pi / 2)) equals UCB(c) for one point."""
+
+  coefficient: float = 1.8
+  num_samples: int = 100
+
+
+_PARALLEL = (QEI, QPI, QUCB)
 
 
 @dataclasses.dataclass
@@ -152,8 +181,17 @@ def _lower_term(fn) -> gp.AcqTermSpec:
       'AcquisitionTrustRegion of those are)')
 
 
-def check_supported(fn) -> None:
-  """Raises NotImplementedError unless `lower_acquisition` can lower `fn` (any labels)."""
+def check_supported(fn, *, parallel: bool = False) -> None:
+  """Raises NotImplementedError unless `lower_acquisition` (or, with parallel=True, `lower_parallel_acquisition`)
+  can lower `fn` (any labels)."""
+  if parallel:
+    if not isinstance(fn, _PARALLEL):
+      raise NotImplementedError(
+          f'acquisition function {type(fn).__name__} is not a parallel acquisition (QEI, QPI and QUCB are); '
+          'scoring_function_is_parallel=True needs one of those')
+    return
+  if isinstance(fn, _PARALLEL):
+    raise NotImplementedError(f'{type(fn).__name__} scores sets of points: use scoring_function_is_parallel=True')
   if isinstance(fn, AcquisitionTrustRegion):
     check_supported(fn.main_acquisition)
     check_supported(fn.thresholding_acquisition)
@@ -181,6 +219,20 @@ def lower_acquisition(fn) -> gp.AcqFnSpec:
   if np.isnan(threshold) or main_only:
     return gp.AcqFnSpec(main)
   return gp.AcqFnSpec(main, thresholding=thr, threshold=threshold, bad_acq_value=float(fn.bad_acq_value))
+
+
+def lower_parallel_acquisition(fn, *, use_trust_region: bool = False, trust_radius: float = 1.0,
+                               tr_dim_mask: Optional[np.ndarray] = None) -> gp.QAcquisition:
+  """QEI / QPI / QUCB -> the `gp.QAcquisition` the set scorer evaluates.  A best label of -inf (no observation) makes
+  QEI and QPI score the expected maximum of the set.  The trust region is the set rule of gp_ucb_pe.py:245-269."""
+  check_supported(fn, parallel=True)
+  common = dict(num_samples=int(fn.num_samples), use_trust_region=bool(use_trust_region),
+                trust_radius=float(trust_radius), tr_dim_mask=tr_dim_mask)
+  if isinstance(fn, QUCB):
+    return gp.QAcquisition(_lib.QACQ_QUCB, coefficient=float(fn.coefficient), **common)
+  kind = _lib.QACQ_QEI if isinstance(fn, QEI) else _lib.QACQ_QPI
+  return gp.QAcquisition(kind, best_label=_best_label(fn.best_labels), **common)
+
 
 TR_MIN_RADIUS = 0.2        # TrustRegion.min_radius (acquisitions.py:751-754)
 TR_DIMENSION_FACTOR = 5.0  # acquisitions.py:760

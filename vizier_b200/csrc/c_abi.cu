@@ -1301,6 +1301,40 @@ int vzgp_eagle_run_ensemble(vzgp_handle* const* hs, int E, const vzgp_eagle_conf
                         best_z, best_score, hs, E);
 }
 
+static int check_qacq(const vzgp_qacq* qa, int n_sets, int q) {
+  VZ_ARG(qa != nullptr, "qacq");
+  VZ_ARG(qa->kind == VZGP_QACQ_QEI || qa->kind == VZGP_QACQ_QPI || qa->kind == VZGP_QACQ_QUCB, "kind");
+  VZ_ARG(q >= 1 && q <= 16, "1 <= q <= 16");
+  VZ_ARG(qa->num_samples >= 1 && qa->num_samples <= 8192, "1 <= num_samples <= 8192");
+  VZ_ARG(n_sets >= 0 && (int64_t)n_sets * q <= INT_MAX / 16, "n_sets");
+  return 0;
+}
+
+int vzgp_score_qsets(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int n_sets, int q,
+                     const vzgp_qacq* qa, uint64_t seed, double* score, double* mu, double* sigma, double* linf) {
+  VZ_TRY(check_ensemble(hs, E));
+  VZ_TRY(check_qacq(qa, n_sets, q));
+  for (int e = 0; e < E; ++e) VZ_ARG(hs[e]->n_metrics == 1, "q-acquisitions: single-metric models");
+  VZ_ARG(hs[0]->dc <= kMaxDc && hs[0]->dk <= kMaxDk, "Dc <= 64, Dk <= 32");
+  VZ_ARG(n_sets == 0 || score != nullptr, "score");
+  VZ_ARG(n_sets == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
+  VZ_ARG(n_sets == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
+  if (n_sets == 0) return 0;
+  Guard g(hs[0]->device);
+  return launch_score_qsets(hs, E, Xs, Zs, n_sets, q, qa, seed, score, mu, sigma, linf);
+}
+
+int vzgp_qacq_from_moments(vzgp_handle* h, int n_sets, int q, int E, const double* mean, const double* cov,
+                           const vzgp_qacq* qa, uint64_t seed, double* score) {
+  VZ_ARG(h != nullptr, "handle");
+  VZ_ARG(E >= 1 && E <= 16, "1 <= E <= 16");
+  VZ_TRY(check_qacq(qa, n_sets, q));
+  VZ_ARG(n_sets == 0 || (mean != nullptr && cov != nullptr && score != nullptr), "mean / cov / score");
+  if (n_sets == 0) return 0;
+  Guard g(h->device);
+  return launch_qacq_mc(h, n_sets, q, E, mean, cov, nullptr, qa, seed, score, nullptr, nullptr);
+}
+
 static int check_stack(vzgp_handle* const* hs, int E, const double* alphas) {
   VZ_ARG(hs != nullptr && alphas != nullptr && E >= 1 && E <= 16, "1 <= E <= 16 handles, alphas");
   for (int e = 0; e < E; ++e) {

@@ -147,6 +147,7 @@ struct vzgp_handle {
   void* eagle_step = nullptr;   // EagleStepState (c_abi.cu) of a host-stepped optimiser run
   vzgp::DevBuf pe_tmp;  // GP-UCB-PE: per-candidate pieces of the two models
   vzgp::DevBuf gen;     // general scoring path: explicit K* and W chunks
+  vzgp::DevBuf qmom;    // q-acquisitions (score_q.cu): per-member set means and covariance blocks, L-inf distances
   vzgp::DevBuf scal;    // multi-metric: [S][M] inverse scalarisation weights, then [S] best observed values
   vzgp::ScalArgs scal_args;
   void* pinned = nullptr;

@@ -11,6 +11,8 @@ namespace vzgp {
 
 constexpr uint32_t kStreamInitCat = 4, kStreamCatLaplace = 5, kStreamCatGumbel = 6, kStreamTrimCat = 7,
                    kStreamPullRand = 9, kStreamPushRand = 10, kStreamSetLaplace = 11;
+// Monte Carlo draws of the q-acquisitions (score_q.cu): Box-Muller normals and mixture members.
+constexpr uint32_t kStreamQacqNormal = 12, kStreamQacqMember = 13;
 
 __device__ __forceinline__ double laplace_from_uniform(double u) {
   const double v = u - 0.5;

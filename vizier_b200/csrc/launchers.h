@@ -92,6 +92,22 @@ int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, cons
                        const AcqFn* fn = nullptr);
 int launch_set_pe_combine(vzgp_handle* h, int n_sets, int q, const vzgp_pe_params* pe, const double* cov, int ldc,
                           const double* mu_a, const double* sd_a, const double* linf, double* score, double* sd_all);
+// General scoring path (score.cu): explicit K* and W = K* Linv^T of at most kGeneralChunk candidates at a time, in the
+// handle's `gen` buffers ([kGeneralChunk x np] each, rows padded to 64; Xp / Zp the padded candidates).
+constexpr int kGeneralChunk = 4096;
+struct GeneralChunk {
+  double* Ks;
+  double* W;
+  double* Xp;
+  int32_t* Zp;
+};
+int general_chunk_buffers(vzgp_handle* h, GeneralChunk* c);
+int launch_general_chunk(vzgp_handle* h, const double* Xs, const int32_t* Zs, int mc, const GeneralChunk& c);
+// Parallel (q-) acquisitions (score_q.cu).
+int launch_score_qsets(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int n_sets, int q,
+                       const vzgp_qacq* qa, uint64_t seed, double* score, double* mu, double* sigma, double* linf);
+int launch_qacq_mc(vzgp_handle* h, int n_sets, int q, int E, const double* mean, const double* cov, const double* linf,
+                   const vzgp_qacq* qa, uint64_t seed, double* score, double* mu, double* sigma);
 int prepare_scalarization(vzgp_handle* h, const vzgp_scalarization* sc);
 int launch_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, double* score, double* mu_out,
                        double* sigma_out);

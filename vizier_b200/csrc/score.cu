@@ -730,18 +730,33 @@ __global__ void __launch_bounds__(256) k_general_finalize(GeneralArgs a) {
   if (a.linf) a.linf[m] = dist;
 }
 
+int general_chunk_buffers(vzgp_handle* h, GeneralChunk* c) {
+  const int np = h->np, dc = h->dc, dk = h->dk;
+  const size_t nks = (size_t)kGeneralChunk * np, nx = (size_t)kGeneralChunk * (dc > 0 ? dc : 1);
+  VZ_TRY(h->gen.reserve(sizeof(double) * (2 * nks + nx) + sizeof(int32_t) * (size_t)kGeneralChunk * (dk > 0 ? dk : 1)));
+  c->Ks = h->gen.as<double>();
+  c->W = c->Ks + nks;
+  c->Xp = c->W + nks;
+  c->Zp = reinterpret_cast<int32_t*>(c->Xp + nx);
+  return 0;
+}
+
+int launch_general_chunk(vzgp_handle* h, const double* Xs, const int32_t* Zs, int mc, const GeneralChunk& c) {
+  const int np = h->np, dc = h->dc, dk = h->dk, mp = round_up(mc, 64);
+  if (dc > 0) VZ_TRY(launch_pad_rows(h, Xs, mc, dc, mp, c.Xp));
+  if (dk > 0) VZ_TRY(launch_pad_rows_i32(h, Zs, mc, dk, mp, c.Zp));
+  VZ_TRY(launch_cross_kernel(h, c.Xp, c.Zp, mp, h->X.as<double>(), h->Z.as<int32_t>(), np, h->n_valid, h->kp, c.Ks, np));
+  return launch_gemm_nt_tri(h, c.Ks, np, mp, h->Linv.as<double>(), np, np, c.W, np);
+}
+
 static int launch_score_general(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
                                 const AcqFn* fn, double* score, double* mu, double* sigma, double* linf) {
   const int np = h->np, dc = h->dc, dk = h->dk;
-  constexpr int kChunk = 4096;
-  const size_t nks = (size_t)kChunk * np, nx = (size_t)kChunk * (dc > 0 ? dc : 1);
-  VZ_TRY(h->gen.reserve(sizeof(double) * (2 * nks + nx) + sizeof(int32_t) * (size_t)kChunk * (dk > 0 ? dk : 1)));
-  double* Ks = h->gen.as<double>();
-  double* W = Ks + nks;
-  double* Xp = W + nks;
-  int32_t* Zp = reinterpret_cast<int32_t*>(Xp + nx);
+  constexpr int kChunk = kGeneralChunk;
+  GeneralChunk c;
+  VZ_TRY(general_chunk_buffers(h, &c));
   GeneralArgs a;
-  a.Ks = Ks; a.W = W; a.Xs = Xp; a.X = h->X.as<double>(); a.alpha = h->alpha.as<double>();
+  a.Ks = c.Ks; a.W = c.W; a.Xs = c.Xp; a.X = h->X.as<double>(); a.alpha = h->alpha.as<double>();
   a.np = np; a.n_valid = h->n_valid; a.dc = dc; a.kp = h->kp; a.sn2 = h->sn2; a.mean_const = h->mean_const;
   a.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient); a.radius = acq->trust_radius;
   a.apply_tr = acq->use_trust_region ? 1 : 0;
@@ -751,11 +766,8 @@ static int launch_score_general(vzgp_handle* h, const double* Xs, const int32_t*
   for (int d = 0; d < kMaxDc; ++d) a.tr_mask[d] = (d < dc) ? (acq->tr_dim_mask ? (acq->tr_dim_mask[d] ? 1 : 0) : 1) : 0;
   a.clamp_count = h->small.as<int>();
   for (int m0 = 0; m0 < M; m0 += kChunk) {
-    const int mc = M - m0 < kChunk ? M - m0 : kChunk, mp = round_up(mc, 64);
-    if (dc > 0) VZ_TRY(launch_pad_rows(h, Xs + (size_t)m0 * dc, mc, dc, mp, Xp));
-    if (dk > 0) VZ_TRY(launch_pad_rows_i32(h, Zs + (size_t)m0 * dk, mc, dk, mp, Zp));
-    VZ_TRY(launch_cross_kernel(h, Xp, Zp, mp, h->X.as<double>(), h->Z.as<int32_t>(), np, h->n_valid, h->kp, Ks, np));
-    VZ_TRY(launch_gemm_nt_tri(h, Ks, np, mp, h->Linv.as<double>(), np, np, W, np));
+    const int mc = M - m0 < kChunk ? M - m0 : kChunk;
+    VZ_TRY(launch_general_chunk(h, dc > 0 ? Xs + (size_t)m0 * dc : Xs, dk > 0 ? Zs + (size_t)m0 * dk : Zs, mc, c));
     a.mc = mc;
     a.score = score + m0; a.mu = mu ? mu + m0 : nullptr; a.sigma = sigma ? sigma + m0 : nullptr;
     a.linf = linf ? linf + m0 : nullptr;

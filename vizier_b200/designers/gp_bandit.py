@@ -21,7 +21,11 @@ gp/gp_models.py:91-140, :245-300; gp/transfer_learning.py), scored through `vzgp
 `scoring_function_factory` (e.g. `acquisitions.bayesian_scoring_function_factory(lambda d: EI(get_best_labels(d.labels)))`
 or `AcquisitionTrustRegion.default_ucb_pi`) selects UCB, LCB, EI, PI or a thresholded pair of those; the device
 scoring kernels evaluate it (`acquisitions.lower_acquisition`).  Multi-metric problems keep their scalarised UCB.
-Not implemented (the reference supports them; SURVEY 8f "next"): parallel (q-) acquisitions, other acquisition
+`scoring_function_is_parallel=True` with a factory returning `QEI`, `QPI` or `QUCB` suggests one set of `count` points
+(gp_bandit.py:496-499): Monte Carlo estimates over each set's joint posterior, scored by `vzgp_score_qsets`
+(csrc/score_q.cu) inside the n_parallel Eagle loop or the random strategy (`optimizers.optimize_qsets`).
+Not implemented (the reference supports them; SURVEY 8f "next"): parallel acquisitions for multi-metric models or
+with priors, other acquisition
 functions (MaxValueEntropySearch, Sample, user callables), non-independent multi-task kernels, priors for multi-metric or ensemble models; each raises NotImplementedError
 instead of silently doing something else.  Categorical parameters ARE supported
 end to end.  `padding_schedule` is accepted and has no numerical effect here: the kernels take
@@ -111,8 +115,11 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     self._ensemble_size = int(ensemble_size or 1)
     if self._ensemble_size < 1 or self._ensemble_size > ard_random_restarts:
       raise ValueError('ensemble_size must be in [1, ard_random_restarts].')
-    if scoring_function_is_parallel:
-      raise NotImplementedError('parallel (q-) scoring functions are not implemented.')
+    # gp_bandit.py:496-499: a parallel scoring function scores sets of `count` points (QEI / QPI / QUCB)
+    self._parallel = bool(scoring_function_is_parallel)
+    if self._parallel and (self._n_metrics > 1 or scoring_function_factory is None):
+      raise NotImplementedError('parallel (q-) scoring functions need a single metric and a scoring_function_factory '
+                                'returning QEI, QPI or QUCB.')
     if self._n_metrics > 1 and self._ensemble_size > 1:
       raise NotImplementedError('ensembles of multi-metric models are not implemented.')
     del padding_schedule, multitask_type
@@ -135,7 +142,7 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     self._acquisition_optimizer = acquisition_optimizer_factory(self._converter)
     if self._scoring_function_factory is not None:
       empty = acq_lib.ModelData(features=None, labels=acq_lib.PaddedArray.as_padded(np.zeros((0, self._n_metrics))))
-      acq_lib.check_supported(self._scoring_function(empty).acquisition_fn)
+      acq_lib.check_supported(self._scoring_function(empty).acquisition_fn, parallel=self._parallel)
     # Scalarisation weights are drawn once per designer (gp_bandit.py:217-222: one weights_rng): |N(0,1)|,
     # rows normalised to unit L2 norm (acquisitions.py:585-589).
     self._scal_weights = None
@@ -164,8 +171,9 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     labels, each further one on the residuals of its study against the stack below (gp/gp_models.py:245-300).  The
     current study's GP is later trained on ITS residuals against the whole prior stack (`_update_gp`).  Each call
     retrains the prior stack from scratch on what it is given."""
-    if self._n_metrics != 1 or self._ensemble_size != 1 or self._linear_coef:
-      raise NotImplementedError('transfer-learning priors: single-metric, single-model Matern GPs only.')
+    if self._n_metrics != 1 or self._ensemble_size != 1 or self._linear_coef or self._parallel:
+      raise NotImplementedError('transfer-learning priors: single-metric, single-model Matern GPs with pointwise '
+                                'acquisitions only.')
     if self._stack is not None:
       self._stack.close()
     self._stack = gp.StackedGP(self._device_index)
@@ -297,23 +305,43 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     seed = int(self._rng.integers(2**62))
     res = self._acquisition_optimizer(dev, acq, count=count, prior_features=None if prior is None else prior[0],
                                       prior_categorical=None if prior is None else prior[1], seed=seed)
-    trials = []
     order = np.argsort(-res.rewards, kind='stable')
-    for ind in order:
-      params = self._converter.to_parameters(
-          res.features[ind:ind + 1], None if res.categorical is None else res.categorical[ind:ind + 1])[0]
-      trial = vz.Trial(parameters=params)
-      md = trial.metadata.ns('devinfo')
-      aux = {k: float(v[ind]) for k, v in res.aux.items()}
-      md['acquisition_optimization'] = json.dumps({'acquisition': float(res.rewards[ind])} | aux)
-      failed_fit = any(getattr(m, 'cholesky_failed', False) for m in getattr(dev, 'members', [dev]))
-      if failed_fit or np.isnan([res.rewards[ind], *aux.values()]).any():
-        md['acquisition_optimization_warning'] = (
-            'NaNs encountered in acquisition optimization. See the "acquisition_optimization" field in the '
-            'metadata for more details.')
-      trial.complete(vz.Measurement({'acquisition': float(res.rewards[ind])}))
-      trials.append(trial)
-    return trials
+    return [self._result_trial(dev, res, ind) for ind in order]
+
+  def _result_trial(self, dev, res: vb.VectorizedStrategyResults, ind: int):
+    """Row `ind` of the optimiser's result as a completed trial carrying its acquisition value and aux arrays."""
+    params = self._converter.to_parameters(
+        res.features[ind:ind + 1], None if res.categorical is None else res.categorical[ind:ind + 1])[0]
+    trial = vz.Trial(parameters=params)
+    md = trial.metadata.ns('devinfo')
+    aux = {k: float(v[ind]) for k, v in res.aux.items()}
+    md['acquisition_optimization'] = json.dumps({'acquisition': float(res.rewards[ind])} | aux)
+    failed_fit = any(getattr(m, 'cholesky_failed', False) for m in getattr(dev, 'members', [dev]))
+    if failed_fit or np.isnan([res.rewards[ind], *aux.values()]).any():
+      md['acquisition_optimization_warning'] = (
+          'NaNs encountered in acquisition optimization. See the "acquisition_optimization" field in the '
+          'metadata for more details.')
+    trial.complete(vz.Measurement({'acquisition': float(res.rewards[ind])}))
+    return trial
+
+  @profiler.record_runtime
+  def _optimize_parallel_acquisition(self, dev, count: int, labels: np.ndarray, features):
+    """gp_bandit.py:482-521 with a parallel scoring function: n_parallel = count, count = 1.  The best set's q points
+    become q trials, each carrying the set's acquisition value (vectorized_base.py:591-651)."""
+    prior = converters.trials_to_sorted_features(self._trials, self._converter, features)
+    seed = int(self._rng.integers(2**62))
+    acq_seed = int(self._rng.integers(2**62))   # one acquisition seed per optimiser run (vectorized_base.py:382-404)
+    data = acq_lib.ModelData(features=features, labels=acq_lib.PaddedArray.as_padded(labels))
+    sf = self._scoring_function(data)
+    region = acq_lib.make_acquisition(
+        labels.shape[0], self._converter.continuous_feasible_values(_MAX_NUM_FEASIBLE_VALUES_FOR_TRUST_REGION),
+        self._converter.n_continuous, self._converter.n_categorical, use_trust_region=self._use_trust_region)
+    qacq = acq_lib.lower_parallel_acquisition(sf.acquisition_fn, use_trust_region=region.use_trust_region,
+                                              trust_radius=region.trust_radius, tr_dim_mask=region.tr_dim_mask)
+    res = self._acquisition_optimizer.optimize_qsets(
+        dev, qacq, n_parallel=count, prior_features=None if prior is None else prior[0],
+        prior_categorical=None if prior is None else prior[1], seed=seed, acq_seed=acq_seed)
+    return [self._result_trial(dev, res, ind) for ind in range(count)]
 
   # ------------------------------------------------------------------ suggest / predict / sample
   @profiler.record_runtime
@@ -325,8 +353,11 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     start = datetime.datetime.now()
     cont, cat, labels = self._trials_to_data(self._trials)
     dev = self._update_gp(cont, cat, labels)
-    acq = self._acquisition(cont.shape[0], labels, features=(cont, cat))
-    best = self._optimize_acquisition(dev, acq, count, features=(cont, cat))
+    if self._parallel:
+      best = self._optimize_parallel_acquisition(dev, count, labels, (cont, cat))
+    else:
+      acq = self._acquisition(cont.shape[0], labels, features=(cont, cat))
+      best = self._optimize_acquisition(dev, acq, count, features=(cont, cat))
     out = []
     for t in best:
       t.metadata.ns(self._metadata_ns).ns('devinfo')['time_spent'] = f'{datetime.datetime.now() - start}'

@@ -197,6 +197,65 @@ class UcbPeAcquisition:
 
 
 @dataclasses.dataclass
+class QAcquisition:
+  """Parallel acquisition of sets of q points (QEI / QPI / QUCB, acquisitions.py:495-568) with the set trust region
+  of gp_ucb_pe.py:245-269; see vzgp_qacq in include/vzgp.h."""
+
+  kind: int                          # _lib.QACQ_QEI / QACQ_QPI / QACQ_QUCB
+  best_label: float = -np.inf        # QEI / QPI; -inf (no observation): E[max f]
+  coefficient: float = 1.8           # QUCB
+  num_samples: int = 100
+  use_trust_region: bool = False
+  trust_radius: float = 1.0
+  tr_dim_mask: Optional[np.ndarray] = None
+  tr_rows: int = 0
+
+  def _c(self, period: int = 0, cov_out: Optional[torch.Tensor] = None):
+    a = _lib.QAcq()
+    a.kind = int(self.kind)
+    a.best_label = float(self.best_label)
+    a.coefficient = float(self.coefficient)
+    a.num_samples = int(self.num_samples)
+    a.period = int(period)
+    a.use_trust_region = 1 if self.use_trust_region else 0
+    a.trust_radius = float(self.trust_radius)
+    a.tr_rows = int(self.tr_rows)
+    a.cov_out = None if cov_out is None else cov_out.data_ptr()
+    keep = None
+    if self.tr_dim_mask is not None:
+      keep = np.ascontiguousarray(np.asarray(self.tr_dim_mask).astype(np.uint8))
+      a.tr_dim_mask = keep.ctypes.data_as(C.POINTER(C.c_uint8))
+    else:
+      a.tr_dim_mask = None
+    return a, keep
+
+
+def _score_qsets(devs: Sequence['DeviceGP'], xs_sets, q: int, qacq: QAcquisition, seed: int, zs=None,
+                 period: int = 0, with_aux: bool = False, with_cov: bool = False) -> dict:
+  """`vzgp_score_qsets` over the uniform mixture of `devs` (one model: a list of one)."""
+  f = devs[0]
+  xst = f._dev(xs_sets, torch.float64).reshape(-1, f.dc)
+  zst = f._dev(zs, torch.int32).reshape(-1, f.dk) if (zs is not None and f.dk > 0) else None
+  m = xst.shape[0]
+  assert m % q == 0, 'xs_sets must hold whole sets of q points'
+  n_sets = m // q
+  res = {'score': torch.empty((n_sets,), dtype=torch.float64, device=f.device)}
+  if with_aux:
+    for k in ('mean', 'stddev', 'linf_distance'):
+      res[k] = torch.empty((m,), dtype=torch.float64, device=f.device)
+  if with_cov:
+    res['cov'] = torch.empty((len(devs), n_sets, q, q), dtype=torch.float64, device=f.device)
+  f._stream.wait_stream(torch.cuda.current_stream(f.device))
+  a, keep = qacq._c(period, res.get('cov'))
+  hs = (C.c_void_p * len(devs))(*[d._h for d in devs])
+  _lib.check('vzgp_score_qsets', f._lib.vzgp_score_qsets(
+      hs, len(devs), _ptr(xst), _ptr(zst), n_sets, int(q), C.byref(a), C.c_uint64(int(seed) & (2**64 - 1)),
+      _ptr(res['score']), _ptr(res.get('mean')), _ptr(res.get('stddev')), _ptr(res.get('linf_distance'))))
+  res['_inputs'] = (xst, zst, keep)
+  return res
+
+
+@dataclasses.dataclass
 class ScalarizedUcbAcquisition:
   """Hyper-volume scalarised UCB for multi-metric problems (gp_bandit.py:214-242); see vzgp_scalarization
   in include/vzgp.h.  weights [S, M] positive with unit-norm rows, reference_point [M], max_scalarized [S]."""
@@ -726,6 +785,27 @@ class DeviceGP:
     res['_inputs'] = (xst, keep)
     return res
 
+  def score_qsets(self, xs_sets, q: int, qacq: QAcquisition, seed: int, zs=None, period: int = 0,
+                  with_aux: bool = False, with_cov: bool = False) -> dict:
+    """q-acquisition of n_sets sets of q points: xs_sets [n_sets * q, Dc] (or [n_sets, q * Dc]), zs [n_sets * q, Dk].
+    The draws of a set depend on its position (index mod `period`; 0: n_sets) and `seed`.  Returns device tensors
+    {'score' [n_sets], ['mean', 'stddev', 'linf_distance' [n_sets * q]], ['cov' [1, n_sets, q, q]]}; asynchronous."""
+    return _score_qsets([self], xs_sets, q, qacq, seed, zs, period, with_aux, with_cov)
+
+  def qacq_from_moments(self, mean, cov, qacq: QAcquisition, seed: int, period: int = 0) -> torch.Tensor:
+    """The Monte Carlo stage alone: mean [E, n_sets, q], cov [E, n_sets, q, q] -> scores [n_sets] (device)."""
+    mt = self._dev(mean, torch.float64)
+    ct = self._dev(cov, torch.float64)
+    e, n_sets, q = mt.shape
+    assert ct.shape == (e, n_sets, q, q)
+    out = torch.empty((n_sets,), dtype=torch.float64, device=self.device)
+    a, keep = qacq._c(period)
+    _lib.check('vzgp_qacq_from_moments', self._lib.vzgp_qacq_from_moments(
+        self._h, n_sets, q, e, _ptr(mt), _ptr(ct), C.byref(a), C.c_uint64(int(seed) & (2**64 - 1)), _ptr(out)))
+    self.synchronize()
+    del keep
+    return out
+
   def eagle_run(self, cfg: '_lib.EagleConfig', acq, count: int, seed: int,
                 prior: Optional[Sequence] = None, prior_z: Optional[Sequence] = None, cat_sizes=None,
                 other: Optional['DeviceGP'] = None):
@@ -1019,6 +1099,11 @@ class EnsembleGP:
         _ptr(res.get('mean')), _ptr(res.get('stddev')), _ptr(res.get('linf_distance'))))
     res['_inputs'] = (xst, zst, keep)
     return res
+
+  def score_qsets(self, xs_sets, q: int, qacq: QAcquisition, seed: int, zs=None, period: int = 0,
+                  with_aux: bool = False, with_cov: bool = False) -> dict:
+    """`DeviceGP.score_qsets` under the uniform mixture of the members ('cov' [E, n_sets, q, q] per member)."""
+    return _score_qsets(self.members, xs_sets, q, qacq, seed, zs, period, with_aux, with_cov)
 
   def eagle_run(self, cfg, acq: Acquisition, count: int, seed: int, prior=None, prior_z=None, cat_sizes=None,
                 other=None):

@@ -135,11 +135,9 @@ class VectorizedOptimizer:
     rewards [q] (the set's acquisition value repeated), aux per point."""
     import torch
     q, d = int(n_parallel), self.n_continuous
-    if isinstance(self.strategy_factory, _RandomStrategyFactory) or self.n_categorical > 0 or q * d > 64 or q > 16:
+    if isinstance(self.strategy_factory, _RandomStrategyFactory):
       raise NotImplementedError('set acquisitions need the Eagle strategy, continuous features, n_parallel * Dc <= 64 '
                                 'and n_parallel <= 16')
-    cfg = self._eagle_config()
-    cfg.n_parallel = q
 
     def score(xs_flat):          # [B, q * Dc] device -> [B] device
       with torch.cuda.stream(dev._stream):
@@ -150,26 +148,82 @@ class VectorizedOptimizer:
           out = out + torch.as_tensor(vals, dtype=torch.float64, device=dev.device)
         return out
 
-    n_sets = 0 if prior_features is None else len(prior_features) // q
-    se = gp.SteppedEagle(dev, cfg, 1, seed, n_sets)
-    if n_sets > 0:
-      ps = np.ascontiguousarray(np.asarray(prior_features, np.float64)[: n_sets * q].reshape(n_sets, q * d))
-      se.seed(ps, None, score(dev._dev(ps, torch.float64)))
-    steps = (self.max_evaluations - 1) // self.suggestion_batch_size + 1
-    for _ in range(steps):
-      xs, _, rewards = se.ask()
-      r = score(xs)
-      with torch.cuda.stream(dev._stream):
-        rewards.copy_(r)
-      se.tell()
-    bx, _, bs = se.end()
-    best = bx[0].reshape(q, d)
+    best, bs = self._eagle_sets(dev, q, score, prior_features, seed)
     out = dev.score_set_pe(other, best, q, pe)
     dev.synchronize()
     aux = {k: out[k].cpu().numpy() for k in ('mean', 'stddev', 'stddev_from_all')}
     if prior_acquisition is not None:
       aux['prior_acq_values'] = np.asarray(prior_acquisition(best[None], np.zeros((1, q, 0), np.int32)), np.float64).reshape(-1)
-    return VectorizedStrategyResults(best, np.full(q, bs[0]), aux, categorical=np.zeros((q, 0), np.int32))
+    return VectorizedStrategyResults(best, np.full(q, bs), aux, categorical=np.zeros((q, 0), np.int32))
+
+  def _eagle_sets(self, dev, q: int, score: Callable, prior_features: Optional[np.ndarray], seed: int):
+    """The n_parallel form of the Eagle optimiser through the host-stepped loop (vectorized_base.py:331-377): a fly is
+    a set of q points and `score([B, q * Dc] device) -> [B] device` rates a batch of them.  prior_features [n, Dc] are
+    grouped into n // q consecutive sets (vectorized_base.py:108-122).  Returns the best set [q, Dc] and its score."""
+    import torch
+    d = self.n_continuous
+    if self.n_categorical > 0 or q * d > 64 or q > 16:
+      raise NotImplementedError('set acquisitions need the Eagle strategy, continuous features, n_parallel * Dc <= 64 '
+                                'and n_parallel <= 16')
+    cfg = self._eagle_config()
+    cfg.n_parallel = q
+    lead = getattr(dev, 'members', [dev])[0]     # an ensemble's optimiser state lives on its first member
+    n_sets = 0 if prior_features is None else len(prior_features) // q
+    se = gp.SteppedEagle(lead, cfg, 1, seed, n_sets)
+    if n_sets > 0:
+      ps = np.ascontiguousarray(np.asarray(prior_features, np.float64)[: n_sets * q].reshape(n_sets, q * d))
+      se.seed(ps, None, score(lead._dev(ps, torch.float64)))
+    steps = (self.max_evaluations - 1) // self.suggestion_batch_size + 1
+    for _ in range(steps):
+      xs, _, rewards = se.ask()
+      r = score(xs)
+      with torch.cuda.stream(lead._stream):
+        rewards.copy_(r)
+      se.tell()
+    bx, _, bs = se.end()
+    return bx[0].reshape(q, d), float(bs[0])
+
+  def optimize_qsets(self, dev, qacq: gp.QAcquisition, *, n_parallel: int, prior_features: Optional[np.ndarray] = None,
+                     prior_categorical: Optional[np.ndarray] = None, seed: int = 0,
+                     acq_seed: int = 0) -> VectorizedStrategyResults:
+    """`acquisition_optimizer(scoring_fn.score, ..., count=1, n_parallel=q)` with a parallel acquisition (QEI / QPI /
+    QUCB; vectorized_base.py:331-377): sets of q points scored by `score_qsets` (dev: DeviceGP or EnsembleGP) with
+    one acquisition seed for the whole run, so the draws depend on a set's position in its batch
+    (vectorized_base.py:382-404, :504-520).  Eagle: continuous features, n_parallel * Dc <= 64.  Random strategy: a
+    Philox pool of n_sets * q points (any features), scored at once, device top-1.  Returns the best set: features
+    [q, Dc], categorical [q, Dk], rewards [q] (the set's acquisition value repeated), aux per point."""
+    import torch
+    q, dc, dk = int(n_parallel), self.n_continuous, self.n_categorical
+    period = self.suggestion_batch_size
+    if q < 1 or q > 16:
+      raise NotImplementedError('parallel acquisitions need 1 <= n_parallel <= 16')
+    lead = getattr(dev, 'members', [dev])[0]
+    if isinstance(self.strategy_factory, _RandomStrategyFactory):
+      n_sets = ((self.max_evaluations - 1) // self.suggestion_batch_size + 1) * self.suggestion_batch_size
+      m = n_sets * q
+      xs = lead.random_pool(m, dc, seed) if dc else torch.zeros((m, 0), dtype=torch.float64, device=lead.device)
+      zs = lead.random_pool_cat(m, list(self.categorical_sizes), seed) if dk else None
+      out = dev.score_qsets(xs, q, qacq, acq_seed, zs=zs, period=period)
+      idx, _ = lead.topk(out['score'], 1)
+      rows = torch.arange(q, device=lead.device) + int(max(idx[0], 0)) * q
+      best = xs[rows].cpu().numpy()
+      best_z = zs[rows].cpu().numpy() if zs is not None else np.zeros((q, 0), np.int32)
+    else:
+      def score(xs_flat):      # [B, q * Dc] device -> [B] device
+        with torch.cuda.stream(lead._stream):
+          return dev.score_qsets(xs_flat.reshape(-1, dc), q, qacq, acq_seed, period=period)['score']
+
+      best, _ = self._eagle_sets(dev, q, score, prior_features, seed)
+      best_z = np.zeros((q, 0), np.int32)
+    # score_with_aux on the winning set (vectorized_base.py:504-526): one set at position 0
+    out = dev.score_qsets(best, q, qacq, acq_seed, zs=best_z if dk else None, period=period, with_aux=True)
+    dev.synchronize()
+    value = float(out['score'].cpu().numpy()[0])
+    aux = {'mean': out['mean'].cpu().numpy(), 'stddev': out['stddev'].cpu().numpy()}
+    if qacq.use_trust_region:
+      aux['linf_distance'] = out['linf_distance'].cpu().numpy()
+      aux['radius'] = np.full(q, qacq.trust_radius)
+    return VectorizedStrategyResults(best, np.full(q, value), aux, categorical=best_z)
 
   def __call__(self, dev: gp.DeviceGP, acq, *, count: int = 1,
                prior_features: Optional[np.ndarray] = None, prior_categorical: Optional[np.ndarray] = None,
