@@ -103,7 +103,7 @@ typedef struct vzgp_acq_fn {
 /* Sets the acquisition function of every later call on h that takes a vzgp_acq (vzgp_score and its host / top-k
  * variants, vzgp_suggest_host, vzgp_random_search, vzgp_eagle_run and the host-stepped loop's scoring); fn = NULL
  * restores UCB with vzgp_acq.ucb_coefficient (the default).  Multi-handle calls (ensemble, stack) use the setting
- * of hs[0].  GP-UCB-PE, set-PE and multi-metric calls ignore it.  Unknown kinds and a non-finite best_label for EI
+ * of hs[0].  GP-UCB-PE (single- and multi-metric), set-PE and multi-metric calls ignore it.  Unknown kinds and a non-finite best_label for EI
  * or PI are rejected with VZGP_ERR_ARG. */
 int vzgp_set_acquisition(vzgp_handle* h, const vzgp_acq_fn* fn);
 
@@ -267,6 +267,42 @@ typedef struct vzgp_scalarization {
   const double* max_scalarized;
   double ucb_coefficient;
 } vzgp_scalarization;
+
+/* Multi-metric GP-UCB-PE (gp_ucb_pe.py:344-381, :434-492) with model A fitted by vzgp_fit_multi (n_metrics metrics
+ * sharing sigma_A) and model B on completed + pending trials (its labels are irrelevant: a single-metric fit on zero
+ * labels will do):
+ *   mode 0: u_m = mu_A,m + ucb_coefficient * sigma_B, then the hyper-volume scalarisation of `scalarization` exactly
+ *           as vzgp_score_multi (floored at max_scalarized when given, mean over the rows; its ucb_coefficient is
+ *           ignored)
+ *   mode 1: sigma_B + agg_m( penalty_coefficient * min(mu_A,m + explore_coefficient * sigma_A - thresholds[m], 0) )
+ *           with agg = mean (AVERAGE), max (UNION) or min (INTERSECTION) (MultimetricPromisingRegionPenaltyType,
+ *           gp_ucb_pe.py:63-78)
+ * followed by the strict trust region of :221-242 over the first tr_rows rows of B, as in vzgp_pe_params. */
+typedef enum vzgp_region_penalty {
+  VZGP_REGION_AVERAGE = 0,
+  VZGP_REGION_UNION = 1,
+  VZGP_REGION_INTERSECTION = 2
+} vzgp_region_penalty;
+typedef struct vzgp_pe_multi_params {
+  int mode;
+  double ucb_coefficient;       /* 1.8  (mode 0) */
+  double explore_coefficient;   /* 0.5  (mode 1) */
+  double penalty_coefficient;   /* 10.0 (mode 1) */
+  int use_trust_region;
+  double trust_radius;
+  const uint8_t* tr_dim_mask;   /* host [Dc] or NULL */
+  int tr_rows;                  /* 0 = all rows of B */
+  int n_metrics;                /* must equal model A's */
+  const double* thresholds;     /* host [n_metrics] (mode 1): _compute_ucb_threshold per metric (:175-218) */
+  int region_penalty;           /* vzgp_region_penalty (mode 1) */
+  const vzgp_scalarization* scalarization;   /* mode 0 */
+} vzgp_pe_multi_params;
+
+/* Scores M device candidates: score [M] required; mu [n_metrics x M] metric-major, sigma (model A) and sigma_all
+ * (model B) [M] optional; all device.  Mode 0 uploads the scalarisation tables (synchronises once), then
+ * asynchronous. */
+int vzgp_score_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
+                        const vzgp_pe_multi_params* pe, double* score, double* mu, double* sigma, double* sigma_all);
 
 /* Copy the fitted factor / alpha out (device destinations). */
 int vzgp_get_cholesky(vzgp_handle* h, double* L, int ldl);
@@ -527,6 +563,12 @@ int vzgp_eagle_run_pe(vzgp_handle* hA, vzgp_handle* hB, const vzgp_eagle_config*
                       const vzgp_pe_params* pe, const double* prior, const int32_t* prior_z, int n_prior,
                       const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
                       double* best_score);
+/* The same with the multi-metric GP-UCB-PE acquisition (vzgp_score_pe_multi); always the replayed-graph form of
+ * the loop. */
+int vzgp_eagle_run_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const vzgp_eagle_config* cfg,
+                            const vzgp_pe_multi_params* pe, const double* prior, const int32_t* prior_z, int n_prior,
+                            const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
+                            double* best_score);
 
 /* RandomVectorizedStrategy with batch = max_evaluations = M
  * (random_vectorized_optimizer.py:32-123): generates M uniform candidates on

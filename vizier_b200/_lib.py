@@ -118,6 +118,26 @@ class Scalarization(C.Structure):
   ]
 
 
+REGION_AVERAGE, REGION_UNION, REGION_INTERSECTION = 0, 1, 2   # vzgp_region_penalty
+
+
+class PeMultiParams(C.Structure):
+  _fields_ = [
+      ('mode', C.c_int),
+      ('ucb_coefficient', C.c_double),
+      ('explore_coefficient', C.c_double),
+      ('penalty_coefficient', C.c_double),
+      ('use_trust_region', C.c_int),
+      ('trust_radius', C.c_double),
+      ('tr_dim_mask', C.POINTER(C.c_uint8)),
+      ('tr_rows', C.c_int),
+      ('n_metrics', C.c_int),
+      ('thresholds', C.POINTER(C.c_double)),
+      ('region_penalty', C.c_int),
+      ('scalarization', C.POINTER(Scalarization)),
+  ]
+
+
 class EagleConfig(C.Structure):
   _fields_ = [
       ('visibility', C.c_double),
@@ -213,6 +233,9 @@ SIGNATURES = {
     'vzgp_eagle_run': (_i, [_vp, _pE, _pA, _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32, _pd]),
     'vzgp_score_pe': (_i, [_vp, _vp, _vp, _vp, _i, _pPE, _vp, _vp, _vp, _vp]),
     'vzgp_eagle_run_pe': (_i, [_vp, _vp, _pE, _pPE, _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32, _pd]),
+    'vzgp_score_pe_multi': (_i, [_vp, _vp, _vp, _vp, _i, C.POINTER(PeMultiParams), _vp, _vp, _vp, _vp]),
+    'vzgp_eagle_run_pe_multi': (_i, [_vp, _vp, _pE, C.POINTER(PeMultiParams), _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32,
+                                     _pd]),
     'vzgp_score_stack': (_i, [C.POINTER(C.c_void_p), _i, _pd, _vp, _vp, _i, _pA, _vp, _vp, _vp, _vp]),
     'vzgp_eagle_run_stack': (_i, [C.POINTER(C.c_void_p), _i, _pd, _pE, _pA, _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32, _pd]),
     'vzgp_score_set_pe': (_i, [_vp, _vp, _vp, _i, _i, _pPE, _vp, _vp, _vp, _vp]),

@@ -464,7 +464,7 @@ int vzgp_destroy(vzgp_handle* h) {
   Guard g(h->device);
   cudaStreamSynchronize(h->stream);
   for (DevBuf* b : {&h->X, &h->Z, &h->L, &h->Linv, &h->alpha, &h->ypad, &h->Kws, &h->Tws, &h->Kinv, &h->XT,
-                    &h->scratch, &h->small, &h->xs_dev, &h->out_dev, &h->eagle, &h->pe_tmp,
+                    &h->scratch, &h->small, &h->xs_dev, &h->out_dev, &h->eagle, &h->pe_tmp, &h->pe_multi_tmp,
                     &h->LinvT, &h->df_tasks[0], &h->df_tasks[1], &h->df_flags, &h->df_S, &h->scal, &h->gen,
                     &h->i8_planes, &h->i8_scale, &h->i8_kdig})
     b->release();
@@ -1003,10 +1003,12 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
                           const vzgp_pe_params* pe, const double* prior, const int32_t* prior_z, int n_prior,
                           const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
                           double* best_score, vzgp_handle* const* ens = nullptr, int n_ens = 0,
-                          const vzgp_scalarization* scal = nullptr, const double* stack_alphas = nullptr) {
-  VZ_ARG(h && cfg && (acq || pe || scal) && best_score, "handle / pointers");
-  const AcqFn* fn = (pe || scal) ? nullptr : handle_acq(ens ? ens[0] : h);   // multi-handle calls: the setting of hs[0]
+                          const vzgp_scalarization* scal = nullptr, const double* stack_alphas = nullptr,
+                          const vzgp_pe_multi_params* pem = nullptr) {
+  VZ_ARG(h && cfg && (acq || pe || scal || pem) && best_score, "handle / pointers");
+  const AcqFn* fn = (pe || scal || pem) ? nullptr : handle_acq(ens ? ens[0] : h);   // multi-handle calls: the setting of hs[0]
   auto score_batch = [&](const double* xs, const int32_t* zs, int m, double* out) -> int {
+    if (pem) return launch_score_pe_multi(h, hB, xs, zs, m, pem, out, nullptr, nullptr, nullptr);
     if (scal) return launch_score_multi(h, xs, zs, m, out, nullptr, nullptr);
     if (pe) return launch_score_pe(h, hB, xs, zs, m, pe, out, nullptr, nullptr, nullptr);
     if (stack_alphas) return launch_score_stack(ens, n_ens, stack_alphas, xs, zs, m, acq, out, nullptr, nullptr, nullptr, fn);
@@ -1030,6 +1032,7 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
   double* chosen_r = es.chosen_r;
   int* ord = es.ord;
   if (scal) VZ_TRY(prepare_scalarization(h, scal));
+  if (pem) VZ_TRY(prepare_score_pe_multi(h, pem));
   VZ_TRY(launch_eagle_init(h, e));
   if (n_prior > 0) {
     VZ_TRY(score_batch(prior, Dk > 0 ? prior_z : nullptr, n_prior, prior_r));
@@ -1046,11 +1049,13 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
   // CUDA graph of the suggest -> score -> update sequence: the iteration counter and all state
   // live in device memory, so the launches are identical and the host only enqueues graphs.
   bool done = false;
-  if (n_ens <= 1 && !scal && !stack_alphas && eagle_persistent_eligible(h, pe ? hB : nullptr, e)) {
+  // the persistent and cooperative forms evaluate single-metric acquisitions only
+  const bool fused_ok = n_ens <= 1 && !scal && !stack_alphas && !pem;
+  if (fused_ok && eagle_persistent_eligible(h, pe ? hB : nullptr, e)) {
     // small study: the whole loop is one persistent single-CTA kernel
     VZ_TRY(launch_eagle_persistent64(h, pe ? hB : nullptr, e, acq, pe, steps, fn));
     done = true;
-  } else if (n_ens <= 1 && !scal && !stack_alphas && eagle_grid_eligible(h, pe ? hB : nullptr, e)) {
+  } else if (fused_ok && eagle_grid_eligible(h, pe ? hB : nullptr, e)) {
     // mid-size study: one cooperative launch, phases separated by grid barriers.  If the cooperative
     // launch is refused (nothing has run then) the launch-per-phase loop below takes over.
     done = launch_eagle_grid(h, pe ? hB : nullptr, e, acq, pe, steps, fn) == 0;
@@ -1267,6 +1272,41 @@ int vzgp_eagle_run_pe(vzgp_handle* hA, vzgp_handle* hB, const vzgp_eagle_config*
   VZ_TRY(check_pe(hA, hB, pe));
   return eagle_run_impl(hA, hB, cfg, nullptr, pe, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z,
                         best_score);
+}
+
+static int check_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const vzgp_pe_multi_params* pe) {
+  VZ_ARG(hA && hB && pe, "handles / pe");
+  if (!hA->fitted || !hB->fitted) { set_error("GP-UCB-PE scoring needs both models fitted"); return VZGP_ERR_STATE; }
+  VZ_ARG(hA->device == hB->device && hA->stream == hB->stream, "both models must share device and stream");
+  VZ_ARG(hA->dc == hB->dc && hA->dk == hB->dk, "both models must have the same feature dimensions");
+  VZ_ARG(pe->mode == 0 || pe->mode == 1, "mode");
+  VZ_ARG(pe->n_metrics >= 1 && pe->n_metrics <= kMaxMetrics, "1 <= n_metrics <= 8");
+  VZ_ARG(pe->n_metrics == hA->n_metrics, "n_metrics must equal the metrics model A was fitted with (vzgp_fit_multi)");
+  VZ_ARG(pe->mode != 1 || pe->thresholds != nullptr, "thresholds (mode 1)");
+  VZ_ARG(pe->mode != 1 || (pe->region_penalty >= VZGP_REGION_AVERAGE && pe->region_penalty <= VZGP_REGION_INTERSECTION),
+         "region_penalty");
+  VZ_ARG(pe->mode != 0 || pe->scalarization != nullptr, "scalarization (mode 0)");
+  return 0;
+}
+
+int vzgp_score_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
+                        const vzgp_pe_multi_params* pe, double* score, double* mu, double* sigma, double* sigma_all) {
+  VZ_TRY(check_pe_multi(hA, hB, pe));
+  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
+  VZ_ARG(M == 0 || Xs != nullptr || hA->dc == 0, "Xs");
+  VZ_ARG(M == 0 || Zs != nullptr || hA->dk == 0, "Zs");
+  Guard g(hA->device);
+  VZ_TRY(prepare_score_pe_multi(hA, pe));
+  return launch_score_pe_multi(hA, hB, Xs, Zs, M, pe, score, mu, sigma, sigma_all);
+}
+
+int vzgp_eagle_run_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const vzgp_eagle_config* cfg,
+                            const vzgp_pe_multi_params* pe, const double* prior, const int32_t* prior_z, int n_prior,
+                            const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
+                            double* best_score) {
+  VZ_TRY(check_pe_multi(hA, hB, pe));
+  return eagle_run_impl(hA, hB, cfg, nullptr, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z,
+                        best_score, nullptr, 0, nullptr, nullptr, pe);
 }
 
 static int check_ensemble(vzgp_handle* const* hs, int E) {

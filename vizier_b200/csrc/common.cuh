@@ -146,6 +146,7 @@ struct vzgp_handle {
   vzgp::DevBuf eagle;   // eagle state
   void* eagle_step = nullptr;   // EagleStepState (c_abi.cu) of a host-stepped optimiser run
   vzgp::DevBuf pe_tmp;  // GP-UCB-PE: per-candidate pieces of the two models
+  vzgp::DevBuf pe_multi_tmp;  // multi-metric GP-UCB-PE (multi.cu): mu_A [n_metrics][M], sigma_A, sigma_B, L-inf, dummies
   vzgp::DevBuf gen;     // general scoring path: explicit K* and W chunks
   vzgp::DevBuf qmom;    // q-acquisitions (score_q.cu): per-member set means and covariance blocks, L-inf distances
   vzgp::DevBuf scal;    // multi-metric: [S][M] inverse scalarisation weights, then [S] best observed values

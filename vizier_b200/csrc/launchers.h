@@ -111,6 +111,9 @@ int launch_qacq_mc(vzgp_handle* h, int n_sets, int q, int E, const double* mean,
 int prepare_scalarization(vzgp_handle* h, const vzgp_scalarization* sc);
 int launch_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, double* score, double* mu_out,
                        double* sigma_out);
+int prepare_score_pe_multi(vzgp_handle* hA, const vzgp_pe_multi_params* pe);
+int launch_score_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
+                          const vzgp_pe_multi_params* pe, double* score, double* mu, double* sigma, double* sigma_all);
 int launch_random_fill(vzgp_handle* h, double* X, int64_t total, int64_t elem_base, uint64_t seed,
                        uint32_t stream, uint32_t iteration);
 struct ArgMax {

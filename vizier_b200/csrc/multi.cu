@@ -77,24 +77,21 @@ __global__ void __launch_bounds__(256) k_mean_multi(const double* __restrict__ X
     }
 }
 
-// weights_inv [S][M] = 1 / w_sm, best [S] (max over the observed labels of the scalarisation).
-__global__ void __launch_bounds__(256) k_scalarize(int M, ScalArgs a, const double* __restrict__ mu, int mpad,
-                                                   const double* __restrict__ sigma,
-                                                   const double* __restrict__ weights_inv,
-                                                   const double* __restrict__ best, double* __restrict__ score) {
-  extern __shared__ double sw[];   // [S][M] inverse weights, then [S] best
+// Stages the scalarisation tables of `a` into shared memory: [S][M] inverse weights, then [S] best.
+__device__ __forceinline__ void stage_scalarization(const ScalArgs& a, const double* __restrict__ weights_inv,
+                                                    const double* __restrict__ best, double* sw) {
   const int nm = a.n_metrics, S = a.n_scal;
   for (int e = threadIdx.x; e < S * nm; e += blockDim.x) sw[e] = weights_inv[e];
   double* sbest = sw + S * nm;
   if (a.has_max) for (int e = threadIdx.x; e < S; e += blockDim.x) sbest[e] = best[e];
-  __syncthreads();
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= M) return;
-  double u[kMaxMetrics];
-  const double sd = sigma[c];
-#pragma unroll
-  for (int m = 0; m < kMaxMetrics; ++m)
-    u[m] = (m < nm) ? fmax(fma(a.coef, sd, mu[(size_t)m * mpad + c]) - a.ref[m], 0.0) : 0.0;
+}
+
+// mean_s max( (min_m u_m / w_sm) ^ n_metrics, best_s ) for u_m already shifted by the reference point and
+// clamped at 0; sw as staged by stage_scalarization.
+__device__ __forceinline__ double scalarized_mean(const ScalArgs& a, const double (&u)[kMaxMetrics],
+                                                  const double* sw) {
+  const int nm = a.n_metrics, S = a.n_scal;
+  const double* sbest = sw + S * nm;
   double total = 0.0;
   for (int s = 0; s < S; ++s) {
     double mn = u[0] * sw[s * nm];
@@ -106,7 +103,81 @@ __global__ void __launch_bounds__(256) k_scalarize(int M, ScalArgs a, const doub
     if (a.has_max) pw = fmax(pw, sbest[s]);
     total += pw;
   }
-  score[c] = total / S;
+  return total / S;
+}
+
+// weights_inv [S][M] = 1 / w_sm, best [S] (max over the observed labels of the scalarisation).
+__global__ void __launch_bounds__(256) k_scalarize(int M, ScalArgs a, const double* __restrict__ mu, int mpad,
+                                                   const double* __restrict__ sigma,
+                                                   const double* __restrict__ weights_inv,
+                                                   const double* __restrict__ best, double* __restrict__ score) {
+  extern __shared__ double sw[];   // [S][M] inverse weights, then [S] best
+  const int nm = a.n_metrics;
+  stage_scalarization(a, weights_inv, best, sw);
+  __syncthreads();
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= M) return;
+  double u[kMaxMetrics];
+  const double sd = sigma[c];
+#pragma unroll
+  for (int m = 0; m < kMaxMetrics; ++m)
+    u[m] = (m < nm) ? fmax(fma(a.coef, sd, mu[(size_t)m * mpad + c]) - a.ref[m], 0.0) : 0.0;
+  score[c] = scalarized_mean(a, u, sw);
+}
+
+// Multi-metric GP-UCB-PE (gp_ucb_pe.py:344-381, :434-492, :63-78) on the pieces of models A and B.  sigma is shared
+// by the metrics of the independent multi-task GP, so mean_m(stddev_B) is stddev_B itself.
+//   mode 0: u_m = mu_A,m + ucb sigma_B, then the floored mean HV scalarisation (as k_scalarize)
+//   mode 1: sigma_B + agg_m( penalty min(mu_A,m + explore sigma_A - thr_m, 0) ),  agg = mean / max / min
+// followed by the strict trust region of :221-242.
+struct PeMultiCombine {
+  int mode, agg, apply_tr;
+  double explore, penalty, radius;
+  double thr[kMaxMetrics];
+};
+__global__ void __launch_bounds__(256) k_pe_multi_combine(int M, PeMultiCombine p, ScalArgs a,
+                                                          const double* __restrict__ mu, int mpad,
+                                                          const double* __restrict__ sd_a,
+                                                          const double* __restrict__ sd_b,
+                                                          const double* __restrict__ linf,
+                                                          const double* __restrict__ weights_inv,
+                                                          const double* __restrict__ best,
+                                                          double* __restrict__ score) {
+  extern __shared__ double sw[];   // mode 0: the scalarisation tables
+  const int nm = a.n_metrics;
+  if (p.mode == 0) stage_scalarization(a, weights_inv, best, sw);
+  __syncthreads();
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= M) return;
+  const double sb = sd_b[c];
+  double acq;
+  if (p.mode == 0) {
+    double u[kMaxMetrics];
+#pragma unroll
+    for (int m = 0; m < kMaxMetrics; ++m)
+      u[m] = (m < nm) ? fmax(fma(a.coef, sb, mu[(size_t)m * mpad + c]) - a.ref[m], 0.0) : 0.0;
+    acq = scalarized_mean(a, u, sw);
+  } else {
+    const double sa = sd_a[c];
+    double agg = 0.0;
+#pragma unroll
+    for (int m = 0; m < kMaxMetrics; ++m) {
+      if (m >= nm) continue;
+      const double pen = p.penalty * fmin(fma(sa, p.explore, mu[(size_t)m * mpad + c]) - p.thr[m], 0.0);
+      if (m == 0) agg = pen;
+      else if (p.agg == VZGP_REGION_UNION) agg = fmax(agg, pen);
+      else if (p.agg == VZGP_REGION_INTERSECTION) agg = fmin(agg, pen);
+      else agg += pen;
+    }
+    if (p.agg == VZGP_REGION_AVERAGE) agg /= nm;
+    acq = sb + agg;
+  }
+  if (p.apply_tr) {
+    const double dist = linf[c];
+    const bool inside = (dist < p.radius) || (p.radius > 0.5);
+    acq = inside ? acq : (-1e4 - dist);
+  }
+  score[c] = acq;
 }
 
 // Uploads 1 / weights and the best observed scalarised values, keeps the small parameters in the handle.
@@ -130,6 +201,16 @@ int prepare_scalarization(vzgp_handle* h, const vzgp_scalarization* sc) {
   return 0;
 }
 
+// mu [n_metrics][M] of the M candidates on the model fitted on `h` (k_mean_multi; not counted in h->launches).
+static int launch_mean_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, double* mu) {
+  const size_t sm = sizeof(double) * (2 * h->dc * 66 + kMaxMetrics * 64) + sizeof(int32_t) * 2 * h->dk * 66;
+  VZ_TRY(raise_dyn_smem((const void*)k_mean_multi, sm));
+  k_mean_multi<<<(M + 63) / 64, 256, sm, h->stream>>>(Xs, Zs, M, h->X.as<double>(), h->Z.as<int32_t>(), h->np, h->n_valid,
+                                                      h->kp, h->alpha.as<double>(), h->n_metrics, mu, M);
+  VZ_CHECK_LAUNCH();
+  return 0;
+}
+
 // Scores M candidates with the scalarisation last prepared on `h`.  mu_out: optional [n_metrics][M]
 // (leading dimension M); sigma_out optional [M].  Asynchronous, capturable.
 int launch_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, double* score, double* mu_out,
@@ -149,17 +230,71 @@ int launch_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int 
   none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0; none.tr_dim_mask = nullptr;
   none.tr_rows = 0; none.tr_strict = 0;
   VZ_TRY(launch_score(h, Xs, Zs, M, &none, dummy, nullptr, sd, nullptr));
-  const size_t sm = sizeof(double) * (2 * h->dc * 66 + kMaxMetrics * 64) + sizeof(int32_t) * 2 * h->dk * 66;
-  VZ_TRY(raise_dyn_smem((const void*)k_mean_multi, sm));
-  k_mean_multi<<<(M + 63) / 64, 256, sm, h->stream>>>(Xs, Zs, M, h->X.as<double>(), h->Z.as<int32_t>(), h->np, h->n_valid,
-                                                      h->kp, h->alpha.as<double>(), nm, mu, M);
-  VZ_CHECK_LAUNCH();
+  VZ_TRY(launch_mean_multi(h, Xs, Zs, M, mu));
   const size_t sm2 = sizeof(double) * (wn + S);
   VZ_TRY(raise_dyn_smem((const void*)k_scalarize, sm2));
   k_scalarize<<<(M + 255) / 256, 256, sm2, h->stream>>>(M, a, mu, M, sd, h->scal.as<double>(),
                                                         h->scal.as<double>() + wn, score);
   VZ_CHECK_LAUNCH();
   h->launches += 2;
+  return 0;
+}
+
+// Multi-metric GP-UCB-PE, mode 0: uploads the scalarisation of `pe` to hA (synchronises, not capturable).  Mode 1
+// carries everything it needs in the kernel arguments.  Call once before a loop of launch_score_pe_multi.
+int prepare_score_pe_multi(vzgp_handle* hA, const vzgp_pe_multi_params* pe) {
+  if (pe->mode == 0) VZ_TRY(prepare_scalarization(hA, pe->scalarization));
+  return 0;
+}
+
+// sigma_A (launch_score on A) -> mu_A,m (k_mean_multi on A) -> sigma_B and the L-inf distance to the first tr_rows
+// trials of B (launch_score on B) -> k_pe_multi_combine.  Optional outputs: mu [n_metrics][M], sigma / sigma_all [M].
+// Asynchronous, capturable; the intermediate pieces live in hA->pe_multi_tmp, which none of the launchers called
+// here touches.
+int launch_score_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
+                          const vzgp_pe_multi_params* pe, double* score, double* mu, double* sigma, double* sigma_all) {
+  if (M <= 0) return 0;
+  const int nm = hA->n_metrics;
+  ScalArgs a;
+  if (pe->mode == 0) {
+    a = hA->scal_args;
+    if (a.n_metrics != nm || a.n_scal < 1) {
+      set_error("multi-metric GP-UCB-PE (mode 0) without a prepared scalarization");
+      return VZGP_ERR_STATE;
+    }
+    a.coef = pe->ucb_coefficient;
+  } else {
+    a.n_metrics = nm; a.n_scal = 0; a.has_max = 0; a.coef = pe->ucb_coefficient;
+  }
+  VZ_TRY(hA->pe_multi_tmp.reserve(sizeof(double) * ((size_t)nm + 5) * (size_t)M));
+  double* t = hA->pe_multi_tmp.as<double>();
+  double* mu_a = mu ? mu : t;
+  double* sd_a = sigma ? sigma : t + (size_t)nm * M;
+  double* sd_b = sigma_all ? sigma_all : t + ((size_t)nm + 1) * M;
+  double* linf_b = t + ((size_t)nm + 2) * M;
+  double* dummy_a = t + ((size_t)nm + 3) * M;
+  double* dummy_b = t + ((size_t)nm + 4) * M;
+  vzgp_acq none;
+  none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0; none.tr_dim_mask = nullptr;
+  none.tr_rows = 0; none.tr_strict = 0;
+  VZ_TRY(launch_score(hA, Xs, Zs, M, &none, dummy_a, nullptr, sd_a, nullptr));
+  VZ_TRY(launch_mean_multi(hA, Xs, Zs, M, mu_a));
+  vzgp_acq accb = none;
+  accb.tr_dim_mask = pe->tr_dim_mask;
+  accb.tr_rows = pe->tr_rows;
+  const bool want_tr = pe->use_trust_region && pe->trust_radius <= 0.5;
+  VZ_TRY(launch_score(hB, Xs, Zs, M, &accb, dummy_b, nullptr, sd_b, want_tr ? linf_b : nullptr));
+  PeMultiCombine p;
+  p.mode = pe->mode; p.agg = pe->region_penalty; p.apply_tr = want_tr ? 1 : 0;
+  p.explore = pe->explore_coefficient; p.penalty = pe->penalty_coefficient; p.radius = pe->trust_radius;
+  for (int m = 0; m < kMaxMetrics; ++m) p.thr[m] = (pe->mode == 1 && m < nm) ? pe->thresholds[m] : 0.0;
+  const size_t wn = (size_t)a.n_scal * nm;
+  const size_t sm = pe->mode == 0 ? sizeof(double) * (wn + a.n_scal) : 0;
+  if (sm) VZ_TRY(raise_dyn_smem((const void*)k_pe_multi_combine, sm));
+  k_pe_multi_combine<<<(M + 255) / 256, 256, sm, hA->stream>>>(M, p, a, mu_a, M, sd_a, sd_b, linf_b,
+                                                               hA->scal.as<double>(), hA->scal.as<double>() + wn, score);
+  VZ_CHECK_LAUNCH();
+  hA->launches += 2;
   return 0;
 }
 

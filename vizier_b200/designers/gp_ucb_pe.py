@@ -20,8 +20,18 @@ like `VizierGPBandit`.  `prior_acquisition` (a callable on NumPy features) is ad
 host-stepped Eagle loop (`gp.SteppedEagle`); `optimize_set_acquisition_for_exploration=True` optimises the rest of a
 batch as ONE set for the set-PE acquisition (`vzgp_score_set_pe`, the optimiser's n_parallel form; continuous search
 spaces with count * Dc <= 64); `mixes_linear_kernel=True` uses the Matern + linear kernel with a constant mean
-(`linear_coef = 1`, libvzgp's general scoring path).  Not implemented: multi-metric, ensembles - each raises
-NotImplementedError.
+(`linear_coef = 1`, libvzgp's general scoring path).
+
+Multi-metric studies (up to 8 metrics, gp_ucb_pe.py:344-381, :434-492, :701-722, :917-942) use one default output
+warper per metric and model A is the independent multi-task GP (one factor, one alpha per metric; ARD on the summed
+losses).  UCB is the hyper-volume scalarisation of mean_A,m + 1.8 stddev_B over 1000 weight rows drawn afresh for
+each UCB suggestion, floored at the best scalarised label and averaged; PE is stddev_B plus the per-metric penalties
+(thresholds per metric) combined by `multimetric_promising_region_penalty_type` (AVERAGE / UNION / INTERSECTION).
+The strict trust region stays on.  Both run in `vzgp_score_pe_multi` / `vzgp_eagle_run_pe_multi`; `sample` returns
+[num_samples, n, num_metrics] and the prediction metadata holds per-metric vectors.
+
+Not implemented: ensembles (NotImplementedError); with several metrics also `mixes_linear_kernel`, task kernels other
+than INDEPENDENT (NotImplementedError) and `optimize_set_acquisition_for_exploration` (ValueError, as in the reference).
 """
 
 from __future__ import annotations
@@ -29,12 +39,14 @@ from __future__ import annotations
 import copy
 import dataclasses
 import datetime
+import enum
 import json
 import random
 from typing import Any, Optional, Sequence
 
 import numpy as np
 
+from vizier_b200 import _lib
 from vizier_b200 import acquisitions as acq_lib
 from vizier_b200 import ard
 from vizier_b200 import converters
@@ -48,9 +60,26 @@ from vizier_b200.designers import gp_bandit as _gpb
 _MAX_NUM_FEASIBLE_VALUES_FOR_TRUST_REGION = 1000
 
 
+class MultimetricPromisingRegionPenaltyType(enum.Enum):
+  """gp_ucb_pe.py:63-78: how the PE penalties of the metrics' promising regions combine."""
+
+  UNION = 'union'                  # max over the metrics: penalised outside the union of the regions
+  INTERSECTION = 'intersection'    # min over the metrics: penalised outside any of the regions
+  AVERAGE = 'average'              # mean over the metrics
+
+
+_REGION_PENALTY_CODE = {
+    MultimetricPromisingRegionPenaltyType.AVERAGE: _lib.REGION_AVERAGE,
+    MultimetricPromisingRegionPenaltyType.UNION: _lib.REGION_UNION,
+    MultimetricPromisingRegionPenaltyType.INTERSECTION: _lib.REGION_INTERSECTION,
+}
+_NUM_SCALARIZATIONS = 1000   # UCBScoreFunction's default (gp_ucb_pe.py:282-340)
+
+
 @dataclasses.dataclass(frozen=True)
 class UCBPEConfig:
-  """gp_ucb_pe.py:80-135 (single-metric fields)."""
+  """gp_ucb_pe.py:80-135.  `multitask_type`: only the INDEPENDENT multi-task kernel (a name or an enum member with
+  that name) is implemented for several metrics."""
 
   ucb_coefficient: float = 1.8
   explore_region_ucb_coefficient: float = 0.5
@@ -60,6 +89,9 @@ class UCBPEConfig:
   pe_overwrite_probability_in_high_noise: float = 0.7
   signal_to_noise_threshold: float = 0.7
   optimize_set_acquisition_for_exploration: bool = False
+  multimetric_promising_region_penalty_type: MultimetricPromisingRegionPenaltyType = (
+      MultimetricPromisingRegionPenaltyType.AVERAGE)
+  multitask_type: Any = 'INDEPENDENT'
 
 
 # gp_ucb_pe.py:678-698
@@ -90,6 +122,12 @@ def default_ard_optimizer() -> ard.ScipyLbfgsB:
   return ard.ScipyLbfgsB(ard.LbfgsBOptions(num_line_search_steps=20, tol=1e-5, maxiter=500))
 
 
+def _json_value(v):
+  """A scalar, or the per-metric vector of a multi-metric aux entry, as a JSON value."""
+  a = np.asarray(v, np.float64)
+  return float(a) if a.ndim == 0 else [float(x) for x in a]
+
+
 def _has_new_completed_trials(completed: Sequence[Any], active: Sequence[Any]) -> bool:
   """gp_ucb_pe.py:142-172."""
   if not completed:
@@ -116,8 +154,22 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
                metadata_ns: str = 'google_gp_ucb_pe_bandit', device: int = 0):
     if problem.search_space.is_conditional:
       raise ValueError(f'{type(self)} does not support conditional search.')
-    if len(problem.metric_information) != 1:
-      raise NotImplementedError('vizier_b200.VizierGPUCBPEBandit implements the single-metric path only.')
+    self._n_metrics = len(problem.metric_information)
+    if self._n_metrics > 1:
+      # gp_ucb_pe.py:701-722
+      if config.optimize_set_acquisition_for_exploration:
+        raise ValueError(f'{type(self)} works with exactly one metric when '
+                         '`optimize_set_acquisition_for_exploration` is enabled.')
+      if self._n_metrics > 8:
+        raise NotImplementedError('at most 8 metrics (libvzgp kMaxMetrics).')
+      mt = config.multitask_type
+      if mt not in (None, 'INDEPENDENT') and getattr(mt, 'name', '') != 'INDEPENDENT':
+        raise NotImplementedError('only the INDEPENDENT multi-task kernel (the default) is implemented.')
+      if mixes_linear_kernel:
+        raise NotImplementedError('mixes_linear_kernel with several metrics is not implemented.')
+      if not isinstance(config.multimetric_promising_region_penalty_type, MultimetricPromisingRegionPenaltyType):
+        raise ValueError('Unsupported multimetric promising region penalty type: '
+                         f'{config.multimetric_promising_region_penalty_type}')
     if (ensemble_size or 1) != 1:
       raise NotImplementedError('ensembles are not implemented for GP-UCB-PE.')
     # mixes_linear_kernel: the Matern + feature-scaled linear kernel with a constant mean, linear_coef = 1
@@ -142,6 +194,7 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     self._all_completed_trials: list = []
     self._all_active_trials: Sequence[Any] = []
     self._output_warper = None
+    self._output_warpers: list = []        # one per metric (gp_ucb_pe.py:917-942)
     self._device_index = device
     self._dev_a: Optional[gp.DeviceGP] = None
     self._dev_b: Optional[gp.DeviceGP] = None
@@ -181,11 +234,14 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
 
   @profiler.record_runtime
   def _trials_to_data(self, trials):
-    """gp_ucb_pe.py:917-942: a fresh default warper per call."""
+    """gp_ucb_pe.py:917-942: a fresh default warper per metric and call; labels [N, n_metrics]."""
     (cont, cat), labels = self._converter.to_xy_cached(trials)   # completed trials: owned deep copies
-    self._output_warper = output_warpers.create_default_warper()
-    warped = self._output_warper.warp(labels[:, 0:1]) if labels.shape[0] else labels[:, 0:1]
-    return cont, cat, warped
+    self._output_warpers = [output_warpers.create_default_warper() for _ in range(self._n_metrics)]
+    self._output_warper = self._output_warpers[0]
+    if not labels.shape[0]:
+      return cont, cat, labels[:, :self._n_metrics]
+    warped = [w.warp(labels[:, i:i + 1]) for i, w in enumerate(self._output_warpers)]
+    return cont, cat, warped[0] if self._n_metrics == 1 else np.concatenate(warped, axis=-1)
 
   @profiler.record_runtime
   def _build_gp_model_and_optimize_parameters(self, cont, cat, labels) -> gp.GPHyperParams:
@@ -203,7 +259,9 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     dev_a, _ = self._devices()
     import torch  # device-memory handles only
     xt = torch.from_numpy(np.ascontiguousarray(cont)).to(dev_a.device)
-    yt = torch.from_numpy(np.ascontiguousarray(labels[:, 0])).to(dev_a.device)
+    # [N], or [N, n_metrics] for the independent multi-task GP (the losses sum over the metrics)
+    y = labels[:, 0] if self._n_metrics == 1 else labels
+    yt = torch.from_numpy(np.ascontiguousarray(y)).to(dev_a.device)
     zt = torch.from_numpy(np.ascontiguousarray(cat)).to(dev_a.device) if dk else None
     lo, hi = gp.param_bounds(dc, dk, bool(lin))
     if lin:
@@ -222,16 +280,62 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     return gp.GPHyperParams.from_vector(best[0], dc, dk, lin)
 
   def _fit_all_features(self, params: gp.GPHyperParams, cont, cat, labels, pend_c, pend_z, noise_is_high: bool):
-    """_get_predictive_all_features (:944-1004): model B on completed + pending, dummy labels."""
+    """_get_predictive_all_features (:944-1004): model B on completed + pending, dummy labels.  Its stddev does not
+    depend on the labels, so a multi-metric study fits B as one metric on zeros."""
     _, dev_b = self._devices()
     xc = np.concatenate([cont, pend_c], axis=0)
     xz = np.concatenate([cat, pend_z], axis=0)
-    y = np.concatenate([labels[:, 0], np.zeros(pend_c.shape[0])])
+    if self._n_metrics == 1:
+      y = np.concatenate([labels[:, 0], np.zeros(pend_c.shape[0])])
+    else:
+      y = np.zeros(xc.shape[0])
     p = params
     if noise_is_high:
       p = dataclasses.replace(params, observation_noise_variance=1e-10)
     dev_b.fit(xc, y, p, z=xz if xz.shape[1] else None)
     return xc, xz
+
+  def _fit_labels(self, labels):
+    """Labels for DeviceGP.fit: [N] for one metric, [N, n_metrics] for the independent multi-task GP."""
+    return labels[:, 0] if self._n_metrics == 1 else labels
+
+  def _prediction_str(self, v) -> str:
+    """A prediction metadata value: repr of the float, or np.array2string of the per-metric vector (:1134-1144; the
+    stddev shared by the metrics of the independent multi-task GP is repeated per metric)."""
+    if self._n_metrics == 1:
+      return repr(float(v))
+    return np.array2string(np.broadcast_to(np.asarray(v, np.float64), (self._n_metrics,)), separator=',')
+
+  def _multi_metric_acquisition(self, use_ucb: bool, labels, xc_all, xz_all, mask, radius, n_tr_rows):
+    """UCBScoreFunction / PEScoreFunction of a multi-metric study (gp_ucb_pe.py:282-381, :434-492)."""
+    cfg = self._config
+    dev_a, _ = self._devices()
+    nm = self._n_metrics
+    common = dict(n_metrics=nm, ucb_coefficient=cfg.ucb_coefficient, explore_coefficient=cfg.explore_region_ucb_coefficient,
+                  penalty_coefficient=cfg.cb_violation_penalty_coefficient, use_trust_region=self._use_trust_region,
+                  trust_radius=radius, tr_dim_mask=mask, tr_rows=n_tr_rows)
+    if use_ucb:
+      # fresh HV scalarisation weights per UCB suggestion (:1057; acquisitions.create_hv_scalarization): |N(0, 1)|,
+      # rows of unit L2 norm, the reference point of the warped labels, floored at the best scalarised label
+      g = np.random.default_rng(int(self._rng.integers(2**62)))
+      w = np.abs(g.standard_normal((_NUM_SCALARIZATIONS, nm)))
+      w = w / np.linalg.norm(w, axis=-1, keepdims=True)
+      ref = acq_lib.hv_reference_point(labels, 0.01)
+      best = acq_lib.hv_scalarize(labels, w, ref).max(axis=-1)
+      sc = gp.ScalarizedUcbAcquisition(w, ref, best, cfg.ucb_coefficient)
+      return gp.UcbPeMultiAcquisition(mode=0, scalarization=sc, **common)
+    # _compute_ucb_threshold (:175-218) per metric: mean_m of A at B's feature with the largest UCB_A of metric m.  The
+    # means and the shared stddev come from the scalarised scorer's aux outputs (its score is not used).
+    probe = gp.ScalarizedUcbAcquisition(np.full((1, nm), 1.0 / np.sqrt(nm)), np.zeros(nm), None, 0.0)
+    out = dev_a.score_multi(xc_all, probe, zs=xz_all, with_aux=True)
+    dev_a.synchronize()
+    mu = out['mean'].cpu().numpy()
+    sd = out['stddev'].cpu().numpy()
+    best_idx = np.argmax(mu + cfg.ucb_coefficient * sd[None, :], axis=1)
+    thresholds = mu[np.arange(nm), best_idx]
+    return gp.UcbPeMultiAcquisition(
+        mode=1, thresholds=thresholds, region_penalty=_REGION_PENALTY_CODE[cfg.multimetric_promising_region_penalty_type],
+        **common)
 
   @profiler.record_runtime
   def _suggest_one(self, active_trials, cont, cat, labels, params, mask, radius, n_tr_rows):
@@ -253,18 +357,21 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     has_model = cont.shape[0] + pend_c.shape[0] > 0
     xc_all, xz_all = self._fit_all_features(params, cont, cat, labels, pend_c, pend_z, noise_is_high) if has_model else (cont, cat)
     dk = cat.shape[1]
-    threshold = 0.0
-    if not use_ucb and cont.shape[0] > 0:
-      # _compute_ucb_threshold (:175-218): mean of A at B's feature with the largest UCB_A
-      out = dev_a.score(xc_all, gp.Acquisition(cfg.ucb_coefficient, False, 1.0), zs=xz_all if dk else None, with_aux=True)
-      dev_a.synchronize()
-      mu = out['mean'].cpu().numpy(); sd = out['stddev'].cpu().numpy()
-      threshold = float(mu[int(np.argmax(mu + cfg.ucb_coefficient * sd))])
-    pe = gp.UcbPeAcquisition(
-        mode=0 if use_ucb else 1, ucb_coefficient=cfg.ucb_coefficient,
-        explore_coefficient=cfg.explore_region_ucb_coefficient,
-        penalty_coefficient=cfg.cb_violation_penalty_coefficient, threshold=threshold,
-        use_trust_region=self._use_trust_region, trust_radius=radius, tr_dim_mask=mask, tr_rows=n_tr_rows)
+    if self._n_metrics > 1:
+      pe = self._multi_metric_acquisition(use_ucb, labels, xc_all, xz_all if dk else None, mask, radius, n_tr_rows)
+    else:
+      threshold = 0.0
+      if not use_ucb and cont.shape[0] > 0:
+        # _compute_ucb_threshold (:175-218): mean of A at B's feature with the largest UCB_A
+        out = dev_a.score(xc_all, gp.Acquisition(cfg.ucb_coefficient, False, 1.0), zs=xz_all if dk else None, with_aux=True)
+        dev_a.synchronize()
+        mu = out['mean'].cpu().numpy(); sd = out['stddev'].cpu().numpy()
+        threshold = float(mu[int(np.argmax(mu + cfg.ucb_coefficient * sd))])
+      pe = gp.UcbPeAcquisition(
+          mode=0 if use_ucb else 1, ucb_coefficient=cfg.ucb_coefficient,
+          explore_coefficient=cfg.explore_region_ucb_coefficient,
+          penalty_coefficient=cfg.cb_violation_penalty_coefficient, threshold=threshold,
+          use_trust_region=self._use_trust_region, trust_radius=radius, tr_dim_mask=mask, tr_rows=n_tr_rows)
     optimizer = self._acquisition_optimizer_factory(self._converter)
     prior = converters.trials_to_sorted_features(self._all_completed_trials, self._converter, (cont, cat))
     seed = int(self._rng.integers(2**62))
@@ -274,11 +381,11 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     params_dict = self._converter.to_parameters(res.features[0:1], None if res.categorical is None else res.categorical[0:1])[0]
     md = vz.Metadata()
     md.ns('devinfo')['acquisition_optimization'] = json.dumps(
-        {'acquisition': float(res.rewards[0])} | {k: float(v[0]) for k, v in res.aux.items()})
+        {'acquisition': float(res.rewards[0])} | {k: _json_value(v[0]) for k, v in res.aux.items()})
     pred = md.ns(self._metadata_ns).ns('prediction_in_warped_y_space')
-    pred['mean'] = repr(float(res.aux['mean'][0]))
-    pred['stddev'] = repr(float(res.aux['stddev'][0]))
-    pred['stddev_from_all'] = repr(float(res.aux['stddev_from_all'][0]))
+    pred['mean'] = self._prediction_str(res.aux['mean'][0])
+    pred['stddev'] = self._prediction_str(res.aux['stddev'][0])
+    pred['stddev_from_all'] = self._prediction_str(res.aux['stddev_from_all'][0])
     pred['acquisition'] = f'{float(res.rewards[0])}'
     pred['use_ucb'] = f'{use_ucb}'
     pred['trust_radius'] = f'{radius}'
@@ -344,7 +451,7 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     dev_a, _ = self._devices()
     prior_only = cont.shape[0] == 0          # only ACTIVE trials so far (parallel workers at study start)
     if not prior_only:
-      dev_a.fit(cont, labels[:, 0], params, z=cat if cat.shape[1] else None)
+      dev_a.fit(cont, self._fit_labels(labels), params, z=cat if cat.shape[1] else None)
     act_c, _ = self._converter.to_features(self._all_active_trials)
     n_tr = cont.shape[0] + act_c.shape[0]   # trust region: completed + initially active trials (:1377-1403)
     mask = acq_lib.trust_region_dim_mask(self._converter.continuous_feasible_values(_MAX_NUM_FEASIBLE_VALUES_FOR_TRUST_REGION))
@@ -394,9 +501,9 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     md.ns('devinfo')['acquisition_optimization'] = json.dumps(
         {'acquisition': float(res.rewards[0]), 'mean': 0.0, 'stddev': prior_sd, 'stddev_from_all': sd_all})
     pred = md.ns(self._metadata_ns).ns('prediction_in_warped_y_space')
-    pred['mean'] = repr(0.0)
-    pred['stddev'] = repr(prior_sd)
-    pred['stddev_from_all'] = repr(sd_all)
+    pred['mean'] = self._prediction_str(0.0)
+    pred['stddev'] = self._prediction_str(prior_sd)
+    pred['stddev_from_all'] = self._prediction_str(sd_all)
     pred['acquisition'] = f'{float(res.rewards[0])}'
     pred['use_ucb'] = 'False'
     pred['trust_radius'] = f'{radius}'
@@ -408,20 +515,29 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
   @profiler.record_runtime
   def sample(self, trials: Sequence[Any], rng: Any = None, num_samples: int = 1000) -> np.ndarray:
     """gp_ucb_pe.py:1262-1329: unwarped joint posterior samples of the model on the COMPLETED trials
-    (re-trained like the reference does), shape (num_samples, num_trials)."""
+    (re-trained like the reference does), shape (num_samples, num_trials), or (num_samples, num_trials,
+    num_metrics) for a multi-metric study."""
     if not trials:
-      return np.zeros((num_samples, 0))
+      return np.zeros((num_samples, 0) if self._n_metrics == 1 else (num_samples, 0, self._n_metrics))
     cont, cat, labels = self._trials_to_data(self._all_completed_trials)
     if cont.shape[0] == 0:
       raise NotImplementedError('sample() before any completed trial is not implemented (prior-only GP).')
     params = self._build_gp_model_and_optimize_parameters(cont, cat, labels)
     dev_a, _ = self._devices()
-    dev_a.fit(cont, labels[:, 0], params, z=cat if cat.shape[1] else None)
+    dev_a.fit(cont, self._fit_labels(labels), params, z=cat if cat.shape[1] else None)
     xs, zs = self._converter.to_features(trials)
     xs = np.nan_to_num(xs, nan=0.0)
     mean, cov = dev_a.posterior(xs, zs if zs.shape[1] else None, add_noise=True)
     chol, _, _ = dev_a.cholesky_retry(cov, jitter=1e-10, max_iters=8)
     g = np.random.default_rng(_gpb._seed_from(rng) if rng is not None else 0)
+    if self._n_metrics > 1:
+      # independent multi-task GP: one shared covariance, a mean [n_metrics, n]; each metric unwarped by its own warper
+      mean, chol = mean.cpu().numpy(), chol.cpu().numpy()
+      out = np.empty((num_samples, mean.shape[1], self._n_metrics))
+      for m, warper in enumerate(self._output_warpers):
+        warped = mean[m][None, :] + g.standard_normal((num_samples, mean.shape[1])) @ chol.T
+        out[:, :, m] = warper.unwarp(warped.reshape(-1, 1)).reshape(num_samples, -1)
+      return out
     samples = mean.cpu().numpy()[None, :] + g.standard_normal((num_samples, mean.shape[0])) @ chol.cpu().numpy().T
     return self._output_warper.unwarp(samples.reshape(-1, 1)).reshape(samples.shape)
 

@@ -278,6 +278,58 @@ class ScalarizedUcbAcquisition:
     return s, (w, r, b)
 
 
+@dataclasses.dataclass
+class UcbPeMultiAcquisition:
+  """Multi-metric GP-UCB-PE acquisition (gp_ucb_pe.py:344-381, :434-492); see vzgp_pe_multi_params in
+  include/vzgp.h.  Mode 0 needs `scalarization` (its ucb_coefficient is not used: `ucb_coefficient` is), mode 1
+  the per-metric `thresholds` [n_metrics] and `region_penalty` (_lib.REGION_AVERAGE / UNION / INTERSECTION)."""
+
+  n_metrics: int
+  mode: int = 0                      # 0 = scalarised UCB (mean_A + c * stddev_B), 1 = PE
+  ucb_coefficient: float = 1.8
+  explore_coefficient: float = 0.5
+  penalty_coefficient: float = 10.0
+  thresholds: Optional[np.ndarray] = None
+  region_penalty: int = 0
+  scalarization: Optional[ScalarizedUcbAcquisition] = None
+  use_trust_region: bool = True
+  trust_radius: float = 1.0
+  tr_dim_mask: Optional[np.ndarray] = None
+  tr_rows: int = 0
+
+  def _c(self):
+    p = _lib.PeMultiParams()
+    p.mode = int(self.mode)
+    p.ucb_coefficient = float(self.ucb_coefficient)
+    p.explore_coefficient = float(self.explore_coefficient)
+    p.penalty_coefficient = float(self.penalty_coefficient)
+    p.use_trust_region = 1 if self.use_trust_region else 0
+    p.trust_radius = float(self.trust_radius)
+    p.tr_rows = int(self.tr_rows)
+    p.n_metrics = int(self.n_metrics)
+    p.region_penalty = int(self.region_penalty)
+    keep = []
+    if self.tr_dim_mask is not None:
+      mask = np.ascontiguousarray(np.asarray(self.tr_dim_mask).astype(np.uint8))
+      p.tr_dim_mask = mask.ctypes.data_as(C.POINTER(C.c_uint8))
+      keep.append(mask)
+    else:
+      p.tr_dim_mask = None
+    if self.thresholds is not None:
+      thr = np.ascontiguousarray(np.asarray(self.thresholds, np.float64).reshape(-1))
+      p.thresholds = thr.ctypes.data_as(C.POINTER(C.c_double))
+      keep.append(thr)
+    else:
+      p.thresholds = None
+    if self.scalarization is not None:
+      s, skeep = self.scalarization._c()
+      p.scalarization = C.pointer(s)
+      keep += [s, skeep]
+    else:
+      p.scalarization = None
+    return p, keep
+
+
 def _ptr(t: Optional[torch.Tensor]):
   return None if t is None else C.c_void_p(t.data_ptr())
 
@@ -766,6 +818,23 @@ class DeviceGP:
     del keep
     return res
 
+  def score_pe_multi(self, other: 'DeviceGP', xs, pe: UcbPeMultiAcquisition, zs=None) -> dict:
+    """Multi-metric GP-UCB-PE score with self = multi-metric model on completed trials, other = model on
+    completed + pending trials.  Returns device tensors {'score' [M], 'mean' [n_metrics, M], 'stddev' [M],
+    'stddev_from_all' [M]}; synchronous."""
+    xst, zst = self._xz(xs, zs)
+    m = xst.shape[0]
+    res = {k: torch.empty((m,), dtype=torch.float64, device=self.device) for k in ('score', 'stddev', 'stddev_from_all')}
+    res['mean'] = torch.empty((self.n_metrics, m), dtype=torch.float64, device=self.device)
+    self._stream.wait_stream(torch.cuda.current_stream(self.device))
+    p, keep = pe._c()
+    _lib.check('vzgp_score_pe_multi', self._lib.vzgp_score_pe_multi(
+        self._h, other._h, _ptr(xst), _ptr(zst), m, C.byref(p), _ptr(res['score']), _ptr(res['mean']),
+        _ptr(res['stddev']), _ptr(res['stddev_from_all'])))
+    self.synchronize()
+    del keep
+    return res
+
   def score_set_pe(self, other: 'DeviceGP', xs_sets, q: int, pe: UcbPeAcquisition) -> dict:
     """Set-PE acquisition (gp_ucb_pe.py:510-594) of n_sets sets of q points: xs_sets [n_sets * q, Dc] (or
     [n_sets, q * Dc]).  self = model on completed trials, other = model on completed + pending trials.  Returns
@@ -810,8 +879,9 @@ class DeviceGP:
                 prior: Optional[Sequence] = None, prior_z: Optional[Sequence] = None, cat_sizes=None,
                 other: Optional['DeviceGP'] = None):
     """Returns (best_x [count,Dc], best_z [count,Dk], best_score [count]).  With `other` and a
-    UcbPeAcquisition the GP-UCB-PE acquisition is optimised (vzgp_eagle_run_pe)."""
-    if isinstance(acq, UcbPeAcquisition):
+    UcbPeAcquisition the GP-UCB-PE acquisition is optimised (vzgp_eagle_run_pe), with a UcbPeMultiAcquisition its
+    multi-metric form (vzgp_eagle_run_pe_multi)."""
+    if isinstance(acq, (UcbPeAcquisition, UcbPeMultiAcquisition)):
       return self._eagle_run_pe(cfg, acq, count, seed, prior, prior_z, cat_sizes, other)
     multi = isinstance(acq, ScalarizedUcbAcquisition)
     if not multi:
@@ -833,7 +903,8 @@ class DeviceGP:
     del keep
     return bx, bz, bs
 
-  def _eagle_run_pe(self, cfg, pe: UcbPeAcquisition, count, seed, prior, prior_z, cat_sizes, other):
+  def _eagle_run_pe(self, cfg, pe, count, seed, prior, prior_z, cat_sizes, other):
+    fn_name = 'vzgp_eagle_run_pe_multi' if isinstance(pe, UcbPeMultiAcquisition) else 'vzgp_eagle_run_pe'
     p, keep = pe._c()
     n_prior = 0 if prior is None else len(prior)
     pt = self._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
@@ -842,7 +913,7 @@ class DeviceGP:
     bz = np.zeros((count, self.dk), np.int32)
     bs = np.zeros(count, np.float64)
     sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
-    _lib.check('vzgp_eagle_run_pe', self._lib.vzgp_eagle_run_pe(
+    _lib.check(fn_name, getattr(self._lib, fn_name)(
         self._h, other._h, C.byref(cfg), C.byref(p), _ptr(pt), _ptr(pz), n_prior,
         sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None, count, seed,
         bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),

@@ -99,11 +99,16 @@ class VectorizedOptimizer:
     per iteration; state, suggest and update stay on the device (gp.SteppedEagle)."""
     import torch
     is_pe = isinstance(acq, gp.UcbPeAcquisition)
+    is_pe_multi = isinstance(acq, gp.UcbPeMultiAcquisition)
     has_cat = self.n_categorical > 0
 
     def score(xs, zs):
       with torch.cuda.stream(dev._stream):
-        out = dev.score_pe(other, xs, acq, zs=zs if has_cat else None) if is_pe else dev.score(xs, acq, zs=zs if has_cat else None)
+        zq = zs if has_cat else None
+        if is_pe_multi:
+          out = dev.score_pe_multi(other, xs, acq, zs=zq)
+        else:
+          out = dev.score_pe(other, xs, acq, zs=zq) if is_pe else dev.score(xs, acq, zs=zq)
         xh = xs.cpu().numpy()
         zh = zs.cpu().numpy() if (has_cat and zs is not None) else np.zeros((xh.shape[0], 0), np.int32)
         vals = np.asarray(prior_acquisition(xh, zh), np.float64).reshape(-1)
@@ -229,10 +234,21 @@ class VectorizedOptimizer:
                prior_features: Optional[np.ndarray] = None, prior_categorical: Optional[np.ndarray] = None,
                seed: int = 0, other: Optional[gp.DeviceGP] = None,
                prior_acquisition: Optional[Callable] = None) -> VectorizedStrategyResults:
-    """acq: gp.Acquisition (UCB + trust region on `dev`) or gp.UcbPeAcquisition (needs `other`)."""
+    """acq: gp.Acquisition (UCB + trust region on `dev`), gp.ScalarizedUcbAcquisition, or gp.UcbPeAcquisition /
+    gp.UcbPeMultiAcquisition (both need `other`; the multi-metric aux 'mean' is [count, n_metrics])."""
     sizes = list(self.categorical_sizes)
-    is_pe = isinstance(acq, gp.UcbPeAcquisition)
+    is_pe = isinstance(acq, (gp.UcbPeAcquisition, gp.UcbPeMultiAcquisition))
     is_multi = isinstance(acq, gp.ScalarizedUcbAcquisition)
+
+    def pe_aux(bx, bz):
+      if isinstance(acq, gp.UcbPeMultiAcquisition):
+        out = dev.score_pe_multi(other, bx, acq, zs=bz if self.n_categorical else None)
+        aux = {k: out[k].cpu().numpy() for k in ('stddev', 'stddev_from_all')}
+        aux['mean'] = out['mean'].cpu().numpy().T
+        return aux
+      out = dev.score_pe(other, bx, acq, zs=bz if self.n_categorical else None)
+      return {k: out[k].cpu().numpy() for k in ('mean', 'stddev', 'stddev_from_all')}
+
     if prior_acquisition is not None:
       if is_multi or isinstance(self.strategy_factory, _RandomStrategyFactory):
         raise NotImplementedError('prior_acquisition is supported with the Eagle strategy on single-metric acquisitions')
@@ -240,8 +256,7 @@ class VectorizedOptimizer:
       zsel = bz if self.n_categorical else None
       prior_vals = np.asarray(prior_acquisition(bx, bz), np.float64).reshape(-1)
       if is_pe:
-        out = dev.score_pe(other, bx, acq, zs=zsel)
-        aux = {k: out[k].cpu().numpy() for k in ('mean', 'stddev', 'stddev_from_all')}
+        aux = pe_aux(bx, bz)
       else:
         out = dev.score(bx, acq, zs=zsel, with_aux=True)
         dev.synchronize()
@@ -272,9 +287,7 @@ class VectorizedOptimizer:
       bx, bz, bs = dev.eagle_run(cfg, acq, count, seed, prior=prior_features, prior_z=prior_categorical,
                                  cat_sizes=sizes, other=other)
     if is_pe:
-      out = dev.score_pe(other, bx, acq, zs=bz if self.n_categorical else None)
-      aux = {k: out[k].cpu().numpy() for k in ('mean', 'stddev', 'stddev_from_all')}
-      return VectorizedStrategyResults(bx, bs, aux, categorical=bz)
+      return VectorizedStrategyResults(bx, bs, pe_aux(bx, bz), categorical=bz)
     if is_multi:   # no trust region -> no aux (acquisitions.py:190-207)
       return VectorizedStrategyResults(bx, bs, {}, categorical=bz)
     # score_with_aux on the winners (vectorized_base.py:504-526)
