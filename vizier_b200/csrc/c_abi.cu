@@ -1250,17 +1250,10 @@ int vzgp_score_set_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, int n_
   double* sd_b = t + 5 * (size_t)M;
   double* mean_b = t + 6 * (size_t)M;
   double* cov = t + 7 * (size_t)M;
-  vzgp_acq none;
-  none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0; none.tr_dim_mask = nullptr;
-  none.tr_rows = 0; none.tr_strict = 0;
+  const vzgp_acq none = posterior_request(), accb = posterior_request(pe->tr_dim_mask, pe->tr_rows);
   VZ_TRY(launch_score(hA, Xs, nullptr, M, &none, dummy_a, mu_a, sd_a, nullptr));
-  const bool want_tr = pe->use_trust_region && pe->trust_radius <= 0.5;
-  if (want_tr) {
-    vzgp_acq accb = none;
-    accb.tr_dim_mask = pe->tr_dim_mask;
-    accb.tr_rows = pe->tr_rows;
-    VZ_TRY(launch_score(hB, Xs, nullptr, M, &accb, dummy_b, nullptr, sd_b, linf_b));
-  }
+  const bool want_tr = tr_needs_distance(trust_region_of(hB, *pe, true));
+  if (want_tr) VZ_TRY(launch_score(hB, Xs, nullptr, M, &accb, dummy_b, nullptr, sd_b, linf_b));
   VZ_TRY(vzgp_posterior_multi(hB, Xs, nullptr, M, 1, mean_b, cov, M));
   return launch_set_pe_combine(hA, n_sets, q, pe, cov, M, mu_a, sd_a, want_tr ? linf_b : nullptr, score, sigma_all);
 }

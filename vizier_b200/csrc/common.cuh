@@ -15,7 +15,6 @@
 namespace vzgp {
 
 constexpr int kBlk = 64;       // padding / factorisation block size
-constexpr int kMaxDc = 64;     // continuous feature dims supported by the tile kernels
 constexpr int kMaxDk = 32;     // categorical feature dims
 constexpr int kMaxMetrics = 8; // metrics of the independent multi-task GP (one factor, several alpha)
 constexpr int kNllBufs = 15;   // handle buffers a captured NLL graph points into

@@ -207,7 +207,7 @@ __device__ __forceinline__ void posterior_tile64(const SmallModel& m, const Mode
       if (i < B) {
         for (int d = 0; d < dc; ++d) {
           const double av = sm.cand[d * kPXLD + i], w = m.kp.inv_ls2_c[d];
-          const bool in_tr = want_linf && q.tr_mask[d];
+          const bool in_tr = want_linf && q.tr.mask[d];
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
             const double df = av - ms.xt[d * kPXLD + j0 + c];
@@ -229,7 +229,7 @@ __device__ __forceinline__ void posterior_tile64(const SmallModel& m, const Mode
         const double kv = (i < B && j < m.n_valid) ? matern52(d2[c], m.kp.sf2) : 0.0;
         sm.ks[i * kPLD + j] = kv;
         mu = fma(kv, ms.alpha[j], mu);
-        if (j < q.tr_rows) lmin = fmin(lmin, lf[c]);
+        if (j < q.tr.rows) lmin = fmin(lmin, lf[c]);
       }
 #pragma unroll
       for (int o = 1; o < 16; o <<= 1) {
@@ -289,15 +289,7 @@ __device__ __forceinline__ void score_batch64(const SmallModel& ma, const SmallM
   stage_candidates64(sm, ma.kp.dc, ma.kp.dk, cand, candz, B);
   if (q.pe_mode < 0) {
     posterior_tile64(ma, sm.a, sm, B, q, sm.mu, sm.sd, q.want_linf ? sm.linf : nullptr, clamp_count);
-    if (tid < B) {
-      double sc = acq_eval<GENERIC>(q.fn, sm.mu[tid], sm.sd[tid]);
-      if (q.apply_tr) {
-        const double dist = sm.linf[tid];
-        const bool inside = (q.tr_strict ? (dist < q.radius) : (dist <= q.radius)) || (q.radius > 0.5);
-        sc = inside ? sc : (-1e4 - dist);
-      }
-      out_score[tid] = sc;
-    }
+    if (tid < B) out_score[tid] = tr_apply(q.tr, acq_eval<GENERIC>(q.fn, sm.mu[tid], sm.sd[tid]), sm.linf[tid]);
   } else {
     posterior_tile64(ma, sm.a, sm, B, q, sm.mu, sm.sd, nullptr, clamp_count);
     posterior_tile64(mb, sm.b, sm, B, q, sm.mu + 64, sm.sd + 64, q.want_linf ? sm.linf : nullptr, clamp_count);
@@ -309,12 +301,7 @@ __device__ __forceinline__ void score_batch64(const SmallModel& ma, const SmallM
         const double explore_ucb = fma(sm.sd[tid], q.explore, sm.mu[tid]);
         acq = sm.sd[64 + tid] + q.penalty * fmin(explore_ucb - q.threshold, 0.0);
       }
-      if (q.want_linf) {
-        const double dist = sm.linf[tid];
-        const bool inside = (dist < q.radius) || (q.radius > 0.5);
-        acq = inside ? acq : (-1e4 - dist);
-      }
-      out_score[tid] = acq;
+      out_score[tid] = tr_apply(q.tr, acq, sm.linf[tid]);
     }
   }
   __syncthreads();
@@ -490,24 +477,17 @@ int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e
                               const vzgp_pe_params* pe, int steps, const AcqFn* fn) {
   const SmallModel m = small_model_of(h);
   const SmallModel mb = hB ? small_model_of(hB) : m;
-  const vzgp_handle* ht = pe ? hB : h;     // the trust region is measured on this model's trials
   SmallAcq q;
   memset(&q, 0, sizeof(q));
-  const uint8_t* mask;
-  int tr_rows;
-  if (pe) {
+  if (pe) {   // GP-UCB-PE: the trust region is measured on model B's trials
     q.pe_mode = pe->mode; q.coef = pe->ucb_coefficient; q.explore = pe->explore_coefficient;
     q.penalty = pe->penalty_coefficient; q.threshold = pe->threshold;
-    q.radius = pe->trust_radius; q.apply_tr = pe->use_trust_region ? 1 : 0; q.tr_strict = 1;
-    mask = pe->tr_dim_mask; tr_rows = pe->tr_rows;
+    q.tr = trust_region_of(hB, *pe, true);
   } else {
-    q.pe_mode = -1; q.fn = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
-    q.radius = acq->trust_radius; q.apply_tr = acq->use_trust_region ? 1 : 0; q.tr_strict = acq->tr_strict ? 1 : 0;
-    mask = acq->tr_dim_mask; tr_rows = acq->tr_rows;
+    q.pe_mode = -1; q.fn = acq_fn_of(acq, fn);
+    q.tr = trust_region_of(h, *acq, acq->tr_strict);
   }
-  q.tr_rows = (tr_rows > 0 && tr_rows < ht->n_valid) ? tr_rows : ht->n_valid;
-  q.want_linf = (q.apply_tr && q.radius <= 0.5) ? 1 : 0;
-  for (int d = 0; d < kMaxDc; ++d) q.tr_mask[d] = (d < h->dc) ? (mask ? (mask[d] ? 1 : 0) : 1) : 0;
+  q.want_linf = tr_needs_distance(q.tr) ? 1 : 0;
   const size_t es = sizeof(double) * (size_t)(kPThreads / 32) * (e.P + e.D) + sizeof(int32_t) * (kPThreads / 32) * (size_t)(e.Dk + 2);
   const size_t eu = eagle_update_smem(e);
   const size_t scratch = ((es > eu ? es : eu) + 15) / 16 * 2;   // doubles, 16-byte multiple

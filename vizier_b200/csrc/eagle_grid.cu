@@ -23,8 +23,8 @@ struct GridArgs {
   ScoreArgs b;        // model B (GP-UCB-PE only)
   int pe_mode;        // -1: UCB on a; 0 / 1: GP-UCB-PE (vzgp_pe_params.mode)
   int wl_a, wl_b;     // trust-region distance wanted from a / b
-  double ucb, explore, penalty, threshold, radius;
-  int apply_tr;       // GP-UCB-PE: strict trust region on b's distance
+  double ucb, explore, penalty, threshold;
+  TrustRegion tr;     // GP-UCB-PE: strict trust region on b's distance
   int steps;
   unsigned* barrier;  // zeroed by the host before the launch
 };
@@ -113,12 +113,7 @@ __global__ void __launch_bounds__(kSmallThreads) k_eagle_grid(const __grid_const
               const double explore_ucb = fma(g.a.sigma[m], g.explore, g.a.mu[m]);
               acq = g.b.sigma[m] + g.penalty * fmin(explore_ucb - g.threshold, 0.0);
             }
-            if (g.apply_tr) {
-              const double dist = g.b.linf[m];
-              const bool inside = (dist < g.radius) || (g.radius > 0.5);
-              acq = inside ? acq : (-1e4 - dist);
-            }
-            e.batch_r[m] = acq;
+            e.batch_r[m] = tr_apply(g.tr, acq, g.wl_b ? g.b.linf[m] : INFINITY);   // b.linf: only with the distance
           }
         }
       }
@@ -162,26 +157,21 @@ int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const 
     VZ_TRY(prepare_small_score(h, xs, zs, e.B, acq, e.batch_r, nullptr, nullptr, nullptr, &G.a, &wl, fn));
     G.b = G.a;
     G.pe_mode = -1; G.wl_a = wl ? 1 : 0; G.wl_b = 0;
-    G.ucb = G.explore = G.penalty = G.threshold = G.radius = 0.0; G.apply_tr = 0;
+    G.ucb = G.explore = G.penalty = G.threshold = 0.0; G.tr = TrustRegion{};
   } else {
     VZ_TRY(h->pe_tmp.reserve(sizeof(double) * 6 * (size_t)e.B));
     double* t = h->pe_tmp.as<double>();
     double* mu_a = t; double* sd_a = t + e.B; double* sd_b = t + 2 * (size_t)e.B;
     double* linf_b = t + 3 * (size_t)e.B; double* dummy_a = t + 4 * (size_t)e.B; double* dummy_b = t + 5 * (size_t)e.B;
-    vzgp_acq none;
-    none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0; none.tr_dim_mask = nullptr;
-    none.tr_rows = 0; none.tr_strict = 0;
+    const vzgp_acq none = posterior_request(), accb = posterior_request(pe->tr_dim_mask, pe->tr_rows);
+    G.tr = trust_region_of(hB, *pe, true);
     VZ_TRY(prepare_small_score(h, xs, zs, e.B, &none, dummy_a, mu_a, sd_a, nullptr, &G.a, &wl));
     G.wl_a = wl ? 1 : 0;
-    vzgp_acq accb = none;
-    accb.tr_dim_mask = pe->tr_dim_mask;
-    accb.tr_rows = pe->tr_rows;
-    const bool want_tr = pe->use_trust_region && pe->trust_radius <= 0.5;
-    VZ_TRY(prepare_small_score(hB, xs, zs, e.B, &accb, dummy_b, nullptr, sd_b, want_tr ? linf_b : nullptr, &G.b, &wl));
+    VZ_TRY(prepare_small_score(hB, xs, zs, e.B, &accb, dummy_b, nullptr, sd_b, tr_needs_distance(G.tr) ? linf_b : nullptr,
+                               &G.b, &wl));
     G.wl_b = wl ? 1 : 0;
     G.pe_mode = pe->mode; G.ucb = pe->ucb_coefficient; G.explore = pe->explore_coefficient;
-    G.penalty = pe->penalty_coefficient; G.threshold = pe->threshold; G.radius = pe->trust_radius;
-    G.apply_tr = want_tr ? 1 : 0;
+    G.penalty = pe->penalty_coefficient; G.threshold = pe->threshold;
   }
   // dynamic shared memory = the largest phase
   size_t sm = eagle_suggest_cta_smem(e);

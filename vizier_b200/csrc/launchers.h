@@ -74,6 +74,30 @@ int chol_dataflow(vzgp_handle* h, double* L, double* Linv, double* LinvT, double
 int chol_dataflow_prepare(vzgp_handle* h, int np, bool want_kinv);
 int chol_dataflow_timed_out(vzgp_handle* h, int* out);
 
+// The trust region of a scoring request (vzgp_acq, vzgp_pe_params, vzgp_pe_multi_params or vzgp_qacq), measured on
+// the trials of `trials`: tr_rows clamped to its valid rows, tr_dim_mask expanded over its dimensions.
+template <class P>
+TrustRegion trust_region_of(const vzgp_handle* trials, const P& p, bool strict) {
+  TrustRegion t;
+  t.apply = p.use_trust_region ? 1 : 0;
+  t.rows = (p.tr_rows > 0 && p.tr_rows < trials->n_valid) ? p.tr_rows : trials->n_valid;
+  t.strict = strict ? 1 : 0;
+  t.radius = p.trust_radius;
+  for (int d = 0; d < kMaxDc; ++d) t.mask[d] = (d < trials->dc) ? (p.tr_dim_mask ? (p.tr_dim_mask[d] ? 1 : 0) : 1) : 0;
+  return t;
+}
+// Whether the region can move a score, so the scoring call must compute the distances.
+inline bool tr_needs_distance(const TrustRegion& t) { return t.apply && t.radius <= 0.5; }
+
+// The posterior alone (UCB coefficient 0, no trust region), as the multi-model launchers score their members; `mask`
+// and `rows` select the distance such a call reports through `linf`.
+inline vzgp_acq posterior_request(const uint8_t* mask = nullptr, int rows = 0) {
+  vzgp_acq a;
+  a.ucb_coefficient = 0.0; a.use_trust_region = 0; a.trust_radius = 1.0; a.tr_dim_mask = mask;
+  a.tr_rows = rows; a.tr_strict = 0;
+  return a;
+}
+
 // The scoring launchers take the acquisition function as `fn`; nullptr means UCB with acq->ucb_coefficient (the
 // per-member scorings inside the ensemble, stack and GP-UCB-PE launchers rely on that).
 int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
@@ -173,11 +197,11 @@ struct SmallModel {
 };
 struct SmallAcq {
   AcqFn fn;                             // pe_mode < 0: acquisition function of (mean, stddev)
-  double coef, radius;                  // coef: GP-UCB-PE mode 0
+  double coef;                          // GP-UCB-PE mode 0
   double explore, penalty, threshold;   // GP-UCB-PE
   int pe_mode;                          // -1: UCB on one model; 0 / 1: GP-UCB-PE modes (vzgp_pe_params.mode)
-  int apply_tr, tr_rows, tr_strict, want_linf;
-  uint8_t tr_mask[kMaxDc];
+  int want_linf;
+  TrustRegion tr;
 };
 bool eagle_persistent_eligible(const vzgp_handle* h, const vzgp_handle* hB, const EagleDev& e);
 int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const vzgp_acq* acq,

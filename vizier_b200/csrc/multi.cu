@@ -131,9 +131,10 @@ __global__ void __launch_bounds__(256) k_scalarize(int M, ScalArgs a, const doub
 //   mode 1: sigma_B + agg_m( penalty min(mu_A,m + explore sigma_A - thr_m, 0) ),  agg = mean / max / min
 // followed by the strict trust region of :221-242.
 struct PeMultiCombine {
-  int mode, agg, apply_tr;
-  double explore, penalty, radius;
+  int mode, agg;
+  double explore, penalty;
   double thr[kMaxMetrics];
+  TrustRegion tr;
 };
 __global__ void __launch_bounds__(256) k_pe_multi_combine(int M, PeMultiCombine p, ScalArgs a,
                                                           const double* __restrict__ mu, int mpad,
@@ -172,12 +173,7 @@ __global__ void __launch_bounds__(256) k_pe_multi_combine(int M, PeMultiCombine 
     if (p.agg == VZGP_REGION_AVERAGE) agg /= nm;
     acq = sb + agg;
   }
-  if (p.apply_tr) {
-    const double dist = linf[c];
-    const bool inside = (dist < p.radius) || (p.radius > 0.5);
-    acq = inside ? acq : (-1e4 - dist);
-  }
-  score[c] = acq;
+  score[c] = tr_apply(p.tr, acq, linf[c]);
 }
 
 // Uploads 1 / weights and the best observed scalarised values, keeps the small parameters in the handle.
@@ -226,9 +222,7 @@ int launch_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int 
   double* mu = mu_out ? mu_out : t;
   double* sd = sigma_out ? sigma_out : t + (size_t)nm * M;
   double* dummy = t + ((size_t)nm + 1) * M;
-  vzgp_acq none;
-  none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0; none.tr_dim_mask = nullptr;
-  none.tr_rows = 0; none.tr_strict = 0;
+  const vzgp_acq none = posterior_request();
   VZ_TRY(launch_score(h, Xs, Zs, M, &none, dummy, nullptr, sd, nullptr));
   VZ_TRY(launch_mean_multi(h, Xs, Zs, M, mu));
   const size_t sm2 = sizeof(double) * (wn + S);
@@ -274,19 +268,14 @@ int launch_score_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, co
   double* linf_b = t + ((size_t)nm + 2) * M;
   double* dummy_a = t + ((size_t)nm + 3) * M;
   double* dummy_b = t + ((size_t)nm + 4) * M;
-  vzgp_acq none;
-  none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0; none.tr_dim_mask = nullptr;
-  none.tr_rows = 0; none.tr_strict = 0;
+  const vzgp_acq none = posterior_request(), accb = posterior_request(pe->tr_dim_mask, pe->tr_rows);
+  PeMultiCombine p;
+  p.mode = pe->mode; p.agg = pe->region_penalty;
+  p.explore = pe->explore_coefficient; p.penalty = pe->penalty_coefficient;
+  p.tr = trust_region_of(hB, *pe, true);
   VZ_TRY(launch_score(hA, Xs, Zs, M, &none, dummy_a, nullptr, sd_a, nullptr));
   VZ_TRY(launch_mean_multi(hA, Xs, Zs, M, mu_a));
-  vzgp_acq accb = none;
-  accb.tr_dim_mask = pe->tr_dim_mask;
-  accb.tr_rows = pe->tr_rows;
-  const bool want_tr = pe->use_trust_region && pe->trust_radius <= 0.5;
-  VZ_TRY(launch_score(hB, Xs, Zs, M, &accb, dummy_b, nullptr, sd_b, want_tr ? linf_b : nullptr));
-  PeMultiCombine p;
-  p.mode = pe->mode; p.agg = pe->region_penalty; p.apply_tr = want_tr ? 1 : 0;
-  p.explore = pe->explore_coefficient; p.penalty = pe->penalty_coefficient; p.radius = pe->trust_radius;
+  VZ_TRY(launch_score(hB, Xs, Zs, M, &accb, dummy_b, nullptr, sd_b, tr_needs_distance(p.tr) ? linf_b : nullptr));
   for (int m = 0; m < kMaxMetrics; ++m) p.thr[m] = (pe->mode == 1 && m < nm) ? pe->thresholds[m] : 0.0;
   const size_t wn = (size_t)a.n_scal * nm;
   const size_t sm = pe->mode == 0 ? sizeof(double) * (wn + a.n_scal) : 0;

@@ -124,7 +124,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   // ring or the barriers untouched is cluster-wide when ncta > 1.
   const unsigned crank = cluster_ctarank(), ncta = cluster_nctarank();
   auto tile_gate = [&]() { if (ncta > 1) cluster_sync(); else __syncthreads(); };
-  if (tid < kMaxDc) s_mask[tid] = a.tr_mask[tid];
+  if (tid < kMaxDc) s_mask[tid] = a.tr.mask[tid];
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) { mbar_init(full_bar + s, 1); mbar_init(empty_bar + s, ncta * (kThreads / 32)); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
@@ -280,7 +280,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
         for (int i = 0; i < 4; ++i)
 #pragma unroll
           for (int j = 0; j < 4; ++j)
-            if ((jb * 64 + GP1::col_of(tx, j)) < a.tr_rows) lmin[i] = fmin(lmin[i], lf[i][j]);
+            if ((jb * 64 + GP1::col_of(tx, j)) < a.tr.rows) lmin[i] = fmin(lmin[i], lf[i][j]);
       }
       // The sixteen kernel values as one straight-line block of the branch-free Matern (independent chains
       // the scheduler can interleave); columns at or past n_valid are zeroed by a select.
@@ -613,8 +613,8 @@ static int max_active_clusters(const void* kfn, const cudaLaunchConfig_t& cfg, i
   return 0;
 }
 
-static void fill_score_args(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
-                            const AcqFn* fn, double* score, double* mu, double* sigma, double* linf, ScoreArgs* pa) {
+void fill_score_args(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq, const AcqFn* fn,
+                     double* score, double* mu, double* sigma, double* linf, ScoreArgs* pa) {
   ScoreArgs& a = *pa;
   const int ntiles = (M + kTM - 1) / kTM;
   a.Xs = Xs; a.Zs = Zs; a.M = M;
@@ -623,13 +623,8 @@ static void fill_score_args(vzgp_handle* h, const double* Xs, const int32_t* Zs,
   a.Linv = h->Linv.as<double>(); a.ldi = h->np;
   a.alpha = h->alpha.as<double>();
   a.kp = h->kp; a.sn2 = h->sn2;
-  a.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
-  a.apply_tr = acq->use_trust_region ? 1 : 0;
-  a.tr_rows = (acq->tr_rows > 0 && acq->tr_rows < h->n_valid) ? acq->tr_rows : h->n_valid;
-  a.tr_strict = acq->tr_strict ? 1 : 0;
-  a.radius = acq->trust_radius;
-  for (int d = 0; d < kMaxDc; ++d)
-    a.tr_mask[d] = (d < h->dc) ? (acq->tr_dim_mask ? (acq->tr_dim_mask[d] ? 1 : 0) : 1) : 0;
+  a.acq = acq_fn_of(acq, fn);
+  a.tr = trust_region_of(h, *acq, acq->tr_strict);
   a.scratch = h->scratch.as<double>();
   a.mpad = ntiles * kTM;
   a.nsplit = 1;
@@ -652,7 +647,7 @@ int prepare_small_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int
   a->part_rs = h->Tws.as<double>();
   a->part_mu = a->part_rs + (size_t)nvb * a->mpad;
   a->part_linf = a->part_mu + (size_t)nmb * a->mpad;
-  *with_linf = (linf != nullptr) || (a->apply_tr && a->radius <= 0.5);
+  *with_linf = (linf != nullptr) || tr_needs_distance(a->tr);
   // TMA boxes of the W phase: K* rows of one tile x 16 doubles, and 8 rows of Linv x 16 doubles.
   a->box_rows = ntiles == 1 ? ((M + 7) / 8) * 8 : kTM;
   VZ_TRY(make_map(&a->mapA, a->scratch, (uint64_t)ntiles * kTM, (uint64_t)h->np, (uint64_t)h->np, (uint32_t)a->box_rows));
@@ -674,10 +669,10 @@ struct GeneralArgs {
   const double* alpha;
   int mc, np, n_valid, dc;
   KernelParams kp;
-  double sn2, mean_const, radius;
+  double sn2, mean_const;
   AcqFn acq;
-  int apply_tr, tr_rows, tr_strict, want_linf;
-  uint8_t tr_mask[kMaxDc];
+  TrustRegion tr;
+  int want_linf;
   double* score; double* mu; double* sigma; double* linf;
   int* clamp_count;
 };
@@ -690,15 +685,7 @@ __global__ void __launch_bounds__(256) k_general_finalize(GeneralArgs a) {
   double mean = 0.0, rs = 0.0;
   for (int j = lane; j < a.n_valid; j += 32) mean = fma(ks[j], a.alpha[j], mean);
   for (int j = lane; j < a.np; j += 32) rs = fma(w[j], w[j], rs);
-  double dist = INFINITY;
-  if (a.want_linf) {
-    for (int n = lane; n < a.tr_rows; n += 32) {
-      double mx = 0.0;
-      for (int d = 0; d < a.dc; ++d)
-        if (a.tr_mask[d]) mx = fmax(mx, fabs(a.Xs[(size_t)m * a.dc + d] - a.X[(size_t)n * a.dc + d]));
-      dist = fmin(dist, mx);
-    }
-  }
+  double dist = a.want_linf ? tr_lane_distance(a.tr, a.Xs + (size_t)m * a.dc, a.X, a.dc, lane) : INFINITY;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     mean += __shfl_xor_sync(0xffffffffu, mean, o);
@@ -719,12 +706,7 @@ __global__ void __launch_bounds__(256) k_general_finalize(GeneralArgs a) {
   double var = kss - rs + a.sn2;
   if (var < 0.0) { var = 0.0; atomicAdd(a.clamp_count, 1); }
   const double sd = sqrt(var);
-  double sc = acq_value(a.acq, mean, sd);
-  if (a.apply_tr) {
-    const bool inside = (a.tr_strict ? (dist < a.radius) : (dist <= a.radius)) || (a.radius > 0.5);
-    sc = inside ? sc : (-1e4 - dist);
-  }
-  a.score[m] = sc;
+  a.score[m] = tr_apply(a.tr, acq_value(a.acq, mean, sd), dist);
   if (a.mu) a.mu[m] = mean;
   if (a.sigma) a.sigma[m] = sd;
   if (a.linf) a.linf[m] = dist;
@@ -758,12 +740,9 @@ static int launch_score_general(vzgp_handle* h, const double* Xs, const int32_t*
   GeneralArgs a;
   a.Ks = c.Ks; a.W = c.W; a.Xs = c.Xp; a.X = h->X.as<double>(); a.alpha = h->alpha.as<double>();
   a.np = np; a.n_valid = h->n_valid; a.dc = dc; a.kp = h->kp; a.sn2 = h->sn2; a.mean_const = h->mean_const;
-  a.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient); a.radius = acq->trust_radius;
-  a.apply_tr = acq->use_trust_region ? 1 : 0;
-  a.tr_rows = (acq->tr_rows > 0 && acq->tr_rows < h->n_valid) ? acq->tr_rows : h->n_valid;
-  a.tr_strict = acq->tr_strict ? 1 : 0;
-  a.want_linf = (linf != nullptr) || (a.apply_tr && a.radius <= 0.5);
-  for (int d = 0; d < kMaxDc; ++d) a.tr_mask[d] = (d < dc) ? (acq->tr_dim_mask ? (acq->tr_dim_mask[d] ? 1 : 0) : 1) : 0;
+  a.acq = acq_fn_of(acq, fn);
+  a.tr = trust_region_of(h, *acq, acq->tr_strict);
+  a.want_linf = (linf != nullptr) || tr_needs_distance(a.tr);
   a.clamp_count = h->small.as<int>();
   for (int m0 = 0; m0 < M; m0 += kChunk) {
     const int mc = M - m0 < kChunk ? M - m0 : kChunk;
@@ -836,13 +815,13 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
   if (ntiles * 2 <= h->sm_count && nblocks >= 2) nsplit = (nblocks + 1) / 2;
   const int nwork = ntiles * nsplit;
   const int csize = nsplit == 1 ? kCluster : 1;
-  const bool need_linf = (linf != nullptr) || (acq->use_trust_region && acq->trust_radius <= 0.5);
+  const bool need_linf = (linf != nullptr) || tr_needs_distance(trust_region_of(h, *acq, acq->tr_strict));
   const size_t sm = score_smem_bytes(h->dc, h->dk, need_linf);
   if (sm > 227 * 1024) {
     set_error("score kernel needs %zu bytes of shared memory (Dc=%d with trust-region distance)", sm, h->dc);
     return VZGP_ERR_UNSUPPORTED;
   }
-  const bool generic = !acq_fn_is_ucb(fn ? *fn : ucb_acq_fn(0.0));
+  const bool generic = !acq_fn_is_ucb(acq_fn_of(acq, fn));
   const void* kfn = generic ? (need_linf ? (const void*)k_score<true, true> : (const void*)k_score<false, true>)
                             : (need_linf ? (const void*)k_score<true, false> : (const void*)k_score<false, false>);
   VZ_TRY(raise_dyn_smem(kfn, sm));
@@ -888,8 +867,7 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
 struct PeCombine {
   int mode;
   double ucb, explore, penalty, threshold;
-  int apply_tr;
-  double radius;
+  TrustRegion tr;
 };
 __global__ void k_pe_combine(int M, PeCombine p, const double* __restrict__ mu, const double* __restrict__ sd,
                              const double* __restrict__ sd_all, const double* __restrict__ linf,
@@ -903,12 +881,7 @@ __global__ void k_pe_combine(int M, PeCombine p, const double* __restrict__ mu, 
     const double explore_ucb = fma(sd[m], p.explore, mu[m]);
     acq = sd_all[m] + p.penalty * fmin(explore_ucb - p.threshold, 0.0);
   }
-  if (p.apply_tr) {
-    const double dist = linf[m];
-    const bool inside = (dist < p.radius) || (p.radius > 0.5);
-    acq = inside ? acq : (-1e4 - dist);
-  }
-  score[m] = acq;
+  score[m] = tr_apply(p.tr, acq, linf[m]);
 }
 
 int launch_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
@@ -922,19 +895,13 @@ int launch_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const in
   double* linf_b = t + 3 * (size_t)M;
   double* dummy_a = t + 4 * (size_t)M;
   double* dummy_b = t + 5 * (size_t)M;
-  vzgp_acq none;
-  none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0; none.tr_dim_mask = nullptr;
-  none.tr_rows = 0; none.tr_strict = 0;
-  VZ_TRY(launch_score(hA, Xs, Zs, M, &none, dummy_a, mu_a, sd_a, nullptr));
-  vzgp_acq accb = none;
-  accb.tr_dim_mask = pe->tr_dim_mask;
-  accb.tr_rows = pe->tr_rows;
-  const bool want_tr = pe->use_trust_region && pe->trust_radius <= 0.5;
-  VZ_TRY(launch_score(hB, Xs, Zs, M, &accb, dummy_b, nullptr, sd_b, want_tr ? linf_b : nullptr));
+  const vzgp_acq none = posterior_request(), accb = posterior_request(pe->tr_dim_mask, pe->tr_rows);
   PeCombine p;
   p.mode = pe->mode; p.ucb = pe->ucb_coefficient; p.explore = pe->explore_coefficient;
   p.penalty = pe->penalty_coefficient; p.threshold = pe->threshold;
-  p.apply_tr = want_tr ? 1 : 0; p.radius = pe->trust_radius;
+  p.tr = trust_region_of(hB, *pe, true);
+  VZ_TRY(launch_score(hA, Xs, Zs, M, &none, dummy_a, mu_a, sd_a, nullptr));
+  VZ_TRY(launch_score(hB, Xs, Zs, M, &accb, dummy_b, nullptr, sd_b, tr_needs_distance(p.tr) ? linf_b : nullptr));
   k_pe_combine<<<(M + 255) / 256, 256, 0, hA->stream>>>(M, p, mu_a, sd_a, sd_b, linf_b, score);
   VZ_CHECK_LAUNCH();
   hA->launches++;
@@ -953,8 +920,7 @@ struct StackCombine {
   int E;
   double alpha[16];
   AcqFn acq;
-  int apply_tr, tr_strict;
-  double radius;
+  TrustRegion tr;
 };
 __global__ void k_stack_combine(int M, StackCombine p, const double* __restrict__ mu_e, const double* __restrict__ sd_e,
                                 const double* __restrict__ linf, double* __restrict__ score, double* __restrict__ mu,
@@ -966,13 +932,7 @@ __global__ void k_stack_combine(int M, StackCombine p, const double* __restrict_
     mean += mu_e[(size_t)e * M + m];
     sd = pow(sd_e[(size_t)e * M + m], p.alpha[e]) * pow(sd, 1.0 - p.alpha[e]);
   }
-  double sc = acq_value(p.acq, mean, sd);
-  if (p.apply_tr) {
-    const double dist = linf[m];
-    const bool inside = (p.tr_strict ? (dist < p.radius) : (dist <= p.radius)) || (p.radius > 0.5);
-    sc = inside ? sc : (-1e4 - dist);
-  }
-  score[m] = sc;
+  score[m] = tr_apply(p.tr, acq_value(p.acq, mean, sd), linf[m]);
   if (mu) mu[m] = mean;
   if (sigma) sigma[m] = sd;
 }
@@ -987,18 +947,14 @@ int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, cons
   double* sd_e = t + (size_t)E * M;
   double* linf_buf = linf ? linf : t + 2 * (size_t)E * M;
   double* dummy = t + (2 * (size_t)E + 1) * M;
-  const bool want_tr = acq->use_trust_region && acq->trust_radius <= 0.5;
-  const bool want_linf = want_tr || linf != nullptr;
-  vzgp_acq none;
-  none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0;
-  none.tr_dim_mask = acq->tr_dim_mask; none.tr_rows = acq->tr_rows; none.tr_strict = 0;
-  for (int e = 0; e < E; ++e)   // the trust region is measured against the trials of the top level (the current study)
+  StackCombine p;
+  p.E = E; p.acq = acq_fn_of(acq, fn);
+  p.tr = trust_region_of(top, *acq, acq->tr_strict);   // measured against the trials of the top level (the current study)
+  const bool want_linf = tr_needs_distance(p.tr) || linf != nullptr;
+  const vzgp_acq none = posterior_request(acq->tr_dim_mask, acq->tr_rows);
+  for (int e = 0; e < E; ++e)
     VZ_TRY(launch_score(hs[e], Xs, Zs, M, &none, dummy, mu_e + (size_t)e * M, sd_e + (size_t)e * M,
                         (e == E - 1 && want_linf) ? linf_buf : nullptr));
-  StackCombine p;
-  p.E = E; p.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
-  p.apply_tr = want_tr ? 1 : 0; p.tr_strict = acq->tr_strict ? 1 : 0;
-  p.radius = acq->trust_radius;
   for (int e = 0; e < 16; ++e) p.alpha[e] = e < E ? alphas[e] : 0.0;
   k_stack_combine<<<(M + 255) / 256, 256, 0, top->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma);
   VZ_CHECK_LAUNCH();
@@ -1009,7 +965,7 @@ int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, cons
 // ---------------------------------------------------------------------------
 // Set-PE acquisition (SetPEScoreFunction, gp_ucb_pe.py:510-594): per set of q points
 //   logdet(joint predictive covariance under model B)  +  penalty * sum_i min(mean_A + explore * stddev_A - threshold, 0)
-//   [+ sum_i (dist_i > radius and radius <= 0.5) * (-1e4 - dist_i)      _apply_trust_region_to_set, :245-269]
+//   [+ sum_i tr_set_term(dist_i) when radius <= 0.5                        _apply_trust_region_to_set, :245-269]
 // One warp per set: the q x q block of the [M x M] covariance is factored in shared memory (q <= 16); a pivot that is
 // not positive gives -inf like the reference's NaN -> -inf rule (:495-507).
 // ---------------------------------------------------------------------------
@@ -1043,10 +999,7 @@ __global__ void __launch_bounds__(32) k_set_pe_combine(int n_sets, int q, PeComb
   double pen = 0.0, tr = 0.0;
   for (int i = lane; i < q; i += 32) {
     pen += fmin(mu_a[r0 + i] + p.explore * sd_a[r0 + i] - p.threshold, 0.0);
-    if (p.apply_tr) {
-      const double dist = linf[r0 + i];
-      if (dist > p.radius) tr += -1e4 - dist;
-    }
+    if (p.tr.apply) tr += tr_set_term(p.tr, linf[r0 + i]);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -1061,8 +1014,8 @@ int launch_set_pe_combine(vzgp_handle* h, int n_sets, int q, const vzgp_pe_param
   PeCombine p;
   p.mode = 1; p.ucb = pe->ucb_coefficient; p.explore = pe->explore_coefficient;
   p.penalty = pe->penalty_coefficient; p.threshold = pe->threshold;
-  p.apply_tr = (pe->use_trust_region && pe->trust_radius <= 0.5 && linf != nullptr) ? 1 : 0;
-  p.radius = pe->trust_radius;
+  p.tr = trust_region_of(h, *pe, true);
+  p.tr.apply = linf != nullptr && tr_needs_distance(p.tr);
   k_set_pe_combine<<<n_sets, 32, 0, h->stream>>>(n_sets, q, p, cov, ldc, mu_a, sd_a, linf, score, sd_all);
   VZ_CHECK_LAUNCH();
   h->launches++;
@@ -1076,8 +1029,7 @@ int launch_set_pe_combine(vzgp_handle* h, int n_sets, int q, const vzgp_pe_param
 struct EnsCombine {
   int E;
   AcqFn acq;
-  int apply_tr, tr_strict;
-  double radius;
+  TrustRegion tr;
 };
 __global__ void k_ensemble_combine(int M, EnsCombine p, const double* __restrict__ mu_e, const double* __restrict__ sd_e,
                                    const double* __restrict__ linf, double* __restrict__ score,
@@ -1094,13 +1046,7 @@ __global__ void k_ensemble_combine(int M, EnsCombine p, const double* __restrict
   double var = s2 / p.E - mean * mean;
   if (var < 0.0) { var = 0.0; atomicAdd(clamp_count, 1); }
   const double sd = sqrt(var);
-  double sc = acq_value(p.acq, mean, sd);
-  if (p.apply_tr) {
-    const double dist = linf[m];
-    const bool inside = (p.tr_strict ? (dist < p.radius) : (dist <= p.radius)) || (p.radius > 0.5);
-    sc = inside ? sc : (-1e4 - dist);
-  }
-  score[m] = sc;
+  score[m] = tr_apply(p.tr, acq_value(p.acq, mean, sd), linf[m]);
   if (mu) mu[m] = mean;
   if (sigma) sigma[m] = sd;
 }
@@ -1115,18 +1061,14 @@ int launch_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const
   double* sd_e = t + (size_t)E * M;
   double* linf_buf = linf ? linf : t + 2 * (size_t)E * M;
   double* dummy = t + (2 * (size_t)E + 1) * M;
-  const bool want_tr = acq->use_trust_region && acq->trust_radius <= 0.5;
-  const bool want_linf = want_tr || linf != nullptr;
-  vzgp_acq none;
-  none.ucb_coefficient = 0.0; none.use_trust_region = 0; none.trust_radius = 1.0;
-  none.tr_dim_mask = acq->tr_dim_mask; none.tr_rows = acq->tr_rows; none.tr_strict = 0;
+  EnsCombine p;
+  p.E = E; p.acq = acq_fn_of(acq, fn);
+  p.tr = trust_region_of(h0, *acq, acq->tr_strict);
+  const bool want_linf = tr_needs_distance(p.tr) || linf != nullptr;
+  const vzgp_acq none = posterior_request(acq->tr_dim_mask, acq->tr_rows);
   for (int e = 0; e < E; ++e)   // all members share the trials: the distance is computed once
     VZ_TRY(launch_score(hs[e], Xs, Zs, M, &none, dummy, mu_e + (size_t)e * M, sd_e + (size_t)e * M,
                         (e == 0 && want_linf) ? linf_buf : nullptr));
-  EnsCombine p;
-  p.E = E; p.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
-  p.apply_tr = want_tr ? 1 : 0; p.tr_strict = acq->tr_strict ? 1 : 0;
-  p.radius = acq->trust_radius;
   k_ensemble_combine<<<(M + 255) / 256, 256, 0, h0->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma, h0->small.as<int>());
   VZ_CHECK_LAUNCH();
   h0->launches++;

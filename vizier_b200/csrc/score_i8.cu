@@ -182,7 +182,7 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
   // the warp index through a shuffle: provably warp-uniform, so the role branches below are uniform branches
   const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   const bool is_kwarp = warp < kKWarps;
-  if (tid < kMaxDc) s_mask[tid] = a.tr_mask[tid];
+  if (tid < kMaxDc) s_mask[tid] = a.tr.mask[tid];
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) mbar_init(full + i, 1);
     for (int i = 0; i < 2; ++i) { mbar_init(kready + i, kKWarps * 32); mbar_init(kfree + i, kEWarps); }
@@ -315,7 +315,7 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
               const bool valid = (jb * 64 + cj) < a.n_valid;
               const double kv = valid ? matern52(d2[i][j], a.kp.sf2) : 0.0;
               mu_part[p][i] = fma(kv, alj[GP::col_of(tx, j)], mu_part[p][i]);
-              if (WITH_LINF && (jb * 64 + cj) < a.tr_rows) lmin[p][i] = fmin(lmin[p][i], lf[i][j]);
+              if (WITH_LINF && (jb * 64 + cj) < a.tr.rows) lmin[p][i] = fmin(lmin[p][i], lf[i][j]);
               q[j] = __double2ll_rn(kv * ia.kscale);    // |q| < 2^55
             }
             uint8_t* row = kd + (size_t)GP::row_of(ty, i) * np + jb * 64 + zoff;
@@ -565,23 +565,7 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
   I8Args ia;
   memset(&ia, 0, sizeof(ia));
   ScoreArgs& a = ia.s;
-  a.Xs = Xs; a.Zs = Zs; a.M = M;
-  a.XT = h->XT.as<double>(); a.Z = h->Z.as<int32_t>();
-  a.np = np; a.n_valid = h->n_valid;
-  a.Linv = h->Linv.as<double>(); a.ldi = np;
-  a.alpha = h->alpha.as<double>();
-  a.kp = h->kp; a.sn2 = h->sn2;
-  a.acq = fn ? *fn : ucb_acq_fn(acq->ucb_coefficient);
-  a.apply_tr = acq->use_trust_region ? 1 : 0;
-  a.tr_rows = (acq->tr_rows > 0 && acq->tr_rows < h->n_valid) ? acq->tr_rows : h->n_valid;
-  a.tr_strict = acq->tr_strict ? 1 : 0;
-  a.radius = acq->trust_radius;
-  for (int d = 0; d < kMaxDc; ++d)
-    a.tr_mask[d] = (d < h->dc) ? (acq->tr_dim_mask ? (acq->tr_dim_mask[d] ? 1 : 0) : 1) : 0;
-  a.nsplit = 1;
-  a.mpad = ntiles * kTM;
-  a.score = score; a.mu = mu; a.sigma = sigma; a.linf = linf;
-  a.clamp_count = h->small.as<int>();
+  fill_score_args(h, Xs, Zs, M, acq, fn, score, mu, sigma, linf, &a);
   ia.kdig = h->i8_kdig.as<uint8_t>();
   ia.lscale = h->i8_scale.as<double>();
   ia.kscale = ldexp(1.0, 56 - ea);
@@ -601,7 +585,7 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
     const uint32_t box[3] = {(uint32_t)kKC, (uint32_t)kJT, 1u};
     VZ_TRY(make_tensor_map_u8(&ia.mapL, h->i8_planes.as<uint8_t>(), 3, dims, strides, box));
   }
-  const bool need_linf = (linf != nullptr) || (a.apply_tr && a.radius <= 0.5);
+  const bool need_linf = (linf != nullptr) || tr_needs_distance(a.tr);
   const size_t sm = score_i8_smem_bytes(h->dc, h->dk, nbuf, plan.sb_bufs);
   if (sm > 227 * 1024) { set_error("k_score_i8 needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
   const bool generic = !acq_fn_is_ucb(a.acq);

@@ -28,10 +28,10 @@ struct QMomArgs {
   const int32_t* Zs;      // [mp x dk]
   const double* X;        // [np x dc] trials
   const double* alpha;
-  int q, np, n_valid, dc, dk, tr_rows, want_linf;
+  int q, np, n_valid, dc, dk, want_linf;
   KernelParams kp;
   double sn2, mean_const;
-  uint8_t tr_mask[kMaxDc];
+  TrustRegion tr;
   double* mu;             // [sets * q] of this chunk
   double* cov;            // [sets][q][q]
   double* linf;           // [sets * q] or nullptr
@@ -95,13 +95,7 @@ __global__ void __launch_bounds__(kQMomThreads) k_qset_moments(const QMomArgs a)
       }
     } else {
       const int row = r0 + (t - q - npairs);
-      double dist = INFINITY;
-      for (int n = lane; n < a.tr_rows; n += 32) {
-        double mx = 0.0;
-        for (int d = 0; d < a.dc; ++d)
-          if (a.tr_mask[d]) mx = fmax(mx, fabs(a.Xs[(size_t)row * a.dc + d] - a.X[(size_t)n * a.dc + d]));
-        dist = fmin(dist, mx);
-      }
+      double dist = tr_lane_distance(a.tr, a.Xs + (size_t)row * a.dc, a.X, a.dc, lane);
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) dist = fmin(dist, __shfl_xor_sync(0xffffffffu, dist, o));
       if (lane == 0) a.linf[row] = dist;
@@ -113,8 +107,9 @@ struct QMcArgs {
   const double* mean;     // [E][n_sets * q]
   const double* cov;      // [E][n_sets][q][q]
   const double* linf;     // [n_sets * q] or nullptr (no trust region)
-  int n_sets, q, E, S, period, kind, apply_tr;
-  double best, coef, radius;
+  int n_sets, q, E, S, period, kind;
+  double best, coef;
+  TrustRegion tr;
   uint64_t seed;
   double* score;
   double* mu;             // optional [n_sets * q]: mixture mean
@@ -227,11 +222,8 @@ __global__ void __launch_bounds__(kQMcThreads) k_qacq_mc(const QMcArgs a) {
   const double total = block_sum(acc, red);
   if (threadIdx.x == 0) {
     double tr = 0.0;
-    if (a.apply_tr)
-      for (int j = 0; j < q; ++j) {
-        const double dist = a.linf[(size_t)set * q + j];
-        if (dist > a.radius) tr += -1e4 - dist;
-      }
+    if (a.tr.apply)
+      for (int j = 0; j < q; ++j) tr += tr_set_term(a.tr, a.linf[(size_t)set * q + j]);
     a.score[set] = bad ? NAN : total / a.S + tr;
   }
 }
@@ -244,8 +236,9 @@ int launch_qacq_mc(vzgp_handle* h, int n_sets, int q, int E, const double* mean,
   a.n_sets = n_sets; a.q = q; a.E = E; a.S = qa->num_samples;
   a.period = qa->period > 0 ? qa->period : n_sets;
   a.kind = qa->kind;
-  a.apply_tr = (linf != nullptr && qa->use_trust_region && qa->trust_radius <= 0.5) ? 1 : 0;
-  a.best = qa->best_label; a.coef = qa->coefficient; a.radius = qa->trust_radius;
+  a.tr = trust_region_of(h, *qa, false);
+  a.tr.apply = linf != nullptr && tr_needs_distance(a.tr);
+  a.best = qa->best_label; a.coef = qa->coefficient;
   a.seed = seed; a.score = score; a.mu = mu; a.sigma = sigma;
   const size_t sm = sizeof(double) * ((size_t)E * q * q + (size_t)E * q + q + 32);
   k_qacq_mc<<<n_sets, kQMcThreads, sm, h->stream>>>(a);
@@ -259,7 +252,8 @@ int launch_score_qsets(vzgp_handle* const* hs, int E, const double* Xs, const in
   if (n_sets <= 0) return 0;
   vzgp_handle* h0 = hs[0];
   const int M = n_sets * q, dc = h0->dc, dk = h0->dk;
-  const bool want_linf = linf != nullptr || (qa->use_trust_region && qa->trust_radius <= 0.5);
+  const TrustRegion tr = trust_region_of(h0, *qa, false);   // measured on member 0's trials
+  const bool want_linf = linf != nullptr || tr_needs_distance(tr);
   const size_t nmean = (size_t)E * M, ncov = (size_t)E * M * q;
   // qmom: member means [E][M] | covariance blocks [E][n_sets][q][q] (unless the caller's cov_out) | distances [M]
   VZ_TRY(h0->qmom.reserve(sizeof(double) * (nmean + (qa->cov_out ? 0 : ncov) + M)));
@@ -275,9 +269,8 @@ int launch_score_qsets(vzgp_handle* const* hs, int E, const double* Xs, const in
     a.Ks = c.Ks; a.W = c.W; a.Xs = c.Xp; a.Zs = c.Zp; a.X = h->X.as<double>(); a.alpha = h->alpha.as<double>();
     a.q = q; a.np = h->np; a.n_valid = h->n_valid; a.dc = dc; a.dk = dk; a.kp = h->kp;
     a.sn2 = h->sn2; a.mean_const = h->mean_const;
-    a.tr_rows = (qa->tr_rows > 0 && qa->tr_rows < h->n_valid) ? qa->tr_rows : h->n_valid;
+    a.tr = tr;
     a.want_linf = (e == 0 && want_linf) ? 1 : 0;
-    for (int d = 0; d < kMaxDc; ++d) a.tr_mask[d] = (d < dc) ? (qa->tr_dim_mask ? (qa->tr_dim_mask[d] ? 1 : 0) : 1) : 0;
     for (int m0 = 0; m0 < M; m0 += rows) {
       const int mc = M - m0 < rows ? M - m0 : rows;
       VZ_TRY(launch_general_chunk(h, dc > 0 ? Xs + (size_t)m0 * dc : Xs, dk > 0 ? Zs + (size_t)m0 * dk : Zs, mc, c));

@@ -30,11 +30,7 @@ struct ScoreArgs {
   const double* alpha;
   KernelParams kp;
   double sn2;
-  int apply_tr;     // trust region modifies the score
-  int tr_rows;      // trusted points = first tr_rows rows of X
-  int tr_strict;    // inside test: dist < radius instead of <=
-  double radius;
-  uint8_t tr_mask[kMaxDc];
+  TrustRegion tr;
   double* scratch;  // [gridDim.x][64][np]
   int nsplit;       // > 1: output column blocks of one tile are shared by nsplit CTAs (small M)
   double* part;     // nsplit > 1: [nsplit + 2][Mpad] partial row sums, then mu, then linf
@@ -60,12 +56,7 @@ __device__ __forceinline__ void emit_score(const ScoreArgs& a, int m, double rs,
   double var = a.kp.sf2 - rs + a.sn2;
   if (var < 0.0) { var = 0.0; ++clamped; }
   const double sd = sqrt(var);
-  double sc = acq_eval<GENERIC>(a.acq, mean, sd);
-  if (a.apply_tr) {
-    const bool inside = (a.tr_strict ? (dist < a.radius) : (dist <= a.radius)) || (a.radius > 0.5);
-    sc = inside ? sc : (-1e4 - dist);
-  }
-  a.score[m] = sc;
+  a.score[m] = tr_apply(a.tr, acq_eval<GENERIC>(a.acq, mean, sd), dist);
   if (a.mu) a.mu[m] = mean;
   if (a.sigma) a.sigma[m] = sd;
   if (a.linf) a.linf[m] = dist;
@@ -133,7 +124,7 @@ __device__ __forceinline__ void cross_small_core(const ScoreArgs& a, int jb, int
     const double bb[4] = {b0.x, b0.y, b1.x, b1.y};
     if (WITH_LINF) {
       const double w = a.kp.inv_ls2_c[d];
-      const bool in_tr = a.tr_mask[d] != 0;
+      const bool in_tr = a.tr.mask[d] != 0;
 #pragma unroll
       for (int i = 0; i < NI; ++i)
 #pragma unroll
@@ -171,7 +162,7 @@ __device__ __forceinline__ void cross_small_core(const ScoreArgs& a, int jb, int
       const int gc = jb * 64 + 4 * tx + j;
       kv[j] = gc < a.n_valid ? matern52(d2[i][j], a.kp.sf2) : 0.0;
       mu_part = fma(kv[j], __ldg(a.alpha + gc), mu_part);
-      if (WITH_LINF && gc < a.tr_rows) lmin = fmin(lmin, lf[i][j]);
+      if (WITH_LINF && gc < a.tr.rows) lmin = fmin(lmin, lf[i][j]);
     }
     *reinterpret_cast<double2*>(scr + (size_t)r * np + 4 * tx) = make_double2(kv[0], kv[1]);
     *reinterpret_cast<double2*>(scr + (size_t)r * np + 4 * tx + 2) = make_double2(kv[2], kv[3]);
@@ -382,8 +373,11 @@ __device__ __forceinline__ void small_finalize_8(const ScoreArgs& a, int m, int 
   if (active && p == 0) emit_score<GENERIC>(a, m, rs, mean, dist, clamped);
 }
 
-// Host side (score.cu): argument block + workspaces of the small-pool path for M candidates on `h`.
-// fn: the acquisition function (nullptr: UCB with acq->ucb_coefficient).
+// Host side (score.cu).  The argument block of the scoring kernels for M candidates on `h`; fn: the acquisition
+// function (nullptr: UCB with acq->ucb_coefficient).
+void fill_score_args(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq, const AcqFn* fn,
+                     double* score, double* mu, double* sigma, double* linf, ScoreArgs* pa);
+// Argument block + workspaces of the small-pool path.
 int prepare_small_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
                         double* score, double* mu, double* sigma, double* linf, ScoreArgs* a, bool* with_linf,
                         const AcqFn* fn = nullptr);
