@@ -7,8 +7,9 @@ runs the k_score<true> instance (L-inf distance); bench.py times that instance a
 Counters are summed over all CTAs and reported per tile: phase 1 (K* tile), the gate after it, phase 2
 (DMMA slab stream), the whole tile (all of math warp 0), the average math warp's wait on the full
 barriers (ring starved: operand feed too slow) and the producer's wait on the empty barriers (ring full:
-the math warps are the limit).  Phase 1 is split into the d2 loop, Matern + mu, the scratch stores and
-the barrier / cp.async waits (math warp 0)."""
+the math warps are the limit).  Phase 1 is split into the d2 loop, Matern + mu, the scratch stores (K* written
+to the shared-memory staging buffer, plus the TMA store issue) and the waits: barriers, cp.async and the TMA
+stores (math warp 0)."""
 import ctypes as C
 import json
 import sys

@@ -1,5 +1,5 @@
 // Asynchronous-copy primitives shared by the scoring kernels and the dataflow factorisation:
-// cp.async (LDGSTS), mbarrier, TMA 2-D box loads (cp.async.bulk.tensor), proxy fence, and the
+// cp.async (LDGSTS), mbarrier, TMA 2-D box loads and stores (cp.async.bulk.tensor), proxy fences, and the
 // thread-block-cluster forms (cluster barrier, remote mbarrier arrive, TMA multicast).
 #pragma once
 #include <cuda.h>
@@ -43,7 +43,28 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
 }
+// 2-D tile store, the inverse of tma_load_2d: the box at smem_src (same layout and swizzle as a loaded box)
+// goes to the box origin (c0, c1) of `map`.  Tracked by bulk async-groups, not by an mbarrier.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, int c0, int c1, const void* smem_src) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];\n" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(c0), "r"(c1), "r"(smem_u32(smem_src))
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
+// At most N of this thread's bulk groups still read their shared-memory source (the source may be rewritten).
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory");
+}
+// At most N of this thread's bulk groups are incomplete (their global writes are not yet performed).
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;\n" ::"n"(N) : "memory");
+}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;\n" ::: "memory"); }
+// Generic-proxy shared-memory writes of this thread before later async-proxy (TMA store) reads of them.
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
 // ---- thread-block clusters ---------------------------------------------------------------
 __device__ __forceinline__ unsigned cluster_ctarank() {

@@ -11,7 +11,8 @@
 // One persistent CTA per SM walks 64-candidate tiles:
 //   phase 1  K* tile [64 x np] = Matern(x*, X) built 64 columns at a time from shared-memory
 //            staged rows; mu = K* alpha and the L-inf trust-region distance are reduced on the
-//            fly; the tile goes to a CTA-private scratch (L2 resident, never re-read by others).
+//            fly; each 64-column step of the tile is written to shared memory in the layout of phase 2's
+//            TMA boxes and leaves by TMA store to a CTA-private scratch (L2 resident, never re-read by others).
 //   phase 2  W = K* . Linv^T in 64 x 128 blocks on the FP64 tensor pipe (mma.sync m16n8k8 f64: on the
 //            H100 the m8n8k4 shape issues at half the rate), operands streamed by a TMA producer warp
 //            (cp.async.bulk.tensor, 128-byte swizzle) through a 4-stage ring with full/empty mbarriers,
@@ -51,8 +52,8 @@ constexpr int kBK = 32;          // k-slab = 32 columns of K* and Linv
 constexpr int kStages = 4;
 // K* is stored in row-pair order so that one 16-byte load gives two A-fragment registers in the order
 // m16n8k8 wants them.  Pair p of a tile holds rows 16 (p / 8) + p % 8 and that + 8 (rows fr and fr + 8
-// of one A fragment); in the scratch a pair is one row of 2 np doubles, [k][2 rows], and in shared memory
-// pair position 2p + e stands for row pair_row(2p + e).
+// of one A fragment); in the scratch each k group of 8 is a dense box of 32 pairs x [8 k][2 rows], and in the
+// phase-1 staging pair position 2p + e stands for row pair_row(2p + e).
 __host__ __device__ constexpr int pair_pos(int r) { return (((r >> 4) * 8 + (r & 7)) << 1) | ((r >> 3) & 1); }
 __host__ __device__ constexpr int pair_row(int pos) { return ((pos >> 4) << 4) + ((pos >> 1) & 7) + ((pos & 1) << 3); }
 static_assert(pair_row(pair_pos(13)) == 13 && pair_row(pair_pos(58)) == 58 && pair_pos(8) == 1, "pair order round trip");
@@ -70,12 +71,30 @@ constexpr int kCluster = 2;
 constexpr int kBPieces = kCluster < 2 ? 2 : kCluster;
 constexpr int kBPieceRows = 2 * kBN / kBPieces;
 static_assert(kBPieces % 2 == 0 && kBN % (kBPieces / 2) == 0, "B pieces tile the two halves of a stage");
+// Phase 1 aliases the ring: K* staging | candidates [dc][LD] | kTrialBufs x (trials [dc][LD], alpha [64]).
+// A staging buffer holds one 64-column step of K* as the eight A boxes that phase 2 loads back, and leaves by
+// TMA store.  A 32 KB step's store can take longer than the math of a step at D = 20.  With an L2 persisting
+// window on the scratch it did, at about 4 bytes per cycle per SM, which is why k_score installs no window.  So
+// the stores get as many staging buffers as fit: three up to dc = 45, two up
+// to dc = 61, and above that one, where each step waits for the previous step's store to have read it (one
+// more barrier per step).
+constexpr int kStgDoubles = 8 * kABox;    // 64 x 64 K* block, 32 KB (a multiple of 1024 bytes: swizzle atoms stay aligned)
+constexpr int kTrialBufs = 3;             // trials staged one step ahead, released one step later: one barrier per step
+__host__ __device__ constexpr int trial_stride(int dc) { return dc * kLD1 + 64; }
+__host__ __device__ constexpr int phase1_doubles(int dc, int nstg) { return nstg * kStgDoubles + dc * kLD1 + kTrialBufs * trial_stride(dc); }
+__host__ __device__ constexpr int stg_buffers(int dc) {
+  return phase1_doubles(dc, 3) <= kStages * kStageDoubles ? 3 : phase1_doubles(dc, 2) <= kStages * kStageDoubles ? 2 : 1;
+}
+static_assert(phase1_doubles(kMaxDc, 1) <= kStages * kStageDoubles, "phase-1 staging fits in the ring at every dc");
+static_assert(stg_buffers(45) == 3 && stg_buffers(46) == 2 && stg_buffers(61) == 2 && stg_buffers(62) == 1,
+              "the staging plan switches at dc = 46 and 62 (tested on both sides)");
 
 #ifdef VZ_SCORE_TIMING
 // Instrumented build only (make timing): clock64 sums over all CTAs, read by vzgp_debug_score_timing.
 // [0] tiles  [1] phase 1  [2] phase 2  [3] tile gate (barrier after phase 1)  [4] whole tile   (math warp 0)
 // [5] math warps waiting on full barriers (summed over the 8 warps)  [6] producer waiting on empty barriers
-// phase 1, math warp 0: [7] d2 loop  [8] Matern + mu  [9] scratch stores  [10] barrier and cp.async waits
+// phase 1, math warp 0: [7] d2 loop  [8] Matern + mu  [9] scratch stores (K* written to the staging buffer, and
+// thread 0's TMA store issue)  [10] barriers, cp.async waits and thread 0's waits for the TMA stores
 constexpr int kScoreCounters = 11;
 __device__ unsigned long long g_score_t[kScoreCounters];
 #define VZ_ST(...) __VA_ARGS__
@@ -96,10 +115,11 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   // reference's FeatureScaled form, 2 flops per dimension).  With it, unscaled features are staged
   // so that |a-b| is exact, and the scaling is applied to the squared difference.
   // Phase 1 and phase 2 never overlap in time, so the phase-1 staging buffers alias the ring.
-  double* sa = ring;                                     // [dc][LD]     candidates (transposed)
-  double* sb = sa + dc * LD;                             // [2][dc][LD]  trials, double buffered
-  double* s_alpha = ring + (kStages * kStageDoubles > 3 * kMaxDc * kLD1 ? kStages * kStageDoubles : 3 * kMaxDc * kLD1);  // [2][64]
-  double* s_mu = s_alpha + 128;                          // [64]
+  const int nstg = stg_buffers(dc);
+  double* sk = ring;                                     // [nstg][8 boxes]  K* of a step, 1024-byte aligned
+  double* sa = sk + nstg * kStgDoubles;                  // [dc][LD]     candidates (transposed)
+  double* sb = sa + dc * LD;                             // [3][trial_stride]  trials [dc][LD] and alpha [64]
+  double* s_mu = ring + kStages * kStageDoubles;         // [64]
   double* s_linf = s_mu + 64;                            // [64]
   double* s_rowsq = s_linf + 64;                         // [4][64]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_rowsq + 256);  // [kStages] TMA bytes landed
@@ -118,7 +138,9 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   // and r^4 land in opposite halves.  So fr = 2i, 2i+1 read rows i, i+4.  Row sums do not care which
   // column a fragment row holds.  (A, in pair order, reads even and odd chunks and needs no remapping.)
   const int pr = ((fr & 1) << 2) | (fr >> 1);
-  double* scr = a.scratch + (size_t)blockIdx.x * kTM * np;
+  // The K* scratch of this CTA is a run of dense 4 KB boxes, one per 8-wide k group g (32 row pairs x 8 k x 2 rows),
+  // at box row (blockIdx.x * np / 8 + g) * 32 of mapA: a step's 32 KB and a slab's 16 KB are contiguous in memory.
+  auto scratch_box_row = [&](int g) { return ((int)blockIdx.x * (np / 8) + g) * (kTM / 2); };
   // Cluster of ncta CTAs (1 for medium pools, which split a tile's blocks between CTAs, else kCluster).
   // The peers write into this CTA's ring and arrive on its empty barriers, so every gate that keeps the
   // ring or the barriers untouched is cluster-wide when ncta > 1.
@@ -174,7 +196,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
             const int k0 = ks * kBK;
             mbar_expect_tx(full_bar + stage, kStageBytes);   // own A boxes + the B pieces of every CTA
             for (int h = 0; h < 4; ++h)
-              tma_load_2d(base + h * kABox, &a.mapA, 2 * k0 + 16 * h, (int)blockIdx.x * (kTM / 2), full_bar + stage);
+              tma_load_2d(base + h * kABox, &a.mapA, 0, scratch_box_row(k0 / 8 + h), full_bar + stage);
             for (int p = (int)crank; p < kBPieces; p += (int)ncta) {   // rows >= np: zero fill
               const int half = p / (kBPieces / 2), r0 = (p % (kBPieces / 2)) * kBPieceRows;
               double* dst = base + 4 * kABox + half * kBHalf + r0 * 16;
@@ -202,15 +224,23 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
 
     // ---------------- phase 1: K* tile, mean, trust-region distance ----------------
     // Trial rows arrive pre-transposed and pre-scaled (XT), 64 columns per step, through a
-    // two-deep cp.async buffer so the copy of block jb+1 overlaps the math of block jb.
+    // three-deep cp.async buffer: the copy of block jb+1 overlaps the math of block jb, and the buffer
+    // it fills was last read in step jb-2, which every thread left before the barrier of step jb-1.
     auto stage_trials = [&](int jb, int buf) {
-      double* dst = sb + buf * dc * LD;
+      double* dst = sb + buf * trial_stride(dc);
       const double* src = WITH_LINF ? XTu : XTs;
       for (int c = tid; c < dc * 32; c += kThreads) {       // dc rows x 32 chunks of 16 B
         const int d = c >> 5, q = c & 31;
         cp_async16(dst + d * LD + q * 2, src + (size_t)d * np + jb * 64 + q * 2, true);
       }
-      if (tid < 32) cp_async16(s_alpha + buf * 64 + tid * 2, a.alpha + jb * 64 + tid * 2, true);
+      if (tid < 32) cp_async16(dst + dc * LD + tid * 2, a.alpha + jb * 64 + tid * 2, true);
+    };
+    // K* of step jb leaves as eight boxes of the scratch's tensor map (mapA, the one phase 2 loads with).
+    auto store_step = [&](int jb) {
+      const double* src = sk + (jb % nstg) * kStgDoubles;
+#pragma unroll 1
+      for (int h = 0; h < 8; ++h) tma_store_2d(&a.mapA, 0, scratch_box_row(8 * jb + h), src + h * kABox);
+      bulk_commit();
     };
     double mu_part[4], lmin[4];
 #pragma unroll
@@ -220,32 +250,49 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     cp_async_commit();
     for (int jb = 0; jb < nj; ++jb) {
       VZ_ST(long long tc = clock64();)
-      const int buf = jb & 1;
-      if (jb + 1 < nj) stage_trials(jb + 1, buf ^ 1);   // buffer buf^1 was released by the barrier below
+      const int buf = jb % kTrialBufs;
+      if (jb + 1 < nj) stage_trials(jb + 1, (jb + 1) % kTrialBufs);
       cp_async_commit();
       cp_async_wait<1>();
+      // With nstg >= 2 staging buffers, step jb writes the one the store of step jb-nstg reads.  That store was
+      // issued at the start of step jb-nstg+1, and at most the nstg-2 stores issued after it may still be reading;
+      // once it is done, the barrier below releases the buffer to every thread.
+      if (tid == 0) { if (nstg == 3) bulk_wait_read<1>(); else bulk_wait_read<0>(); }
+      // Trials of step jb have landed for every thread; every thread has written (and fenced) its part of step
+      // jb-1's K* and is done reading the trial buffer of step jb-1.
       consumer_sync();
       if (dk > 0) {  // categorical rows are rare: staged synchronously
         stage_rows_T_i32(a.Z, np, dk, jb * 64, 64, zb, LD, kThreads);
         consumer_sync();
       }
       VZ_ST(t_sync += clock64() - tc; tc = clock64();)
-      const double* sbj = sb + buf * dc * LD;
-      const double* alj = s_alpha + buf * 64;
+      if (jb > 0 && tid == 0) store_step(jb - 1);
+      VZ_ST(t_st += clock64() - tc; tc = clock64();)
+      const double* sbj = sb + buf * trial_stride(dc);
+      const double* alj = sbj + dc * LD;
       double d2[4][4], lf[4][4];
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) { d2[i][j] = 0.0; lf[i][j] = 0.0; }
+      // Software-pipelined over d: the LDS.128 operands of dimension d + 1 (and its weight and mask) are loaded
+      // while the 32 FP64 operations of dimension d run.  The FMA sequence of every element is unchanged.
+      auto ld2 = [](const double* p) { return *reinterpret_cast<const double2*>(p); };
+      double2 a0 = ld2(sa + GP1::row_of(ty, 0)), a1 = ld2(sa + GP1::row_of(ty, 2));
+      double2 b0 = ld2(sbj + GP1::col_of(tx, 0)), b1 = ld2(sbj + GP1::col_of(tx, 2));
+      double w_n = WITH_LINF ? a.kp.inv_ls2_c[0] : 0.0;
+      bool in_tr_n = WITH_LINF ? s_mask[0] != 0 : false;
       for (int d = 0; d < dc; ++d) {
-        const double2 a0 = *reinterpret_cast<const double2*>(sa + d * LD + GP1::row_of(ty, 0));
-        const double2 a1 = *reinterpret_cast<const double2*>(sa + d * LD + GP1::row_of(ty, 2));
-        const double2 b0 = *reinterpret_cast<const double2*>(sbj + d * LD + GP1::col_of(tx, 0));
-        const double2 b1 = *reinterpret_cast<const double2*>(sbj + d * LD + GP1::col_of(tx, 2));
+        const int dn = d + 1 < dc ? d + 1 : d;
+        const double2 a0n = ld2(sa + dn * LD + GP1::row_of(ty, 0)), a1n = ld2(sa + dn * LD + GP1::row_of(ty, 2));
+        const double2 b0n = ld2(sbj + dn * LD + GP1::col_of(tx, 0)), b1n = ld2(sbj + dn * LD + GP1::col_of(tx, 2));
         const double aa[4] = {a0.x, a0.y, a1.x, a1.y}, bb[4] = {b0.x, b0.y, b1.x, b1.y};
+        a0 = a0n; a1 = a1n; b0 = b0n; b1 = b1n;
         if (WITH_LINF) {
-          const double w = a.kp.inv_ls2_c[d];
-          const bool in_tr = s_mask[d] != 0;
+          const double w = w_n;
+          const bool in_tr = in_tr_n;
+          w_n = a.kp.inv_ls2_c[dn];
+          in_tr_n = s_mask[dn] != 0;
 #pragma unroll
           for (int i = 0; i < 4; ++i)
 #pragma unroll
@@ -298,19 +345,45 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
           mu_part[i] = fma(kv[i][j], alj[cj], mu_part[i]);
         }
       VZ_ST(t_mat += clock64() - tc; tc = clock64();)
-      // rows i = 2 ip, 2 ip + 1 of this thread are pair positions 2p, 2p + 1: one 16-byte store per column
-#pragma unroll
-      for (int ip = 0; ip < 2; ++ip) {
-        double* dst = scr + (size_t)(GP1::row_of(ty, 2 * ip) >> 1) * (2 * np) + 2 * jb * 64;
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          *reinterpret_cast<double2*>(dst + 2 * GP1::col_of(tx, j)) = make_double2(kv[2 * ip][j], kv[2 * ip + 1][j]);
+      if (nstg == 1) {   // the single staging buffer: the store of step jb-1 must have read it
+        if (tid == 0) bulk_wait_read<0>();
+        consumer_sync();
       }
+      VZ_ST(t_sync += clock64() - tc; tc = clock64();)
+      // Rows i = 2 ip, 2 ip + 1 of this thread are pair p = 16 ip + ty: one 16-byte store per column, into chunk
+      // c = col % 8 of row p of box col / 8, swizzled to chunk c ^ (p % 8).  A 16-byte store is served 8 lanes at
+      // a time, lanes tx = 0-7 of one ty: tx 0-3 and 4-7 write the same chunks of two boxes (4 KB apart, the same
+      // banks), so lanes with tx >= 4 take their two columns of a chunk pair in swapped order, filling the odd
+      // chunks while tx 0-3 fill the even ones.
+      {
+        double* stg = sk + (jb % nstg) * kStgDoubles;
+        const bool swap = (tx & 4) != 0;
+#pragma unroll
+        for (int ip = 0; ip < 2; ++ip) {
+          const int p = 16 * ip + ty;
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = jj ^ 1;
+            const double v0 = swap ? kv[2 * ip][j] : kv[2 * ip][jj], v1 = swap ? kv[2 * ip + 1][j] : kv[2 * ip + 1][jj];
+            const int cj = GP1::col_of(tx, jj) ^ (swap ? 1 : 0);
+            *reinterpret_cast<double2*>(stg + (cj >> 3) * kABox + p * 16 + (((cj & 7) ^ (p & 7)) * 2)) = make_double2(v0, v1);
+          }
+        }
+      }
+      fence_proxy_async_smem();   // these writes before the TMA store that reads them (issued after the next barrier)
       VZ_ST(t_st += clock64() - tc;)
-      VZ_ST(tc = clock64();)
-      consumer_sync();  // everyone is done with buffer `buf` (and zb) before it is refilled
-      VZ_ST(t_sync += clock64() - tc;)
     }
+    // The staging writes of the last step are done everywhere; its store goes out, and every K* store of the
+    // tile is complete (written to global memory) before the tile gate.  The gate's barrier then orders them
+    // before the producer's TMA loads of the tile in phase 2: both are async-proxy accesses to global memory,
+    // so completion of the bulk group, followed by the barrier, is all the ordering the loads need.
+    VZ_ST(long long tc = clock64();)
+    consumer_sync();
+    VZ_ST(t_sync += clock64() - tc; tc = clock64();)
+    if (tid == 0) store_step(nj - 1);
+    VZ_ST(t_st += clock64() - tc; tc = clock64();)
+    if (tid == 0) bulk_wait<0>();
+    VZ_ST(t_sync += clock64() - tc;)
     cp_async_wait<0>();
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -560,18 +633,31 @@ int make_tensor_map_u8(void* map, const void* base, int rank, const uint64_t* di
 }
 
 size_t score_smem_bytes(int dc, int dk, bool with_linf) {
-  (void)with_linf; (void)dc;
-  const size_t big = kStages * kStageDoubles > 3 * kMaxDc * kLD1 ? kStages * kStageDoubles : 3 * kMaxDc * kLD1;
-  return 1024 + sizeof(double) * (big + 128 + 64 * 2 + 256 + 8) +
+  (void)with_linf; (void)dc;   // phase 1's plan for any dc fits in the ring (stg_buffers)
+  return 1024 + sizeof(double) * (kStages * kStageDoubles + 64 * 2 + 256 + 8) +
          sizeof(int32_t) * dk * 2 * kLD1 + kMaxDc;
 }
 
-// K* scratch of `bytes` bytes on the handle.  It is written and re-read by the same CTA tile after tile:
-// pin it in L2 (persisting access-policy window) so its dirty lines are overwritten in place instead
-// of being evicted to HBM.  Best effort: failures only cost DRAM write-backs.
-static int ensure_scratch(vzgp_handle* h, size_t scratch_bytes) {
-  if (scratch_bytes > h->scratch.bytes || h->scratch_window != h->scratch.ptr) {
-    VZ_TRY(h->scratch.reserve(scratch_bytes));
+// K* scratch of `bytes` bytes on the handle.  It is written and re-read by the same CTA tile after tile.
+// persist: pin it in L2 (persisting access-policy window) so its dirty lines are overwritten in place instead
+// of being evicted to HBM; the small-pool route asks for that.  Best effort: failures only cost DRAM write-backs.
+// k_score asks for no window and removes one a small-pool call installed: its K* leaves by TMA store, and with
+// the window installed those stores drained so slowly that phase 1 waited on them (C2: 2.90 ms per pass against
+// 2.77 ms without the window, H100 80GB HBM3, 700 W), while the generic stores it replaced ran at the same speed
+// either way.
+static int ensure_scratch(vzgp_handle* h, size_t scratch_bytes, bool persist) {
+  if (scratch_bytes > h->scratch.bytes) VZ_TRY(h->scratch.reserve(scratch_bytes));
+  if (!persist) {
+    if (h->scratch_window != nullptr) {
+      cudaStreamAttrValue attr;
+      memset(&attr, 0, sizeof(attr));   // num_bytes 0: no window
+      cudaStreamSetAttribute(h->stream, cudaStreamAttributeAccessPolicyWindow, &attr);
+      cudaGetLastError();
+      h->scratch_window = nullptr;
+    }
+    return 0;
+  }
+  if (h->scratch_window != h->scratch.ptr) {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, h->device) == cudaSuccess && prop.persistingL2CacheMaxSize > 0) {
       size_t want = h->scratch.bytes;
@@ -640,7 +726,7 @@ int prepare_small_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int
                         double* score, double* mu, double* sigma, double* linf, ScoreArgs* a, bool* with_linf,
                         const AcqFn* fn) {
   const int ntiles = (M + kTM - 1) / kTM;
-  VZ_TRY(ensure_scratch(h, (size_t)ntiles * kTM * h->np * sizeof(double)));
+  VZ_TRY(ensure_scratch(h, (size_t)ntiles * kTM * h->np * sizeof(double), true));
   fill_score_args(h, Xs, Zs, M, acq, fn, score, mu, sigma, linf, a);
   const int nvb = h->np / kVarCols, nmb = h->np / 64;
   VZ_TRY(h->Tws.reserve(sizeof(double) * (size_t)(nvb + 2 * nmb) * a->mpad));
@@ -838,10 +924,11 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
   const int grid = (want < slots ? want : slots) * csize;
   cfg.gridDim = dim3(grid);
   record(nsplit > 1 ? VZGP_ROUTE_SPLIT : VZGP_ROUTE_CLUSTER, nsplit, grid);
-  VZ_TRY(ensure_scratch(h, (size_t)grid * kTM * h->np * sizeof(double)));
+  VZ_TRY(ensure_scratch(h, (size_t)grid * kTM * h->np * sizeof(double), false));
   fill_score_args(h, Xs, Zs, M, acq, fn, score, mu, sigma, linf, &a);
-  // K* in pair order: grid * 32 row pairs of 2 np doubles; a box is one k group (32 pairs x 8 k x 2 rows)
-  VZ_TRY(make_map(&a.mapA, a.scratch, (uint64_t)grid * (kTM / 2), 2 * (uint64_t)h->np, 2 * (uint64_t)h->np, kTM / 2));
+  // K* in pair order, box by box: per CTA np / 8 dense boxes of one k group (32 pairs x 8 k x 2 rows), so the map
+  // is [grid * np / 8 * 32 rows][16 doubles] and every box, stored or loaded, is 4 KB of consecutive bytes
+  VZ_TRY(make_map(&a.mapA, a.scratch, (uint64_t)grid * (kTM / 2) * (h->np / 8), 16, 16, kTM / 2));
   static_assert(4 * kABox == kTM * kBK, "four A boxes hold one slab of K*");
   VZ_TRY(make_map(&a.mapB, a.Linv, (uint64_t)h->np, (uint64_t)h->np, (uint64_t)h->np, kBPieceRows));
   a.nsplit = nsplit;
