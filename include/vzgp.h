@@ -177,11 +177,23 @@ typedef enum vzgp_factor_route {
   VZGP_FACTOR_DATAFLOW = 1 /* k_chol_dataflow: factor, L^-1, L^-T (and K_y^-1 for the NLL) in one launch */
 } vzgp_factor_route;
 
+/* Form the last Eagle loop on a handle took (vzgp_get_int key "eagle_route"; -1 before the first).  Every
+ * vzgp_eagle_run* call records it on the handle that owns the optimiser state (its first handle argument; the
+ * stack's top level); vzgp_eagle_begin records the stepped form.  The forms are chosen by size: a cooperative
+ * launch that the device refuses records the graph form that ran in its place. */
+typedef enum vzgp_eagle_route {
+  VZGP_EAGLE_PERSISTENT = 0,   /* np == 64, batch <= 64: the whole loop in one CTA, k_eagle_persistent64 */
+  VZGP_EAGLE_COOPERATIVE = 1,  /* batch <= 512, single-metric acquisition: one cooperative launch, k_eagle_grid */
+  VZGP_EAGLE_GRAPH = 2,        /* suggest -> score -> update launches, replayed from a CUDA graph after step 0 */
+  VZGP_EAGLE_STEPPED = 3       /* vzgp_eagle_begin / seed / ask / tell / end: the caller scores every batch */
+} vzgp_eagle_route;
+
 /* Counters.  "launches" (= vzgp_launch_count), "score_i8_launches": launches of the integer-split scoring kernel.
  * "sm_count": multiprocessors of the handle's device.  Of the last scoring call: "score_route" (vzgp_score_route),
  * "score_nsplit" (CTAs per 64-candidate tile: > 1 on the split route only, 1 on the cluster and i8 routes, 0
  * otherwise), "score_grid" (CTAs of the k_score / k_score_i8 launch, 0 on the other routes).  Of the last NLL
- * evaluation and factorisation: "nll_route" (vzgp_nll_route), "factor_route" (vzgp_factor_route). */
+ * evaluation and factorisation: "nll_route" (vzgp_nll_route), "factor_route" (vzgp_factor_route).  Of the last
+ * Eagle loop: "eagle_route" (vzgp_eagle_route). */
 int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value);
 
 /* ---- stage-wise entry points (parity tests call these one by one) -------- */

@@ -241,6 +241,16 @@ def suggest(state: EagleState, batch_size: int, signs: np.ndarray, cfg: EagleCon
   return np.clip(new, 0.0, 1.0)
 
 
+def batch_best(best_reward: float, batch_rewards: np.ndarray) -> float:
+  """The best reward seen so far after one more batch, a NaN reward counting as -inf.
+
+  Deliberate deviation (DESIGN.md 6b): the reference's `jnp.max` over a batch with a NaN is NaN, which becomes
+  `best_reward` for the rest of the run, so `rewards != best_reward` holds for every fly and the best fly loses its
+  protection from trimming.  NaN ranks as -inf everywhere else in the optimiser (update_best), and here as well."""
+  r = np.where(np.isnan(batch_rewards), -np.inf, batch_rewards)
+  return max(best_reward, float(np.max(r)))
+
+
 def update(
     state: EagleState, batch_size: int, batch_features: np.ndarray, batch_rewards: np.ndarray,
     random_features: np.ndarray, cfg: EagleConfig,
@@ -248,7 +258,7 @@ def update(
   """eagle_strategy.py:1075-1247 (update, _update_pool_features_and_rewards, _trim_pool)."""
   pool_size = state.features.shape[0]
   nb = pool_size // batch_size
-  new_best = max(state.best_reward, float(np.max(batch_rewards)))
+  new_best = batch_best(state.best_reward, batch_rewards)
   start = (state.iterations % nb) * batch_size
   sl = slice(start, start + batch_size)
   pert = state.perturbations[sl]
@@ -289,9 +299,10 @@ def update_best(best_f, best_r, best_id, new_f, new_r, new_id, count):
 def run_eagle_optimizer(
     score_fn: Callable[[np.ndarray], np.ndarray], *, dim: int, pool_size: int, batch_size: int,
     max_evaluations: int, count: int, seed: int, cfg: EagleConfig = EagleConfig(),
-    prior_features: Optional[np.ndarray] = None,
+    prior_features: Optional[np.ndarray] = None, on_step: Optional[Callable[[int, EagleState], None]] = None,
 ):
-  """VectorizedOptimizer.__call__ with the eagle strategy and Philox draws."""
+  """VectorizedOptimizer.__call__ with the eagle strategy and Philox draws.  on_step(t, state) sees the strategy
+  state after the update of step t (tests count trims and protected flies there)."""
   prior_rewards = None
   if prior_features is not None and prior_features.shape[0] > 0:
     prior_rewards = score_fn(prior_features)
@@ -307,6 +318,8 @@ def run_eagle_optimizer(
     r = score_fn(x)
     rnd = philox_uniform(seed, STREAM_TRIM, t, batch_size * dim).reshape(batch_size, dim)
     state = update(state, batch_size, x, r, rnd, cfg)
+    if on_step is not None:
+      on_step(t, state)
     ids = np.arange(batch_size, dtype=np.int64) + t * batch_size
     best_f, best_r, best_id = update_best(best_f, best_r, best_id, x, r, ids, count)
   return best_f, best_r, state
@@ -394,7 +407,8 @@ def categorical_logits(pool_z, batch_z, scale, sizes, cfg: EagleConfig) -> np.nd
     for i in range(b):
       lg = np.array([np.sum(np.where(pool_z[:, k] == c, scale[i], 0.0)) for c in range(max_size)]) + log_diff
       lg = np.where(np.arange(max_size) < s_k, lg, -np.inf)
-      lg[batch_z[i, k]] += -np.sum(scale[i]) + log_same - log_diff
+      with np.errstate(invalid='ignore'):    # a size-1 feature: inf - inf, and its logits are never sampled
+        lg[batch_z[i, k]] += -np.sum(scale[i]) + log_same - log_diff
       out[i, k] = lg
   return out
 
@@ -418,7 +432,8 @@ def create_features_mixed(pool, pool_z, rewards, batch, batch_z, rewards_batch, 
 
 
 def run_eagle_optimizer_mixed(score_fn, *, dim: int, sizes, pool_size: int, batch_size: int, max_evaluations: int,
-                              count: int, seed: int, cfg: EagleConfig = EagleConfig(), prior_c=None, prior_z=None):
+                              count: int, seed: int, cfg: EagleConfig = EagleConfig(), prior_c=None, prior_z=None,
+                              on_step=None):
   """VectorizedOptimizer + eagle strategy with continuous AND categorical features, Philox draws.
 
   score_fn(xc [B,Dc], xz [B,Dk]) -> [B].  Element numbering of the draws is the contract shared
@@ -465,7 +480,7 @@ def run_eagle_optimizer_mixed(score_fn, *, dim: int, sizes, pool_size: int, batc
                                      lap * factor * perts[sl][:, None, None], gum, sizes, cfg, pu, qu)
     bc = np.clip(bc, 0.0, 1.0)
     r = score_fn(bc, bz)
-    new_best = max(best_reward, float(np.max(r)))
+    new_best = batch_best(best_reward, r)
     if t < nb:
       pool_c[sl], pool_z[sl], rewards[sl] = bc, bz, r
     else:
@@ -478,6 +493,8 @@ def run_eagle_optimizer_mixed(score_fn, *, dim: int, sizes, pool_size: int, batc
       pool_c[sl] = np.where(trim[:, None], rc, nc); pool_z[sl] = np.where(trim[:, None], rz, nz)
       rewards[sl] = np.where(trim, -np.inf, nr); perts[sl] = np.where(trim, cfg.perturbation, npert)
     best_reward = new_best
+    if on_step is not None:     # as in run_eagle_optimizer; the state's features are the continuous ones
+      on_step(t, EagleState(t + 1, pool_c, rewards, best_reward, perts).copy())
     ids = np.arange(batch_size, dtype=np.int64) + t * batch_size
     f = np.concatenate([bc, best_c]); z = np.concatenate([bz, best_z]); rr = np.concatenate([r, best_r]); ii = np.concatenate([ids, best_id])
     order = np.lexsort((ii, -np.where(np.isnan(rr), -np.inf, rr)))[:count]
@@ -503,7 +520,7 @@ def set_perturbation_directions(seed: int, iteration: int, batch_size: int, q: i
 def run_eagle_optimizer_sets(
     score_fn: Callable[[np.ndarray], np.ndarray], *, dim: int, n_parallel: int, pool_size: int, batch_size: int,
     max_evaluations: int, count: int, seed: int, cfg: EagleConfig = EagleConfig(),
-    prior_features: Optional[np.ndarray] = None,
+    prior_features: Optional[np.ndarray] = None, on_step: Optional[Callable[[int, EagleState], None]] = None,
 ):
   """VectorizedOptimizer.__call__(n_parallel=q) with the eagle strategy and Philox draws.
 
@@ -528,6 +545,8 @@ def run_eagle_optimizer_sets(
     r = score_fn(x.reshape(batch_size, q, dim))
     rnd = philox_uniform(seed, STREAM_TRIM, t, batch_size * width).reshape(batch_size, width)
     state = update(state, batch_size, x, r, rnd, cfg)
+    if on_step is not None:
+      on_step(t, state)
     ids = np.arange(batch_size, dtype=np.int64) + t * batch_size
     best_f, best_r, best_id = update_best(best_f, best_r, best_id, x, r, ids, count)
   return best_f.reshape(count, q, dim), best_r, state

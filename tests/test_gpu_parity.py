@@ -290,7 +290,9 @@ def test_random_search_matches_oracle(dev):
 
 # The last two rows are BASELINE C3's shape (P = B = 1000 fireflies, N = 1000 trials, D = 20) and a
 # batch-600 case: batches above 512 take the replayed CUDA-graph form of the loop (c_abi.cu,
-# eagle_run_impl) with k_eagle_suggest / k_eagle_update at 1000 flies and the large-pool k_score.
+# eagle_run_impl) with k_eagle_suggest / k_eagle_update at 1000 flies and the large-pool k_score.  The form each row
+# takes is asserted.  At every size here the trust radius is above 0.5 (the region is off) and no fly is visited often
+# enough to be trimmed: tests/test_gpu_eagle_steps.py covers the active region, trimming, ties and non-finite rewards.
 @pytest.mark.parametrize('n,d,pool,batch,steps', [(30, 4, 25, 25, 6), (60, 5, 20, 5, 14), (130, 3, 50, 25, 7),
                                                   (1000, 20, 1000, 1000, 6), (700, 12, 1200, 600, 7)])
 def test_eagle_run_matches_oracle(dev, n, d, pool, batch, steps):
@@ -308,6 +310,8 @@ def test_eagle_run_matches_oracle(dev, n, d, pool, batch, steps):
                          cfg_o.perturbation_lower_bound, cfg_o.penalize_factor, cfg_o.normalization_scale,
                          cfg_o.prior_trials_pool_pct, pool, batch, steps * batch)
   bx, _, br = dev.eagle_run(cfg, _gp().Acquisition(1.8, True, radius), count=3, seed=7, prior=x)
+  assert radius > 0.5
+  assert dev.get_int('eagle_route') == (0 if n <= 64 else 1 if batch <= 512 else 2)   # persistent, cooperative, graph
   np.testing.assert_allclose(br, wr, atol=1e-9)
   np.testing.assert_allclose(bx, wx, atol=1e-9)
 

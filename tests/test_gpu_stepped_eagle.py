@@ -73,8 +73,9 @@ def test_stepped_loop_reproduces_eagle_run_and_oracle_with_prior_term(dev, n, d,
       se.tell()
     return se.end()
 
-  # 1. the library's acquisition as the scorer: the same run as vzgp_eagle_run (graph / cooperative forms)
+  # 1. the library's acquisition as the scorer: the same run as vzgp_eagle_run (the cooperative form at these sizes)
   bx0, _, br0 = dev.eagle_run(cfg, acq, count=3, seed=7, prior=x)
+  assert dev.get_int('eagle_route') == 1          # vzgp_eagle_route: cooperative
   bx1, _, br1 = run_stepped(False)
   np.testing.assert_allclose(br1, br0, atol=1e-9)
   np.testing.assert_allclose(bx1, bx0, atol=1e-9)

@@ -656,6 +656,7 @@ int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value) {
   if (std::strcmp(key, "score_grid") == 0) { *value = h->score_grid; return 0; }
   if (std::strcmp(key, "nll_route") == 0) { *value = h->nll_route; return 0; }
   if (std::strcmp(key, "factor_route") == 0) { *value = h->factor_route; return 0; }
+  if (std::strcmp(key, "eagle_route") == 0) { *value = h->eagle_route; return 0; }
   set_error("vzgp_get_int: unknown key '%s'", key);
   return VZGP_ERR_ARG;
 }
@@ -1165,14 +1166,17 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
   if (fused_ok && eagle_persistent_eligible(h, pe ? hB : nullptr, e)) {
     // small study: the whole loop is one persistent single-CTA kernel
     VZ_TRY(launch_eagle_persistent64(h, pe ? hB : nullptr, e, acq, pe, steps, fn));
+    h->eagle_route = VZGP_EAGLE_PERSISTENT;
     done = true;
   } else if (fused_ok && eagle_grid_eligible(h, pe ? hB : nullptr, e)) {
     // mid-size study: one cooperative launch, phases separated by grid barriers.  If the cooperative
     // launch is refused (nothing has run then) the launch-per-phase loop below takes over.
     done = launch_eagle_grid(h, pe ? hB : nullptr, e, acq, pe, steps, fn) == 0;
-    if (!done) cudaGetLastError();
+    if (done) h->eagle_route = VZGP_EAGLE_COOPERATIVE;
+    else cudaGetLastError();
   }
   if (!done) {
+  h->eagle_route = VZGP_EAGLE_GRAPH;
   VZ_TRY(one_step());
   if (steps > 1) {
     const int64_t l0 = h->launches;
@@ -1240,6 +1244,7 @@ int vzgp_eagle_begin(vzgp_handle* h, const vzgp_eagle_config* cfg, const int32_t
   if (rc < 0) { delete st; return rc; }
   st->n_prior = n_prior;
   h->eagle_step = st;
+  h->eagle_route = VZGP_EAGLE_STEPPED;
   if (prior_rewards_dev) *prior_rewards_dev = st->es.prior_r;
   return 0;
 }

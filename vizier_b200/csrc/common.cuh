@@ -194,6 +194,10 @@ struct vzgp_handle {
   int small_tiles = -1;
   int score_route = -1, score_nsplit = 0, score_grid = 0;
 
+  // Form of the last Eagle loop on this handle (vzgp_eagle_route); -1 before the first.  A cooperative launch that was
+  // refused records the graph form that ran instead.  Tests read it through vzgp_get_int.
+  int eagle_route = -1;
+
   // Acquisition function set by vzgp_set_acquisition (c_abi.cu); without one the calls score UCB with their
   // vzgp_acq.ucb_coefficient.  Read at every call: no launch state is built from it.
   bool has_acq_fn = false;
