@@ -534,6 +534,26 @@ int vzgp_eagle_run_ensemble(vzgp_handle* const* hs, int E, const vzgp_eagle_conf
 int vzgp_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
                   const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all);
 
+/* GP-UCB-PE over uniform ensembles (VizierGPUCBPEBandit(ensemble_size = E), gp_ucb_pe.py with
+ * stochastic_process_model.py:835-868): hAs are the E members of model A (completed trials), hBs the E members of
+ * model B (completed + pending trials), 1 <= E <= 8, member e of both with the same hyper-parameters.  All 2E handles
+ * share device and stream and are single-metric; the members of one model share their trials.  Each prediction is the
+ * equal-weight mixture of the members, in the two-pass form
+ *   mean = (1/E) sum_e mu_e,   var = (1/E) sum_e sigma_e^2 + (1/E) sum_e (mu_e - mean)^2
+ * (members summed in index order: repeated calls are bit-identical), and the acquisition is vzgp_score_pe's on the
+ * mixtures: UCB = mean_A + c sigma_B, PE = sigma_B + p min(mean_A + e sigma_A - threshold, 0), then the strict trust
+ * region against the first tr_rows trials of hBs[0].  mu / sigma (mixture of A) and sigma_all (mixture of B) are
+ * optional device outputs [M].  E = 1 computes what vzgp_score_pe computes. */
+int vzgp_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const double* Xs, const int32_t* Zs,
+                           int M, const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all);
+/* vzgp_eagle_run with vzgp_score_pe_ensemble as the scoring function.  Forms (vzgp_get_int "eagle_route" on hAs[0]):
+ * E = 1 is the single-model loop of vzgp_eagle_run_pe; for 2 <= E <= 7 the cooperative form runs all 2E member models
+ * in one persistent grid (batch <= 512, Matern kernels, distinct handles); otherwise the replayed graph. */
+int vzgp_eagle_run_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const vzgp_eagle_config* cfg,
+                               const vzgp_pe_params* pe, const double* prior, const int32_t* prior_z, int n_prior,
+                               const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
+                               double* best_score);
+
 /* Transfer learning: a stack of residual GPs (StackedResidualGP, gp/gp_models.py:91-140, :245-300; VizierGPBandit.
  * set_priors, gp_bandit.py:289-318).  hs[0] is fitted on the first prior study, every further hs[e] on the residuals
  * y - (sum of the means of the levels below) of the next study, hs[E-1] on the current study.  Combined prediction

@@ -240,6 +240,9 @@ SIGNATURES = {
     'vzgp_eagle_run': (_i, [_vp, _pE, _pA, _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32, _pd]),
     'vzgp_score_pe': (_i, [_vp, _vp, _vp, _vp, _i, _pPE, _vp, _vp, _vp, _vp]),
     'vzgp_eagle_run_pe': (_i, [_vp, _vp, _pE, _pPE, _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32, _pd]),
+    'vzgp_score_pe_ensemble': (_i, [C.POINTER(_vp), C.POINTER(_vp), _i, _vp, _vp, _i, _pPE, _vp, _vp, _vp, _vp]),
+    'vzgp_eagle_run_pe_ensemble': (_i, [C.POINTER(_vp), C.POINTER(_vp), _i, _pE, _pPE, _vp, _vp, _i, _pi32, _i, _u64,
+                                        _pd, _pi32, _pd]),
     'vzgp_score_pe_multi': (_i, [_vp, _vp, _vp, _vp, _i, C.POINTER(PeMultiParams), _vp, _vp, _vp, _vp]),
     'vzgp_eagle_run_pe_multi': (_i, [_vp, _vp, _pE, C.POINTER(PeMultiParams), _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32,
                                      _pd]),

@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "launchers.h"
+#include "pe_ensemble.cuh"
 
 namespace vzgp {
 
@@ -1115,10 +1116,12 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
                           double* best_score, vzgp_handle* const* ens = nullptr, int n_ens = 0,
                           const vzgp_scalarization* scal = nullptr, const double* stack_alphas = nullptr,
                           const vzgp_pe_multi_params* pem = nullptr, vzgp_handle* const* sep = nullptr,
-                          int n_sep = 0) {
+                          int n_sep = 0, vzgp_handle* const* ens_b = nullptr) {
   VZ_ARG(h && cfg && (acq || pe || scal || pem) && best_score, "handle / pointers");
   const AcqFn* fn = (pe || scal || pem) ? nullptr : handle_acq(ens ? ens[0] : h);   // multi-handle calls: the setting of hs[0]
+  // GP-UCB-PE ensembles: ens = the E members of model A (h = ens[0]), ens_b those of model B (hB = ens_b[0])
   auto score_batch = [&](const double* xs, const int32_t* zs, int m, double* out) -> int {
+    if (pe && ens_b) return launch_score_pe_ensemble(ens, ens_b, n_ens, xs, zs, m, pe, out, nullptr, nullptr, nullptr);
     if (pem) return launch_score_pe_multi(h, hB, xs, zs, m, pem, out, nullptr, nullptr, nullptr);
     if (sep) return launch_score_separable(sep, n_sep, xs, zs, m, out, nullptr, nullptr);
     if (scal) return launch_score_multi(h, xs, zs, m, out, nullptr, nullptr);
@@ -1172,6 +1175,11 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
     // mid-size study: one cooperative launch, phases separated by grid barriers.  If the cooperative
     // launch is refused (nothing has run then) the launch-per-phase loop below takes over.
     done = launch_eagle_grid(h, pe ? hB : nullptr, e, acq, pe, steps, fn) == 0;
+    if (done) h->eagle_route = VZGP_EAGLE_COOPERATIVE;
+    else cudaGetLastError();
+  } else if (pe && ens_b && eagle_grid_pe_ensemble_eligible(ens, ens_b, n_ens, e)) {
+    // the same cooperative loop over the 2E member models (E = 1 took the single-model forms above)
+    done = launch_eagle_grid_pe_ensemble(ens, ens_b, n_ens, e, pe, steps) == 0;
     if (done) h->eagle_route = VZGP_EAGLE_COOPERATIVE;
     else cudaGetLastError();
   }
@@ -1448,6 +1456,42 @@ int vzgp_eagle_run_ensemble(vzgp_handle* const* hs, int E, const vzgp_eagle_conf
   VZ_ARG(acq != nullptr, "acq");
   return eagle_run_impl(hs[0], nullptr, cfg, acq, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
                         best_z, best_score, hs, E);
+}
+
+static int check_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const vzgp_pe_params* pe) {
+  VZ_ARG(hAs != nullptr && hBs != nullptr && pe != nullptr, "handles / pe");
+  VZ_ARG(E >= 1 && E <= kMaxPeEnsemble, "1 <= E <= 8 members per model");
+  for (int k = 0; k < 2 * E; ++k) {
+    vzgp_handle* h = k < E ? hAs[k] : hBs[k - E];
+    VZ_ARG(h != nullptr, "handle");
+    if (!h->fitted) { set_error("GP-UCB-PE ensemble scoring needs every member of both models fitted"); return VZGP_ERR_STATE; }
+    VZ_ARG(h->device == hAs[0]->device && h->stream == hAs[0]->stream, "all members must share device and stream");
+    VZ_ARG(h->dc == hAs[0]->dc && h->dk == hAs[0]->dk, "all members must have the same feature dimensions");
+    VZ_ARG(h->n_metrics == 1, "GP-UCB-PE ensembles: single-metric members");
+    const vzgp_handle* first = k < E ? hAs[0] : hBs[0];
+    VZ_ARG(h->n_valid == first->n_valid && h->np == first->np, "the members of a model must be fitted on the same trials");
+  }
+  VZ_ARG(pe->mode == 0 || pe->mode == 1, "mode");
+  return 0;
+}
+
+int vzgp_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const double* Xs, const int32_t* Zs,
+                           int M, const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all) {
+  VZ_TRY(check_pe_ensemble(hAs, hBs, E, pe));
+  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
+  VZ_ARG(M == 0 || Xs != nullptr || hAs[0]->dc == 0, "Xs");
+  VZ_ARG(M == 0 || Zs != nullptr || hAs[0]->dk == 0, "Zs");
+  Guard g(hAs[0]->device);
+  return launch_score_pe_ensemble(hAs, hBs, E, Xs, Zs, M, pe, score, mu, sigma, sigma_all);
+}
+
+int vzgp_eagle_run_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const vzgp_eagle_config* cfg,
+                               const vzgp_pe_params* pe, const double* prior, const int32_t* prior_z, int n_prior,
+                               const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
+                               double* best_score) {
+  VZ_TRY(check_pe_ensemble(hAs, hBs, E, pe));
+  return eagle_run_impl(hAs[0], hBs[0], cfg, nullptr, pe, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
+                        best_z, best_score, hAs, E, nullptr, nullptr, nullptr, nullptr, 0, hBs);
 }
 
 static int check_qacq(const vzgp_qacq* qa, int n_sets, int q) {

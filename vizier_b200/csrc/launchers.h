@@ -111,6 +111,10 @@ int make_tensor_map_u8(void* map, const void* base, int rank, const uint64_t* di
                        const uint32_t* box, bool promote_256 = true);
 int launch_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
                     const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all);
+// GP-UCB-PE over uniform ensembles of E members per model (pe_ensemble.cuh; score.cu).
+int launch_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const double* Xs,
+                             const int32_t* Zs, int M, const vzgp_pe_params* pe, double* score, double* mu,
+                             double* sigma, double* sigma_all);
 int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const double* Xs, const int32_t* Zs, int M,
                        const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf,
                        const AcqFn* fn = nullptr);
@@ -221,6 +225,10 @@ int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e
 bool eagle_grid_eligible(const vzgp_handle* h, const vzgp_handle* hB, const EagleDev& e);
 int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const vzgp_acq* acq,
                       const vzgp_pe_params* pe, int steps, const AcqFn* fn = nullptr);
+// Its GP-UCB-PE ensemble form: the E members of A (hAs) and of B (hBs), E <= kMaxGridPeEnsemble (eagle_grid.cu).
+bool eagle_grid_pe_ensemble_eligible(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const EagleDev& e);
+int launch_eagle_grid_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const EagleDev& e,
+                                  const vzgp_pe_params* pe, int steps);
 size_t eagle_suggest_smem(const EagleDev& e);
 size_t eagle_update_smem(const EagleDev& e);
 size_t eagle_suggest_cta_smem(const EagleDev& e);

@@ -34,6 +34,7 @@
 
 #include "launchers.h"
 #include "matern_fast.cuh"
+#include "pe_ensemble.cuh"
 #include "score_small.cuh"
 #include "topk_merge.cuh"
 #include "tiles.cuh"
@@ -1157,6 +1158,59 @@ int launch_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const
     VZ_TRY(launch_score(hs[e], Xs, Zs, M, &none, dummy, mu_e + (size_t)e * M, sd_e + (size_t)e * M,
                         (e == 0 && want_linf) ? linf_buf : nullptr));
   k_ensemble_combine<<<(M + 255) / 256, 256, 0, h0->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma, h0->small.as<int>());
+  VZ_CHECK_LAUNCH();
+  h0->launches++;
+  return 0;
+}
+
+// ---------------------------------------------------------------------------
+// GP-UCB-PE over uniform ensembles (pe_ensemble.cuh): per candidate the mixtures of the E members of A and of B,
+// then the UCB / PE acquisition and the strict trust region.  Outputs: score, optional mixture mean / stddev of A
+// and stddev of B.
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_pe_ensemble_combine(int M, PeEnsCombine p, const double* __restrict__ mu_a,
+                                                             const double* __restrict__ sd_a,
+                                                             const double* __restrict__ mu_b,
+                                                             const double* __restrict__ sd_b,
+                                                             const double* __restrict__ linf, double* __restrict__ score,
+                                                             double* __restrict__ mu, double* __restrict__ sigma,
+                                                             double* __restrict__ sigma_all) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  double mean_a, s_a, mean_b, s_b;
+  pe_mixture(p.E, mu_a, sd_a, (size_t)M, m, mean_a, s_a);
+  pe_mixture(p.E, mu_b, sd_b, (size_t)M, m, mean_b, s_b);
+  score[m] = pe_ensemble_score(p, mean_a, s_a, s_b, linf[m]);
+  if (mu) mu[m] = mean_a;
+  if (sigma) sigma[m] = s_a;
+  if (sigma_all) sigma_all[m] = s_b;
+}
+
+// Every member is scored by launch_score (its own route): A members give mean and stddev, B members mean and stddev,
+// B member 0 also the trust-region distance (all B members share the trials).  The pieces live in hAs[0]->pe_tmp,
+// which launch_score does not touch: [4E + 2][M] = mu_a | sd_a | mu_b | sd_b (E rows each) | linf | dummy.
+int launch_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const double* Xs,
+                             const int32_t* Zs, int M, const vzgp_pe_params* pe, double* score, double* mu,
+                             double* sigma, double* sigma_all) {
+  if (M <= 0) return 0;
+  vzgp_handle* h0 = hAs[0];
+  VZ_TRY(h0->pe_tmp.reserve(sizeof(double) * (4 * (size_t)E + 2) * (size_t)M));
+  double* t = h0->pe_tmp.as<double>();
+  double* mu_a = t;
+  double* sd_a = t + (size_t)E * M;
+  double* mu_b = t + 2 * (size_t)E * M;
+  double* sd_b = t + 3 * (size_t)E * M;
+  double* linf_b = t + 4 * (size_t)E * M;
+  double* dummy = t + (4 * (size_t)E + 1) * M;
+  const PeEnsCombine p = pe_ensemble_args(hBs[0], E, pe);
+  const vzgp_acq none = posterior_request(), accb = posterior_request(pe->tr_dim_mask, pe->tr_rows);
+  for (int e = 0; e < E; ++e)
+    VZ_TRY(launch_score(hAs[e], Xs, Zs, M, &none, dummy, mu_a + (size_t)e * M, sd_a + (size_t)e * M, nullptr));
+  for (int e = 0; e < E; ++e)
+    VZ_TRY(launch_score(hBs[e], Xs, Zs, M, e == 0 ? &accb : &none, dummy, mu_b + (size_t)e * M, sd_b + (size_t)e * M,
+                        (e == 0 && tr_needs_distance(p.tr)) ? linf_b : nullptr));
+  k_pe_ensemble_combine<<<(M + 255) / 256, 256, 0, h0->stream>>>(M, p, mu_a, sd_a, mu_b, sd_b, linf_b, score, mu,
+                                                                 sigma, sigma_all);
   VZ_CHECK_LAUNCH();
   h0->launches++;
   return 0;

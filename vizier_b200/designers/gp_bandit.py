@@ -92,6 +92,21 @@ _PRIMES = [2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37, 41, 43, 47, 53, 59, 61, 6
            197, 199, 211, 223, 227, 229, 233, 239, 241, 251, 257, 263, 269, 271, 277, 281, 283, 293, 307, 311]
 
 
+def mixture_samples(comps, chol_dev, g: np.random.Generator, num_samples: int) -> np.ndarray:
+  """Warped joint samples [num_samples, n] of the equal-weight mixture of the members' joint posteriors `comps`
+  [(mean [n], cov [n, n]) device tensors]: every sample is a joint draw from one uniformly chosen member (one member:
+  no member draw).  Each (small) covariance is factored on the device by `chol_dev`; the retry adds a tiny jitter only
+  if round-off made it indefinite."""
+  factors = []
+  for mean, cov in comps:
+    chol, _, _ = chol_dev.cholesky_retry(cov, jitter=1e-10, max_iters=8)
+    factors.append((mean.cpu().numpy(), chol.cpu().numpy()))
+  m = factors[0][0].shape[0]
+  normals = g.standard_normal((num_samples, m))
+  member = g.integers(0, len(factors), size=num_samples) if len(factors) > 1 else np.zeros(num_samples, int)
+  return np.stack([factors[e][0] + normals[i] @ factors[e][1].T for i, e in enumerate(member)])
+
+
 class VizierGPBandit(vz.Designer, vz.Predictor):
   """GP-Bandit designer; see module docstring."""
 
@@ -392,17 +407,7 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
       samples = mean[None, :] + g.standard_normal((num_samples, mean.shape[0])) * sd[None, :]
       return self._output_warper.unwarp(samples.reshape(-1, 1)).reshape(samples.shape)
     comps = dev.posterior(xs, zq, add_noise=True) if self._ensemble_size > 1 else [dev.posterior(xs, zq, add_noise=True)]
-    # Cholesky of each (small) posterior covariance on the device as well; the retry adds a tiny
-    # jitter only if round-off made it indefinite.
-    factors = []
-    for mean, cov in comps:
-      chol, _, _ = self._ard_dev.cholesky_retry(cov, jitter=1e-10, max_iters=8)
-      factors.append((mean.cpu().numpy(), chol.cpu().numpy()))
-    m = factors[0][0].shape[0]
-    normals = g.standard_normal((num_samples, m))
-    # equal-weight mixture: every sample is a joint draw from one uniformly chosen member
-    member = g.integers(0, len(factors), size=num_samples) if len(factors) > 1 else np.zeros(num_samples, int)
-    samples = np.stack([factors[e][0] + normals[i] @ factors[e][1].T for i, e in enumerate(member)])
+    samples = mixture_samples(comps, self._ard_dev, g, num_samples)
     # one vectorised unwarp of all num_samples x num_trials values (the warpers act element-wise)
     return self._output_warper.unwarp(samples.reshape(-1, 1)).reshape(samples.shape)
 

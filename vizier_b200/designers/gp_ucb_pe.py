@@ -14,7 +14,7 @@ configuration (`UCBPEConfig()` with `optimize_set_acquisition_for_exploration=Fa
   * acquisition optimiser: Eagle with the tuned UCB-PE config and RANDOM force normalisation
     (:678-698).
 
-Everything numeric runs in libvzgp (two handles on one stream, `vzgp_score_pe`,
+Everything numeric runs in libvzgp (two handles, or two ensembles, on one stream, `vzgp_score_pe`,
 `vzgp_eagle_run_pe`); `sample` / `predict` (:1262-1354) draw from the device-computed joint posterior
 like `VizierGPBandit`.  `prior_acquisition` (a callable on NumPy features) is added to both acquisitions through the
 host-stepped Eagle loop (`gp.SteppedEagle`); `optimize_set_acquisition_for_exploration=True` optimises the rest of a
@@ -30,8 +30,18 @@ each UCB suggestion, floored at the best scalarised label and averaged; PE is st
 The strict trust region stays on.  Both run in `vzgp_score_pe_multi` / `vzgp_eagle_run_pe_multi`; `sample` returns
 [num_samples, n, num_metrics] and the prediction metadata holds per-metric vectors.
 
-Not implemented: ensembles (NotImplementedError); with several metrics also `mixes_linear_kernel`, task kernels other
-than INDEPENDENT (NotImplementedError) and `optimize_set_acquisition_for_exploration` (ValueError, as in the reference).
+Ensembles (`ensemble_size = E > 1`, single metric; stochastic_process_model.py:835-878): the E best of the 1 fixed +
+`ard_random_restarts` ARD initialisations (the first E initial points before any trial completes) give E members of
+model A (completed trials) and E of model B (completed + pending trials, the real labels on completed rows and 0 on
+pending rows); every prediction is the members' equal-weight mixture (two-pass variance), UCB / PE / the threshold
+are taken on the mixtures and model B's noise is forced to 1e-10 when every member's signal-to-noise ratio is low.
+Scoring and Eagle run in `vzgp_score_pe_ensemble` / `vzgp_eagle_run_pe_ensemble`; `sample` draws each joint sample
+from one uniformly chosen member.  The set-PE batch path raises ValueError with E > 1 (the reference cannot run it:
+its `if noise_is_high:` meets a per-member array there).
+
+Not implemented: ensembles with several metrics (NotImplementedError); with several metrics also
+`mixes_linear_kernel`, task kernels other than INDEPENDENT (NotImplementedError) and
+`optimize_set_acquisition_for_exploration` (ValueError, as in the reference).
 """
 
 from __future__ import annotations
@@ -170,8 +180,11 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
       if not isinstance(config.multimetric_promising_region_penalty_type, MultimetricPromisingRegionPenaltyType):
         raise ValueError('Unsupported multimetric promising region penalty type: '
                          f'{config.multimetric_promising_region_penalty_type}')
-    if (ensemble_size or 1) != 1:
-      raise NotImplementedError('ensembles are not implemented for GP-UCB-PE.')
+    self._ensemble_size = int(ensemble_size or 1)
+    if self._n_metrics > 1 and self._ensemble_size != 1:
+      raise NotImplementedError('ensembles of multi-metric models are not implemented for GP-UCB-PE.')
+    if self._ensemble_size < 1 or self._ensemble_size > ard_random_restarts + 1:
+      raise ValueError('ensemble_size must be in [1, ard_random_restarts + 1].')
     # mixes_linear_kernel: the Matern + feature-scaled linear kernel with a constant mean, linear_coef = 1
     # (gp_ucb_pe.py:805-809, :844-853; tuned_gp_models.py:203-245)
     self._linear_coef = 1.0 if mixes_linear_kernel else None
@@ -196,8 +209,8 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     self._output_warper = None
     self._output_warpers: list = []        # one per metric (gp_ucb_pe.py:917-942)
     self._device_index = device
-    self._dev_a: Optional[gp.DeviceGP] = None
-    self._dev_b: Optional[gp.DeviceGP] = None
+    self._dev_a = None    # gp.DeviceGP, or gp.EnsembleGP when ensemble_size > 1
+    self._dev_b = None
 
   # ------------------------------------------------------------------ API
   def update(self, completed, all_active) -> None:
@@ -212,9 +225,28 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
   # ------------------------------------------------------------------ internals
   def _devices(self):
     if self._dev_a is None:
-      self._dev_a = gp.DeviceGP(self._device_index)
-      self._dev_b = gp.DeviceGP(self._device_index, stream=self._dev_a.stream)  # same stream: ordered launches
+      if self._ensemble_size > 1:
+        self._dev_a = gp.EnsembleGP(self._device_index, self._ensemble_size)
+        self._dev_b = gp.EnsembleGP(self._device_index, self._ensemble_size, stream=self._dev_a.stream)
+      else:
+        self._dev_a = gp.DeviceGP(self._device_index)
+        self._dev_b = gp.DeviceGP(self._device_index, stream=self._dev_a.stream)  # same stream: ordered launches
     return self._dev_a, self._dev_b
+
+  def _ard_dev(self) -> gp.DeviceGP:
+    dev_a, _ = self._devices()
+    return dev_a.members[0] if self._ensemble_size > 1 else dev_a
+
+  def _params_out(self, vectors, dc: int, dk: int):
+    """GPHyperParams of the kept ARD results: one, or the list of E ensemble members."""
+    ps = [gp.GPHyperParams.from_vector(v, dc, dk, self._linear_coef) for v in vectors[:self._ensemble_size]]
+    return ps[0] if self._ensemble_size == 1 else ps
+
+  def _noise_is_high(self, params) -> bool:
+    """gp_ucb_pe.py:1018-1021: the signal-to-noise ratio is below the threshold (for every ensemble member)."""
+    members = params if isinstance(params, list) else [params]
+    return all(p.signal_variance / max(p.observation_noise_variance, 1e-12) < self._config.signal_to_noise_threshold
+               for p in members)
 
   def _generate_seed_trials(self, count: int):
     """gp_ucb_pe.py:750-787: centre first (if nothing exists yet), quasi-random afterwards."""
@@ -244,8 +276,9 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     return cont, cat, warped[0] if self._n_metrics == 1 else np.concatenate(warped, axis=-1)
 
   @profiler.record_runtime
-  def _build_gp_model_and_optimize_parameters(self, cont, cat, labels) -> gp.GPHyperParams:
-    """gp_ucb_pe.py:789-894: one fixed + `ard_random_restarts` random initialisations."""
+  def _build_gp_model_and_optimize_parameters(self, cont, cat, labels):
+    """gp_ucb_pe.py:789-894: one fixed + `ard_random_restarts` random initialisations; the best one, or the E best
+    (a list) for an ensemble (:867-878)."""
     dc, dk = cont.shape[1], cat.shape[1]
     rng = np.random.default_rng(int(self._rng.integers(2**62)))
     lin = self._linear_coef
@@ -254,9 +287,10 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
                              linear_shift=0.0, mean_constant=0.0).to_vector()[None, :]    # :833-853
     inits = np.concatenate([fixed, random_inits], axis=0)
     if cont.shape[0] == 0:
-      # no completed trial yet: the dummy loss makes the optimiser return its first initial point
-      return gp.GPHyperParams.from_vector(inits[0], dc, dk, lin)
-    dev_a, _ = self._devices()
+      # no completed trial yet: the dummy loss makes every loss equal, so the optimiser returns its first initial
+      # point(s)
+      return self._params_out(inits, dc, dk)
+    dev_a = self._ard_dev()
     import torch  # device-memory handles only
     xt = torch.from_numpy(np.ascontiguousarray(cont)).to(dev_a.device)
     # [N], or [N, n_metrics] for the independent multi-task GP (the losses sum over the metrics)
@@ -274,14 +308,15 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     else:
       fns = ard.loss_functions(dev_a, xt, yt, zt, dc, dk, workers=min(ard.MAX_ARD_WORKERS, inits.shape[0]), linear_coef=lin)
     try:
-      best, _ = self._ard_optimizer(inits, fns, list(zip(lo, hi)), best_n=1)
+      best, _ = self._ard_optimizer(inits, fns, list(zip(lo, hi)), best_n=self._ensemble_size)
     finally:
       dev_a.set_int('dataflow_ctas', 0)
-    return gp.GPHyperParams.from_vector(best[0], dc, dk, lin)
+    return self._params_out(best, dc, dk)
 
-  def _fit_all_features(self, params: gp.GPHyperParams, cont, cat, labels, pend_c, pend_z, noise_is_high: bool):
-    """_get_predictive_all_features (:944-1004): model B on completed + pending, dummy labels.  Its stddev does not
-    depend on the labels, so a multi-metric study fits B as one metric on zeros."""
+  def _fit_all_features(self, params, cont, cat, labels, pend_c, pend_z, noise_is_high: bool):
+    """_get_predictive_all_features (:944-1004): model B on completed + pending trials, the real labels on completed
+    rows and 0 on pending rows.  A single model's stddev does not depend on the labels, so a multi-metric study fits B
+    as one metric on zeros; an ensemble's mixture stddev does (the spread of the members' means)."""
     _, dev_b = self._devices()
     xc = np.concatenate([cont, pend_c], axis=0)
     xz = np.concatenate([cat, pend_z], axis=0)
@@ -291,7 +326,8 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
       y = np.zeros(xc.shape[0])
     p = params
     if noise_is_high:
-      p = dataclasses.replace(params, observation_noise_variance=1e-10)
+      p = ([dataclasses.replace(q, observation_noise_variance=1e-10) for q in params] if isinstance(params, list)
+           else dataclasses.replace(params, observation_noise_variance=1e-10))
     dev_b.fit(xc, y, p, z=xz if xz.shape[1] else None)
     return xc, xz
 
@@ -337,14 +373,26 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
         mode=1, thresholds=thresholds, region_penalty=_REGION_PENALTY_CODE[cfg.multimetric_promising_region_penalty_type],
         **common)
 
+  def _ucb_threshold(self, xc_all, xz_all) -> float:
+    """_compute_ucb_threshold (:175-218): mean of A at B's feature with the largest UCB_A; an ensemble takes the mixture
+    of A's members, which score_pe reports as its aux."""
+    cfg = self._config
+    dev_a, dev_b = self._devices()
+    if self._ensemble_size > 1:
+      out = dev_a.score_pe(dev_b, xc_all, gp.UcbPeAcquisition(use_trust_region=False), zs=xz_all)
+    else:
+      out = dev_a.score(xc_all, gp.Acquisition(cfg.ucb_coefficient, False, 1.0), zs=xz_all, with_aux=True)
+    dev_a.synchronize()
+    mu = out['mean'].cpu().numpy(); sd = out['stddev'].cpu().numpy()
+    return float(mu[int(np.argmax(mu + cfg.ucb_coefficient * sd))])
+
   @profiler.record_runtime
   def _suggest_one(self, active_trials, cont, cat, labels, params, mask, radius, n_tr_rows):
     """gp_ucb_pe.py:1006-1155."""
     start = datetime.datetime.now()
     cfg = self._config
     dev_a, dev_b = self._devices()
-    snr = params.signal_variance / max(params.observation_noise_variance, 1e-12)
-    noise_is_high = snr < cfg.signal_to_noise_threshold
+    noise_is_high = self._noise_is_high(params)
     pe_overwrite = cfg.pe_overwrite_probability_in_high_noise if noise_is_high else cfg.pe_overwrite_probability
     u = float(self._rng.uniform())
     if _has_new_completed_trials(self._all_completed_trials, active_trials):
@@ -362,11 +410,7 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     else:
       threshold = 0.0
       if not use_ucb and cont.shape[0] > 0:
-        # _compute_ucb_threshold (:175-218): mean of A at B's feature with the largest UCB_A
-        out = dev_a.score(xc_all, gp.Acquisition(cfg.ucb_coefficient, False, 1.0), zs=xz_all if dk else None, with_aux=True)
-        dev_a.synchronize()
-        mu = out['mean'].cpu().numpy(); sd = out['stddev'].cpu().numpy()
-        threshold = float(mu[int(np.argmax(mu + cfg.ucb_coefficient * sd))])
+        threshold = self._ucb_threshold(xc_all, xz_all if dk else None)
       pe = gp.UcbPeAcquisition(
           mode=0 if use_ucb else 1, ucb_coefficient=cfg.ucb_coefficient,
           explore_coefficient=cfg.explore_region_ucb_coefficient,
@@ -402,8 +446,7 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     start = datetime.datetime.now()
     cfg = self._config
     dev_a, dev_b = self._devices()
-    snr = params.signal_variance / max(params.observation_noise_variance, 1e-12)
-    noise_is_high = snr < cfg.signal_to_noise_threshold
+    noise_is_high = self._noise_is_high(params)
     pend_c, pend_z = self._converter.to_features(active_trials)
     pend_c = np.nan_to_num(pend_c, nan=0.0)
     xc_all, xz_all = self._fit_all_features(params, cont, cat, labels, pend_c, pend_z, noise_is_high)
@@ -461,6 +504,9 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     if count > 1 and self._config.optimize_set_acquisition_for_exploration and not prior_only:
       # gp_ucb_pe.py:1423-1434: one UCB / PE suggestion if trials completed since the newest active one, then the
       # rest of the batch as ONE set optimised for the set-PE acquisition
+      if self._ensemble_size > 1:
+        # the reference's set path tests `if noise_is_high:` on the per-member array (:996, :1168-1177) and fails
+        raise ValueError('optimize_set_acquisition_for_exploration does not support ensemble_size > 1.')
       if _has_new_completed_trials(self._all_completed_trials, active):
         out.append(self._suggest_one(active, cont, cat, labels, params, mask, radius, n_tr))
         active.append(out[-1].to_trial())
@@ -481,12 +527,11 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     degenerates to the prior mean 0 (_compute_ucb_threshold over no valid point, :175-218), so both the
     PE acquisition  stddev_B + 10 min(0 + 0.5 stddev_A - 0, 0)  and the UCB acquisition  0 + 1.8 stddev_B
     are maximised by the stddev of model B = the GP conditioned on the pending points with dummy labels.
-    That is `vzgp_eagle_run` on model B with a unit UCB coefficient (its mean is exactly 0)."""
+    That is `vzgp_eagle_run` on model B with a unit UCB coefficient (its mean is exactly 0; an ensemble: every member's
+    mean is 0, so `vzgp_eagle_run_ensemble` maximises the mixture stddev)."""
     start = datetime.datetime.now()
-    cfg = self._config
     _, dev_b = self._devices()
-    snr = params.signal_variance / max(params.observation_noise_variance, 1e-12)
-    noise_is_high = snr < cfg.signal_to_noise_threshold
+    noise_is_high = self._noise_is_high(params)
     pend_c, pend_z = self._converter.to_features(active_trials)
     pend_c = np.nan_to_num(pend_c, nan=0.0)
     empty_c = np.zeros((0, pend_c.shape[1])); empty_z = np.zeros((0, pend_z.shape[1]), np.int32)
@@ -495,7 +540,8 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     optimizer = self._acquisition_optimizer_factory(self._converter)
     res = optimizer(dev_b, acq, count=1, prior_features=None, prior_categorical=None, seed=int(self._rng.integers(2**62)))
     params_dict = self._converter.to_parameters(res.features[0:1], None if res.categorical is None else res.categorical[0:1])[0]
-    prior_sd = float(np.sqrt(params.signal_variance + params.observation_noise_variance))
+    members = params if isinstance(params, list) else [params]   # an ensemble: the mixture of the members' priors
+    prior_sd = float(np.sqrt(np.mean([p.signal_variance + p.observation_noise_variance for p in members])))
     sd_all = float(res.aux['stddev'][0]) if 'stddev' in res.aux else float(res.rewards[0])
     md = vz.Metadata()
     md.ns('devinfo')['acquisition_optimization'] = json.dumps(
@@ -527,6 +573,12 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     dev_a.fit(cont, self._fit_labels(labels), params, z=cat if cat.shape[1] else None)
     xs, zs = self._converter.to_features(trials)
     xs = np.nan_to_num(xs, nan=0.0)
+    if self._ensemble_size > 1:
+      # the uniform mixture: each joint sample from one uniformly drawn member (as VizierGPBandit)
+      g = np.random.default_rng(_gpb._seed_from(rng) if rng is not None else 0)
+      comps = dev_a.posterior(xs, zs if zs.shape[1] else None, add_noise=True)
+      samples = _gpb.mixture_samples(comps, dev_a.members[0], g, num_samples)
+      return self._output_warper.unwarp(samples.reshape(-1, 1)).reshape(samples.shape)
     mean, cov = dev_a.posterior(xs, zs if zs.shape[1] else None, add_noise=True)
     chol, _, _ = dev_a.cholesky_retry(cov, jitter=1e-10, max_iters=8)
     g = np.random.default_rng(_gpb._seed_from(rng) if rng is not None else 0)

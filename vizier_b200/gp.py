@@ -1149,10 +1149,13 @@ class EnsembleGP:
   (`VizierGPBandit(ensemble_size=E)`: the E best ARD restarts, gp_models.py:200-223; predictive =
   UniformEnsemblePredictive, stochastic_process_model.py:836-868).  The members are E libvzgp handles on
   ONE stream; scoring and the Eagle loop run through `vzgp_score_ensemble` / `vzgp_eagle_run_ensemble`.
-  Exposes the subset of the `DeviceGP` interface the acquisition optimiser drives."""
+  Exposes the subset of the `DeviceGP` interface the acquisition optimiser drives.  GP-UCB-PE pairs two ensembles
+  on one stream (`stream`): `score_pe` / `eagle_run(other=...)` with a `UcbPeAcquisition` score the mixture of both
+  (`vzgp_score_pe_ensemble` / `vzgp_eagle_run_pe_ensemble`), and the host-stepped loop (`SteppedEagle`) runs on
+  member 0's handle."""
 
-  def __init__(self, device: int, size: int):
-    first = DeviceGP(device)
+  def __init__(self, device: int, size: int, stream: Optional[torch.cuda.Stream] = None):
+    first = DeviceGP(device, stream=stream)
     self.members = [first] + [DeviceGP(device, stream=first.stream) for _ in range(size - 1)]
     self.device = first.device
     self._lib = first._lib
@@ -1161,6 +1164,22 @@ class EnsembleGP:
   @property
   def stream(self):
     return self.members[0].stream
+
+  # member 0 carries the state of the host-stepped Eagle loop (SteppedEagle drives these)
+  @property
+  def _h(self):
+    return self.members[0]._h
+
+  @property
+  def _stream(self):
+    return self.members[0]._stream
+
+  def _dev(self, a, dtype):
+    return self.members[0]._dev(a, dtype)
+
+  def close(self):
+    for m in self.members:
+      m.close()
 
   @property
   def launch_count(self) -> int:
@@ -1203,12 +1222,42 @@ class EnsembleGP:
     """`DeviceGP.score_qsets` under the uniform mixture of the members ('cov' [E, n_sets, q, q] per member)."""
     return _score_qsets(self.members, xs_sets, q, qacq, seed, zs, period, with_aux, with_cov)
 
+  def _pe_handles(self, other: 'EnsembleGP'):
+    assert isinstance(other, EnsembleGP) and len(other.members) == len(self.members), 'B needs one member per A member'
+    return self._handles(), other._handles()
+
+  def score_pe(self, other: 'EnsembleGP', xs, pe: UcbPeAcquisition, zs=None) -> dict:
+    """GP-UCB-PE score of the mixtures, self = ensemble on completed trials, other = ensemble on completed + pending
+    trials (member e of both with the same hyper-parameters).  Returns device tensors {'score', 'mean', 'stddev',
+    'stddev_from_all'} (mixture mean / stddev of A, mixture stddev of B); synchronous."""
+    f = self.members[0]
+    xst, zst = f._xz(xs, zs)
+    m = xst.shape[0]
+    res = {k: torch.empty((m,), dtype=torch.float64, device=self.device) for k in ('score', 'mean', 'stddev', 'stddev_from_all')}
+    f._stream.wait_stream(torch.cuda.current_stream(self.device))
+    p, keep = pe._c()
+    ha, hb = self._pe_handles(other)
+    _lib.check('vzgp_score_pe_ensemble', self._lib.vzgp_score_pe_ensemble(
+        ha, hb, len(self.members), _ptr(xst), _ptr(zst), m, C.byref(p), _ptr(res['score']), _ptr(res['mean']),
+        _ptr(res['stddev']), _ptr(res['stddev_from_all'])))
+    self.synchronize()
+    del keep
+    return res
+
   def eagle_run(self, cfg, acq: Acquisition, count: int, seed: int, prior=None, prior_z=None, cat_sizes=None,
                 other=None):
-    assert other is None
+    """`DeviceGP.eagle_run` on the mixture; with `other` (an EnsembleGP) and a UcbPeAcquisition the GP-UCB-PE
+    acquisition of the two mixtures is optimised (vzgp_eagle_run_pe_ensemble)."""
     f = self.members[0]
-    f._use_acq(acq)
-    a, keep = acq._c()
+    if isinstance(acq, UcbPeAcquisition):
+      p, keep = acq._c()
+      ha, hb = self._pe_handles(other)
+      fn, args = 'vzgp_eagle_run_pe_ensemble', (ha, hb, len(self.members), C.byref(cfg), C.byref(p))
+    else:
+      assert other is None
+      f._use_acq(acq)
+      a, keep = acq._c()
+      fn, args = 'vzgp_eagle_run_ensemble', (self._handles(), len(self.members), C.byref(cfg), C.byref(a))
     n_prior = 0 if prior is None else len(prior)
     pt = f._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
     pz = f._dev(prior_z, torch.int32) if n_prior > 0 and self.dk > 0 else None
@@ -1216,10 +1265,9 @@ class EnsembleGP:
     bz = np.zeros((count, self.dk), np.int32)
     bs = np.zeros(count, np.float64)
     sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
-    _lib.check('vzgp_eagle_run_ensemble', self._lib.vzgp_eagle_run_ensemble(
-        self._handles(), len(self.members), C.byref(cfg), C.byref(a), _ptr(pt), _ptr(pz), n_prior,
-        sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None, count, seed,
-        bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
+    _lib.check(fn, getattr(self._lib, fn)(
+        *args, _ptr(pt), _ptr(pz), n_prior, sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None,
+        count, seed, bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
         bs.ctypes.data_as(C.POINTER(C.c_double))))
     del keep
     return bx, bz, bs
