@@ -567,6 +567,37 @@ int vzgp_eagle_run_stack(vzgp_handle* const* hs, int E, const double* alphas, co
                          const vzgp_acq* acq, const double* prior, const int32_t* prior_z, int n_prior,
                          const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
                          double* best_score);
+/* A stack whose levels are uniform ensembles of E members each (VizierGPBandit(ensemble_size=E).set_priors):
+ * hs[l * E + e] is member e of level l (level-major), 1 <= n_levels <= 16, 1 <= E <= 8, all single-metric; the members
+ * of a level share its trials.  Each level's prediction is the two-pass mixture of its members (as in
+ * vzgp_score_pe_ensemble), and the levels are stacked as in vzgp_score_stack: mean = sum_l mean_l, s = sd_l^alphas[l] *
+ * s^(1 - alphas[l]) bottom-up.  The acquisition (vzgp_set_acquisition of hs[0]) and the trust region follow, the trust
+ * region measured against the trials of the top level's member 0, hs[(n_levels - 1) * E], which also computes linf.
+ * mu / sigma / linf are optional device outputs [M].  E = 1 calls vzgp_score_stack (bit-identical results). */
+int vzgp_score_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, const double* alphas, const double* Xs,
+                              const int32_t* Zs, int M, const vzgp_acq* acq, double* score, double* mu, double* sigma,
+                              double* linf);
+/* vzgp_eagle_run with vzgp_score_stack_ensemble as the scoring function; E = 1 calls vzgp_eagle_run_stack.  The loop
+ * runs as the replayed graph (the persistent and cooperative forms evaluate single models only); "eagle_route" is
+ * recorded on hs[(n_levels - 1) * E]. */
+int vzgp_eagle_run_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, const double* alphas,
+                                  const vzgp_eagle_config* cfg, const vzgp_acq* acq, const double* prior,
+                                  const int32_t* prior_z, int n_prior, const int32_t* cat_sizes, int count,
+                                  uint64_t seed, double* best_x, int32_t* best_z, double* best_score);
+/* A stack of independent multi-task levels (several metrics, vzgp_fit_multi; no linear kernel): every level has the
+ * same n_metrics >= 2, one factor (so one stddev per candidate, shared by the metrics) and one alpha per metric.
+ * mean_m = sum_l mean_l,m; the stddevs are stacked as in vzgp_score_stack; then the scalarised UCB of vzgp_score_multi
+ * on (mean_m, s), without a trust region.  The scalarisation is uploaded to the top level hs[n_levels - 1]
+ * (synchronises).  mu [n_metrics][M] and sigma [M] are optional device outputs. */
+int vzgp_score_stack_multi(vzgp_handle* const* hs, int n_levels, const double* alphas, const double* Xs,
+                           const int32_t* Zs, int M, const vzgp_scalarization* sc, double* score, double* mu,
+                           double* sigma);
+/* vzgp_eagle_run with vzgp_score_stack_multi as the scoring function, as the replayed graph (the persistent and
+ * cooperative forms evaluate single models only); "eagle_route" is recorded on hs[n_levels - 1]. */
+int vzgp_eagle_run_stack_multi(vzgp_handle* const* hs, int n_levels, const double* alphas, const vzgp_eagle_config* cfg,
+                               const vzgp_scalarization* sc, const double* prior, const int32_t* prior_z, int n_prior,
+                               const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
+                               double* best_score);
 
 /* Set-PE acquisition of GP-UCB-PE batches (SetPEScoreFunction, gp_ucb_pe.py:510-594): Xs holds n_sets sets of q points
  * ([n_sets * q x Dc] device, continuous features, q <= 16).  score[s] = logdet of the q x q joint predictive covariance

@@ -248,6 +248,13 @@ SIGNATURES = {
                                      _pd]),
     'vzgp_score_stack': (_i, [C.POINTER(C.c_void_p), _i, _pd, _vp, _vp, _i, _pA, _vp, _vp, _vp, _vp]),
     'vzgp_eagle_run_stack': (_i, [C.POINTER(C.c_void_p), _i, _pd, _pE, _pA, _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32, _pd]),
+    'vzgp_score_stack_ensemble': (_i, [C.POINTER(C.c_void_p), _i, _i, _pd, _vp, _vp, _i, _pA, _vp, _vp, _vp, _vp]),
+    'vzgp_eagle_run_stack_ensemble': (_i, [C.POINTER(C.c_void_p), _i, _i, _pd, _pE, _pA, _vp, _vp, _i, _pi32, _i, _u64,
+                                           _pd, _pi32, _pd]),
+    'vzgp_score_stack_multi': (_i, [C.POINTER(C.c_void_p), _i, _pd, _vp, _vp, _i, C.POINTER(Scalarization), _vp, _vp,
+                                    _vp]),
+    'vzgp_eagle_run_stack_multi': (_i, [C.POINTER(C.c_void_p), _i, _pd, _pE, C.POINTER(Scalarization), _vp, _vp, _i,
+                                        _pi32, _i, _u64, _pd, _pi32, _pd]),
     'vzgp_score_set_pe': (_i, [_vp, _vp, _vp, _i, _i, _pPE, _vp, _vp, _vp, _vp]),
     'vzgp_score_qsets': (_i, [C.POINTER(_vp), _i, _vp, _vp, _i, _i, C.POINTER(QAcq), _u64, _vp, _vp, _vp, _vp]),
     'vzgp_qacq_from_moments': (_i, [_vp, _i, _i, _i, _vp, _vp, C.POINTER(QAcq), _u64, _vp]),

@@ -1116,12 +1116,17 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
                           double* best_score, vzgp_handle* const* ens = nullptr, int n_ens = 0,
                           const vzgp_scalarization* scal = nullptr, const double* stack_alphas = nullptr,
                           const vzgp_pe_multi_params* pem = nullptr, vzgp_handle* const* sep = nullptr,
-                          int n_sep = 0, vzgp_handle* const* ens_b = nullptr) {
+                          int n_sep = 0, vzgp_handle* const* ens_b = nullptr, int stack_members = 1) {
   VZ_ARG(h && cfg && (acq || pe || scal || pem) && best_score, "handle / pointers");
   const AcqFn* fn = (pe || scal || pem) ? nullptr : handle_acq(ens ? ens[0] : h);   // multi-handle calls: the setting of hs[0]
   // GP-UCB-PE ensembles: ens = the E members of model A (h = ens[0]), ens_b those of model B (hB = ens_b[0])
+  // Stacks: ens = the handles of n_ens levels (stack_members each, level-major), h = the top level's (first) handle
   auto score_batch = [&](const double* xs, const int32_t* zs, int m, double* out) -> int {
     if (pe && ens_b) return launch_score_pe_ensemble(ens, ens_b, n_ens, xs, zs, m, pe, out, nullptr, nullptr, nullptr);
+    if (stack_alphas && scal) return launch_score_stack_multi(ens, n_ens, stack_alphas, xs, zs, m, out, nullptr, nullptr);
+    if (stack_alphas && stack_members > 1)
+      return launch_score_stack_ensemble(ens, n_ens, stack_members, stack_alphas, xs, zs, m, acq, out, nullptr, nullptr,
+                                         nullptr, fn);
     if (pem) return launch_score_pe_multi(h, hB, xs, zs, m, pem, out, nullptr, nullptr, nullptr);
     if (sep) return launch_score_separable(sep, n_sep, xs, zs, m, out, nullptr, nullptr);
     if (scal) return launch_score_multi(h, xs, zs, m, out, nullptr, nullptr);
@@ -1559,6 +1564,90 @@ int vzgp_eagle_run_stack(vzgp_handle* const* hs, int E, const double* alphas, co
   VZ_ARG(acq != nullptr, "acq");
   return eagle_run_impl(hs[E - 1], nullptr, cfg, acq, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
                         best_z, best_score, hs, E, nullptr, alphas);
+}
+
+// Stacks of uniform ensembles and of independent multi-metric levels: every handle fitted, on one device and stream,
+// with the same feature dimensions; the members of a level (hs[l * E .. l * E + E)) fitted on the same trials.
+static int check_stack_levels(vzgp_handle* const* hs, int L, int E, const double* alphas) {
+  VZ_ARG(hs != nullptr && alphas != nullptr, "handles / alphas");
+  VZ_ARG(L >= 1 && L <= kMaxStackLevels, "1 <= n_levels <= 16");
+  VZ_ARG(E >= 1 && E <= kMaxPeEnsemble, "1 <= E <= 8 members per level");
+  for (int k = 0; k < L * E; ++k) VZ_ARG(hs[k] != nullptr, "handle");
+  for (int k = 0; k < L * E; ++k) {
+    vzgp_handle* h = hs[k];
+    if (!h->fitted) { set_error("stacked scoring needs every member of every level fitted"); return VZGP_ERR_STATE; }
+    VZ_ARG(h->device == hs[0]->device && h->stream == hs[0]->stream, "levels must share device and stream");
+    VZ_ARG(h->dc == hs[0]->dc && h->dk == hs[0]->dk, "levels must have the same feature dimensions");
+    const vzgp_handle* first = hs[(k / E) * E];
+    VZ_ARG(h->n_valid == first->n_valid && h->np == first->np, "the members of a level must be fitted on the same trials");
+  }
+  for (int l = 1; l < L; ++l) VZ_ARG(alphas[l] >= 0.0 && alphas[l] <= 1.0, "0 <= alpha <= 1");
+  return 0;
+}
+
+static int check_stack_ensemble(vzgp_handle* const* hs, int L, int E, const double* alphas) {
+  VZ_TRY(check_stack_levels(hs, L, E, alphas));
+  for (int k = 0; k < L * E; ++k) VZ_ARG(hs[k]->n_metrics == 1, "stacked ensembles: single-metric members");
+  return 0;
+}
+
+static int check_stack_multi(vzgp_handle* const* hs, int L, const double* alphas, const vzgp_scalarization* sc) {
+  VZ_TRY(check_stack_levels(hs, L, 1, alphas));
+  VZ_ARG(sc != nullptr, "scalarization");
+  for (int l = 0; l < L; ++l) {
+    VZ_ARG(hs[l]->n_metrics >= 2 && hs[l]->n_metrics == hs[0]->n_metrics,
+           "stacked multi-metric levels: the same number of metrics (>= 2) on every level");
+    VZ_ARG(!hs[l]->kp.use_linear, "stacked multi-metric levels: no linear kernel");
+  }
+  return 0;
+}
+
+int vzgp_score_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, const double* alphas, const double* Xs,
+                              const int32_t* Zs, int M, const vzgp_acq* acq, double* score, double* mu, double* sigma,
+                              double* linf) {
+  VZ_TRY(check_stack_ensemble(hs, n_levels, E, alphas));
+  if (E == 1) return vzgp_score_stack(hs, n_levels, alphas, Xs, Zs, M, acq, score, mu, sigma, linf);
+  VZ_ARG(acq != nullptr, "acq");
+  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
+  VZ_ARG(M == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
+  VZ_ARG(M == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
+  Guard g(hs[0]->device);
+  return launch_score_stack_ensemble(hs, n_levels, E, alphas, Xs, Zs, M, acq, score, mu, sigma, linf,
+                                     handle_acq(hs[0]));
+}
+
+int vzgp_eagle_run_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, const double* alphas,
+                                  const vzgp_eagle_config* cfg, const vzgp_acq* acq, const double* prior,
+                                  const int32_t* prior_z, int n_prior, const int32_t* cat_sizes, int count,
+                                  uint64_t seed, double* best_x, int32_t* best_z, double* best_score) {
+  VZ_TRY(check_stack_ensemble(hs, n_levels, E, alphas));
+  if (E == 1)
+    return vzgp_eagle_run_stack(hs, n_levels, alphas, cfg, acq, prior, prior_z, n_prior, cat_sizes, count, seed,
+                                best_x, best_z, best_score);
+  VZ_ARG(acq != nullptr, "acq");
+  return eagle_run_impl(hs[(n_levels - 1) * E], nullptr, cfg, acq, nullptr, prior, prior_z, n_prior, cat_sizes, count,
+                        seed, best_x, best_z, best_score, hs, n_levels, nullptr, alphas, nullptr, nullptr, 0, nullptr, E);
+}
+
+int vzgp_score_stack_multi(vzgp_handle* const* hs, int n_levels, const double* alphas, const double* Xs,
+                           const int32_t* Zs, int M, const vzgp_scalarization* sc, double* score, double* mu,
+                           double* sigma) {
+  VZ_TRY(check_stack_multi(hs, n_levels, alphas, sc));
+  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
+  VZ_ARG(M == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
+  VZ_ARG(M == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
+  Guard g(hs[0]->device);
+  VZ_TRY(prepare_scalarization(hs[n_levels - 1], sc));
+  return launch_score_stack_multi(hs, n_levels, alphas, Xs, Zs, M, score, mu, sigma);
+}
+
+int vzgp_eagle_run_stack_multi(vzgp_handle* const* hs, int n_levels, const double* alphas, const vzgp_eagle_config* cfg,
+                               const vzgp_scalarization* sc, const double* prior, const int32_t* prior_z, int n_prior,
+                               const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
+                               double* best_score) {
+  VZ_TRY(check_stack_multi(hs, n_levels, alphas, sc));
+  return eagle_run_impl(hs[n_levels - 1], nullptr, cfg, nullptr, nullptr, prior, prior_z, n_prior, cat_sizes, count,
+                        seed, best_x, best_z, best_score, hs, n_levels, sc, alphas);
 }
 
 // The graph-batched evaluation behind vzgp_nll_grad_batch and vzgp_nll_grad_separable_batch: branch r evaluates

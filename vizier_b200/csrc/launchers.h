@@ -118,6 +118,14 @@ int launch_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, i
 int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const double* Xs, const int32_t* Zs, int M,
                        const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf,
                        const AcqFn* fn = nullptr);
+// Stacks whose levels are uniform ensembles of E members (hs[l * E + e], score.cu) or independent multi-metric GPs
+// scored with the scalarisation prepared on the top level (multi.cu).
+constexpr int kMaxStackLevels = 16;
+int launch_score_stack_ensemble(vzgp_handle* const* hs, int L, int E, const double* alphas, const double* Xs,
+                                const int32_t* Zs, int M, const vzgp_acq* acq, double* score, double* mu, double* sigma,
+                                double* linf, const AcqFn* fn = nullptr);
+int launch_score_stack_multi(vzgp_handle* const* hs, int L, const double* alphas, const double* Xs, const int32_t* Zs,
+                             int M, double* score, double* mu, double* sigma);
 int launch_set_pe_combine(vzgp_handle* h, int n_sets, int q, const vzgp_pe_params* pe, const double* cov, int ldc,
                           const double* mu_a, const double* sd_a, const double* linf, double* score, double* sd_all);
 // General scoring path (score.cu): explicit K* and W = K* Linv^T of at most kGeneralChunk candidates at a time, in the

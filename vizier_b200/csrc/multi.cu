@@ -234,6 +234,84 @@ int launch_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int 
   return 0;
 }
 
+// Stacked residual GPs of independent multi-task levels (transfer learning with several metrics): every level has one
+// factor, so its stddev is shared by the metrics, and one alpha per metric.  mean_m = sum_l mu_l,m; the stddevs are
+// stacked bottom-up as in k_stack_combine, s <- sd_l^alpha_l * s^(1 - alpha_l); then u_m = mean_m + c s and the
+// floored HV scalarisation of k_scalarize, without a trust region (gp_bandit.py:242).
+// mu: [L][n_metrics][M], sd: [L][M]; mu_out optional [n_metrics][M], sigma_out optional [M].
+struct StackMultiCombine {
+  int L;
+  double alpha[kMaxStackLevels];
+};
+__global__ void __launch_bounds__(256) k_stack_multi_combine(int M, StackMultiCombine p, ScalArgs a,
+                                                             const double* __restrict__ mu,
+                                                             const double* __restrict__ sd,
+                                                             const double* __restrict__ weights_inv,
+                                                             const double* __restrict__ best,
+                                                             double* __restrict__ score, double* __restrict__ mu_out,
+                                                             double* __restrict__ sigma_out) {
+  extern __shared__ double sw[];
+  const int nm = a.n_metrics;
+  stage_scalarization(a, weights_inv, best, sw);
+  __syncthreads();
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= M) return;
+  const size_t level = (size_t)nm * M;
+  double mean[kMaxMetrics];
+#pragma unroll
+  for (int m = 0; m < kMaxMetrics; ++m) mean[m] = (m < nm) ? mu[(size_t)m * M + c] : 0.0;
+  double s = sd[c];
+  for (int l = 1; l < p.L; ++l) {
+#pragma unroll
+    for (int m = 0; m < kMaxMetrics; ++m)
+      if (m < nm) mean[m] += mu[l * level + (size_t)m * M + c];
+    s = pow(sd[(size_t)l * M + c], p.alpha[l]) * pow(s, 1.0 - p.alpha[l]);
+  }
+  double u[kMaxMetrics];
+#pragma unroll
+  for (int m = 0; m < kMaxMetrics; ++m) {
+    u[m] = (m < nm) ? fmax(fma(a.coef, s, mean[m]) - a.ref[m], 0.0) : 0.0;
+    if (m < nm && mu_out) mu_out[(size_t)m * M + c] = mean[m];
+  }
+  score[c] = scalarized_mean(a, u, sw);
+  if (sigma_out) sigma_out[c] = s;
+}
+
+// hs[0 .. L): one multi-metric handle per level, the scalarisation prepared on the top one (prepare_scalarization).
+// Per level the stddev (launch_score, UCB-0 request) and the per-metric means (k_mean_multi), then
+// k_stack_multi_combine.  The pieces live in the top handle's pe_tmp: [L n_metrics + L + 1][M] = mu | sd | dummy.
+// Asynchronous, capturable.
+int launch_score_stack_multi(vzgp_handle* const* hs, int L, const double* alphas, const double* Xs, const int32_t* Zs,
+                             int M, double* score, double* mu_out, double* sigma_out) {
+  if (M <= 0) return 0;
+  vzgp_handle* top = hs[L - 1];
+  const ScalArgs& a = top->scal_args;
+  const int nm = top->n_metrics, S = a.n_scal;
+  if (a.n_metrics != nm || S < 1) { set_error("stacked multi-metric scoring without a prepared scalarization"); return VZGP_ERR_STATE; }
+  VZ_TRY(top->pe_tmp.reserve(sizeof(double) * ((size_t)L * nm + L + 1) * (size_t)M));
+  double* mu = top->pe_tmp.as<double>();
+  double* sd = mu + (size_t)L * nm * M;
+  double* dummy = sd + (size_t)L * M;
+  const vzgp_acq none = posterior_request();
+  for (int l = 0; l < L; ++l) {
+    VZ_TRY(launch_score(hs[l], Xs, Zs, M, &none, dummy, nullptr, sd + (size_t)l * M, nullptr));
+    VZ_TRY(launch_mean_multi(hs[l], Xs, Zs, M, mu + (size_t)l * nm * M));
+    hs[l]->launches++;
+  }
+  StackMultiCombine p;
+  p.L = L;
+  for (int l = 0; l < kMaxStackLevels; ++l) p.alpha[l] = l < L ? alphas[l] : 0.0;
+  const size_t wn = (size_t)S * nm;
+  const size_t sm = sizeof(double) * (wn + S);
+  VZ_TRY(raise_dyn_smem((const void*)k_stack_multi_combine, sm));
+  k_stack_multi_combine<<<(M + 255) / 256, 256, sm, top->stream>>>(M, p, a, mu, sd, top->scal.as<double>(),
+                                                                   top->scal.as<double>() + wn, score, mu_out,
+                                                                   sigma_out);
+  VZ_CHECK_LAUNCH();
+  top->launches++;
+  return 0;
+}
+
 // Multi-metric GP-UCB-PE, mode 0: uploads the scalarisation of `pe` to hA (synchronises, not capturable).  Mode 1
 // carries everything it needs in the kernel arguments.  Call once before a loop of launch_score_pe_multi.
 int prepare_score_pe_multi(vzgp_handle* hA, const vzgp_pe_multi_params* pe) {

@@ -1051,6 +1051,72 @@ int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, cons
 }
 
 // ---------------------------------------------------------------------------
+// Stacked levels of uniform ensembles (VizierGPBandit(ensemble_size=E).set_priors: every level of the stack is trained
+// with the designer's spec, gp_bandit.py:402-447).  Per candidate, each level's prediction is the two-pass mixture of
+// its E members (pe_mixture), then the stack of k_stack_combine over the level mixtures: mean = sum of the level
+// means, s <- sd_l^alpha_l * s^(1 - alpha_l) bottom-up.  The acquisition and the non-strict trust region (distances to
+// the top level's trials) follow.  mu_e / sd_e: [L][E][M], level-major like the handles.
+// ---------------------------------------------------------------------------
+struct StackEnsCombine {
+  int L, E;
+  double alpha[kMaxStackLevels];
+  AcqFn acq;
+  TrustRegion tr;
+};
+__global__ void __launch_bounds__(256) k_stack_ensemble_combine(int M, StackEnsCombine p,
+                                                                const double* __restrict__ mu_e,
+                                                                const double* __restrict__ sd_e,
+                                                                const double* __restrict__ linf,
+                                                                double* __restrict__ score, double* __restrict__ mu,
+                                                                double* __restrict__ sigma) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  const size_t level = (size_t)p.E * M;
+  double mean, sd;
+  pe_mixture(p.E, mu_e, sd_e, (size_t)M, m, mean, sd);
+  for (int l = 1; l < p.L; ++l) {
+    double mean_l, sd_l;
+    pe_mixture(p.E, mu_e + l * level, sd_e + l * level, (size_t)M, m, mean_l, sd_l);
+    mean += mean_l;
+    sd = pow(sd_l, p.alpha[l]) * pow(sd, 1.0 - p.alpha[l]);
+  }
+  score[m] = tr_apply(p.tr, acq_value(p.acq, mean, sd), linf[m]);
+  if (mu) mu[m] = mean;
+  if (sigma) sigma[m] = sd;
+}
+
+// hs[l * E + e] = member e of level l.  Every member is scored by launch_score on its own route (mean and stddev);
+// top-level member 0 also gives the trust-region distance (the members of a level share its trials).  The pieces
+// live in the top handle's pe_tmp, which launch_score does not touch: [2 L E + 2][M] = mu | sd (L E rows each) |
+// linf | dummy.  Asynchronous, capturable.
+int launch_score_stack_ensemble(vzgp_handle* const* hs, int L, int E, const double* alphas, const double* Xs,
+                                const int32_t* Zs, int M, const vzgp_acq* acq, double* score, double* mu, double* sigma,
+                                double* linf, const AcqFn* fn) {
+  if (M <= 0) return 0;
+  const int n = L * E;
+  vzgp_handle* top = hs[(L - 1) * E];
+  VZ_TRY(top->pe_tmp.reserve(sizeof(double) * (2 * (size_t)n + 2) * (size_t)M));
+  double* t = top->pe_tmp.as<double>();
+  double* mu_e = t;
+  double* sd_e = t + (size_t)n * M;
+  double* linf_buf = linf ? linf : t + 2 * (size_t)n * M;
+  double* dummy = t + (2 * (size_t)n + 1) * M;
+  StackEnsCombine p;
+  p.L = L; p.E = E; p.acq = acq_fn_of(acq, fn);
+  p.tr = trust_region_of(top, *acq, acq->tr_strict);
+  const bool want_linf = tr_needs_distance(p.tr) || linf != nullptr;
+  const vzgp_acq none = posterior_request(acq->tr_dim_mask, acq->tr_rows);
+  for (int k = 0; k < n; ++k)
+    VZ_TRY(launch_score(hs[k], Xs, Zs, M, &none, dummy, mu_e + (size_t)k * M, sd_e + (size_t)k * M,
+                        (k == (L - 1) * E && want_linf) ? linf_buf : nullptr));
+  for (int l = 0; l < kMaxStackLevels; ++l) p.alpha[l] = l < L ? alphas[l] : 0.0;
+  k_stack_ensemble_combine<<<(M + 255) / 256, 256, 0, top->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma);
+  VZ_CHECK_LAUNCH();
+  top->launches++;
+  return 0;
+}
+
+// ---------------------------------------------------------------------------
 // Set-PE acquisition (SetPEScoreFunction, gp_ucb_pe.py:510-594): per set of q points
 //   logdet(joint predictive covariance under model B)  +  penalty * sum_i min(mean_A + explore * stddev_A - threshold, 0)
 //   [+ sum_i tr_set_term(dist_i) when radius <= 0.5                        _apply_trust_region_to_set, :245-269]

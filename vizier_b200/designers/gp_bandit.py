@@ -20,6 +20,11 @@ task_kernels.py), scored, optimised and sampled the same way.
 (general launch sequences: no captured graph, explicit K* for the scoring).
 `set_priors` trains a stack of residual GPs, one level per prior study plus the current study on top (gp_bandit.py:289-318;
 gp/gp_models.py:91-140, :245-300; gp/transfer_learning.py), scored through `vzgp_score_stack` (`gp.StackedGP`).
+Every level is trained with the designer's own spec (gp_bandit.py:402-447): with `ensemble_size > 1` each level is a
+uniform mixture of its E best restarts (`vzgp_score_stack_ensemble`), `linear_coef` applies to every level, and a
+multi-metric problem stacks independent multi-task levels on [N, M] residuals, scored by the scalarised UCB
+(`vzgp_score_stack_multi`).  Separable multi-task types and parallel scoring functions with priors raise
+NotImplementedError.
 `scoring_function_factory` (e.g. `acquisitions.bayesian_scoring_function_factory(lambda d: EI(get_best_labels(d.labels)))`
 or `AcquisitionTrustRegion.default_ucb_pi`) selects UCB, LCB, EI, PI or a thresholded pair of those; the device
 scoring kernels evaluate it (`acquisitions.lower_acquisition`).  Multi-metric problems keep their scalarised UCB.
@@ -28,7 +33,7 @@ scoring kernels evaluate it (`acquisitions.lower_acquisition`).  Multi-metric pr
 (csrc/score_q.cu) inside the n_parallel Eagle loop or the random strategy (`optimizers.optimize_qsets`).
 Not implemented (the reference supports them; SURVEY 8f "next"): parallel acquisitions for multi-metric models or
 with priors, other acquisition
-functions (MaxValueEntropySearch, Sample, user callables), priors for multi-metric or ensemble models; each raises NotImplementedError
+functions (MaxValueEntropySearch, Sample, user callables), priors for separable multi-task models; each raises NotImplementedError
 instead of silently doing something else.  Categorical parameters ARE supported
 end to end.  `padding_schedule` is accepted and has no numerical effect here: the kernels take
 explicit sizes (`n_valid`, Dc, Dk) instead of padded shapes + masks, which is what the reference's
@@ -189,9 +194,11 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     labels, each further one on the residuals of its study against the stack below (gp/gp_models.py:245-300).  The
     current study's GP is later trained on ITS residuals against the whole prior stack (`_update_gp`).  Each call
     retrains the prior stack from scratch on what it is given."""
-    if self._n_metrics != 1 or self._ensemble_size != 1 or self._linear_coef or self._parallel:
-      raise NotImplementedError('transfer-learning priors: single-metric, single-model Matern GPs with pointwise '
-                                'acquisitions only.')
+    if self._parallel:
+      raise NotImplementedError('transfer-learning priors with parallel (q-) scoring functions are not implemented.')
+    if self._multitask_type:
+      raise NotImplementedError(f'transfer-learning priors with the separable multi-task type {self._multitask_type} '
+                                'are not implemented.')
     if self._stack is not None:
       self._stack.close()
     self._stack = gp.StackedGP(self._device_index)
@@ -201,7 +208,7 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
         continue
       (cont, cat), labels = self._converter.to_xy(trials)
       labels = self._warp_labels(labels)
-      self._push_level(cont, cat, labels[:, 0])
+      self._push_level(cont, cat, labels[:, 0] if self._n_metrics == 1 else labels)
     self._n_prior_levels = len(self._stack.levels)
     if self._n_prior_levels == 0:
       self._stack = None
@@ -209,16 +216,22 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     self._incorporated_trials_count = -1
 
   def _push_level(self, cont, cat, y):
-    """Trains one more level of the stack on the residuals of (cont, cat, y) against the levels below."""
+    """Trains one more level of the stack on the residuals of (cont, cat, y) against the levels below, with the
+    designer's model spec (gp_bandit.py:402-447): the `ensemble_size` best ARD restarts, `linear_coef`, and labels
+    y [N] or [N, n_metrics] (one residual column per metric).  Returns the level's hyper-parameters (a list of them for
+    an ensemble)."""
     z = cat if cat.shape[1] else None
-    resid = y - self._stack.mean(cont, z)
-    level = self._stack.new_level()
+    resid = y - self._stack.mean(cont, z) if self._stack.levels else y
+    level = self._stack.new_level(self._ensemble_size)
+    ard_dev = level.members[0] if self._ensemble_size > 1 else level
     ard_rng = np.random.default_rng(int(self._rng.integers(2**62)))
-    best, _ = ard.train_gp(level, cont, resid, z, rng=ard_rng, random_restarts=self._ard_random_restarts,
-                           ensemble_size=1, optimizer=self._ard_optimizer)
-    level.fit(cont, resid, best[0], z=z)
+    best, _ = ard.train_gp(ard_dev, cont, resid, z, rng=ard_rng, random_restarts=self._ard_random_restarts,
+                           ensemble_size=self._ensemble_size, optimizer=self._ard_optimizer,
+                           linear_coef=self._linear_coef)
+    params = list(best) if self._ensemble_size > 1 else best[0]
+    level.fit(cont, resid, params, z=z)
     self._stack.push(level, cont.shape[0])
-    return best[0]
+    return params
 
   @classmethod
   def from_problem(cls, problem, seed: Optional[int] = None, **kwargs) -> 'VizierGPBandit':
@@ -273,7 +286,7 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
         return self._stack
       self._incorporated_trials_count = len(self._trials)
       self._stack.truncate(self._n_prior_levels)
-      self._last_params = self._push_level(cont, cat, labels[:, 0])
+      self._last_params = self._push_level(cont, cat, labels[:, 0] if self._n_metrics == 1 else labels)
       return self._stack
     dev = self._device()
     if len(self._trials) == self._incorporated_trials_count and self._last_params is not None:
@@ -397,6 +410,8 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     xs = np.nan_to_num(xs, nan=0.0)
     g = np.random.default_rng(_seed_from(rng) if rng is not None else 0)
     zq = zs if zs.shape[1] else None
+    if self._n_metrics > 1 and self._stack is not None:
+      return self._sample_stack_multi(dev, xs, zq, g, num_samples)
     if self._n_metrics > 1:
       return self._sample_multi(dev, xs, zq, g, num_samples)
     if self._stack is not None:
@@ -425,6 +440,16 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
       warped = mean[m][None, :] + z @ chol.T
       out[:, :, m] = self._output_warper.unwarp(warped.reshape(-1, 1)).reshape(num_samples, -1)
     return out
+
+  def _sample_stack_multi(self, stack, xs, zq, g, num_samples: int) -> np.ndarray:
+    """Stack of multi-metric levels: the combined prediction is a diagonal normal per metric (gp/transfer_learning.py:
+    150-152) with the stddev shared by the metrics.  Returns unwarped samples [num_samples, num_trials, num_metrics]."""
+    mean, sd = stack.predict(xs, zq)                            # [n, M], [n]
+    res = np.empty((num_samples, mean.shape[0], self._n_metrics))
+    for m in range(self._n_metrics):
+      warped = mean[:, m][None, :] + g.standard_normal((num_samples, mean.shape[0])) * sd[None, :]
+      res[:, :, m] = self._output_warper.unwarp(warped.reshape(-1, 1)).reshape(num_samples, -1)
+    return res
 
   @profiler.record_runtime
   def predict(self, trials: Sequence[Any], rng: Any = None, num_samples: Optional[int] = 1000):

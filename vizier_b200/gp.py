@@ -965,11 +965,16 @@ class StackedGP:
   gp/gp_models.py:91-140, :245-300): level 0 is fitted on the first prior study, each further level on the residuals
   of the next study against the stack below it, the last level on the current study.  The levels are libvzgp handles
   on ONE stream; scoring and the Eagle loop run through `vzgp_score_stack` / `vzgp_eagle_run_stack`.  Exposes the
-  subset of the `DeviceGP` interface the acquisition optimiser drives."""
+  subset of the `DeviceGP` interface the acquisition optimiser drives.
+
+  Every level has the same kind, the designer's model spec: a single-metric `DeviceGP` (the calls above), an
+  `EnsembleGP` of E members (each level's prediction is the two-pass mixture of its members;
+  `vzgp_score_stack_ensemble` / `vzgp_eagle_run_stack_ensemble`) or a multi-metric `DeviceGP` (independent multi-task
+  levels scored by the scalarised UCB; `vzgp_score_stack_multi` / `vzgp_eagle_run_stack_multi`)."""
 
   def __init__(self, device: int):
     self._device_index = device
-    self.levels: list = []          # DeviceGP per level, base first
+    self.levels: list = []          # DeviceGP or EnsembleGP per level, base first
     self.counts: list = []          # training points per level
     self.alphas: list = []          # alphas[e]: weight of level e's stddev against the stack below (alphas[0] unused)
     self.device = None
@@ -978,6 +983,44 @@ class StackedGP:
   @property
   def top(self) -> 'DeviceGP':
     return self.levels[-1]
+
+  @staticmethod
+  def _members(level) -> list:
+    return level.members if isinstance(level, EnsembleGP) else [level]
+
+  @staticmethod
+  def _kind(level) -> tuple:
+    """(members per level, metrics per level)."""
+    members = StackedGP._members(level)
+    return len(members), int(getattr(members[0], 'n_metrics', 1))
+
+  @property
+  def ensemble_size(self) -> int:
+    return self._kind(self.levels[0])[0] if self.levels else 1
+
+  @property
+  def n_metrics(self) -> int:
+    return self._kind(self.levels[0])[1] if self.levels else 1
+
+  def _lead(self) -> 'DeviceGP':
+    """The top level's (first) handle: it owns the Eagle state and the scratch of the combine."""
+    return self._members(self.levels[-1])[0]
+
+  # the lead handle carries the state of the host-stepped Eagle loop (SteppedEagle drives these)
+  @property
+  def _h(self):
+    return self._lead()._h
+
+  @property
+  def _lib(self):
+    return self._lead()._lib
+
+  @property
+  def _stream(self):
+    return self._lead()._stream
+
+  def _dev(self, a, dtype):
+    return self._lead()._dev(a, dtype)
 
   @property
   def stream(self):
@@ -1001,22 +1044,43 @@ class StackedGP:
       m.close()
     del self.levels[n_levels:], self.counts[n_levels:], self.alphas[n_levels:]
 
-  def new_level(self) -> 'DeviceGP':
-    m = DeviceGP(self._device_index) if not self.levels else DeviceGP(self._device_index, stream=self.levels[0].stream)
+  def new_level(self, ensemble_size: int = 1):
+    """A new (unfitted) level on the stack's stream: a DeviceGP, or an EnsembleGP of `ensemble_size` members."""
+    stream = self.levels[0].stream if self.levels else None
+    if ensemble_size > 1:
+      return EnsembleGP(self._device_index, ensemble_size, stream=stream)
+    m = DeviceGP(self._device_index) if not self.levels else DeviceGP(self._device_index, stream=stream)
     return m
 
   def mean(self, xs, zs=None) -> np.ndarray:
-    """Mean of the stack built so far at xs (0 for an empty stack): the quantity the next level's labels are reduced by
-    (`_pred_mean`, gp/gp_models.py:268-283)."""
+    """Mean of the stack built so far at xs (0 for an empty stack), [N] or [N, n_metrics]: the quantity the next
+    level's labels are reduced by (`_pred_mean`, gp/gp_models.py:268-283)."""
     n = len(xs)
     if not self.levels:
       return np.zeros(n)
+    return self.predict(xs, zs)[0]
+
+  def predict(self, xs, zs=None):
+    """Combined prediction of the stack at xs (host arrays): mean [N] or [N, n_metrics], stddev [N] (shared by the
+    metrics of multi-metric levels)."""
+    if self.n_metrics > 1:
+      nm = self.n_metrics
+      # mean and stddev do not depend on the scalarisation: any valid one will do
+      sc = ScalarizedUcbAcquisition(np.full((1, nm), 1.0 / np.sqrt(nm)), np.zeros(nm), None, 0.0)
+      out = self.score_multi(xs, sc, zs=zs, with_aux=True)
+      self.synchronize()
+      return out['mean'].cpu().numpy().T, out['stddev'].cpu().numpy()
     out = self.score(xs, Acquisition(0.0, False, 1.0), zs=zs, with_aux=True)
     self.synchronize()
-    return out['mean'].cpu().numpy()
+    return out['mean'].cpu().numpy(), out['stddev'].cpu().numpy()
 
-  def push(self, level: 'DeviceGP', n_points: int) -> None:
-    """Adds a fitted level on top of the stack."""
+  def push(self, level, n_points: int) -> None:
+    """Adds a fitted level on top of the stack (of the same kind as the levels below)."""
+    if self.levels and self._kind(level) != self._kind(self.levels[0]):
+      raise ValueError(f'every level of a stack has the same kind: (members, metrics) {self._kind(level)} on top of '
+                       f'{self._kind(self.levels[0])}')
+    if self._kind(level)[0] > 1 and self._kind(level)[1] > 1:
+      raise NotImplementedError('stacks of multi-metric ensembles are not implemented.')
     h = level.dc + level.dk + 2           # GPState.num_hyperparameters (gp/gp_models.py:77-88)
     self.alphas.append(0.0 if not self.levels else transfer_alpha(n_points, self.counts[-1], h))
     self.levels.append(level)
@@ -1024,13 +1088,14 @@ class StackedGP:
     self.device, self.dc, self.dk, self.n = level.device, level.dc, level.dk, level.n
 
   def _handles(self):
-    return (C.c_void_p * len(self.levels))(*[m._h for m in self.levels])
+    hs = [m._h for level in self.levels for m in self._members(level)]   # level-major: hs[l * E + e]
+    return (C.c_void_p * len(hs))(*hs)
 
   def _alphas(self):
     return (C.c_double * len(self.levels))(*self.alphas)
 
   def score(self, xs, acq: Acquisition, zs=None, with_aux: bool = False) -> dict:
-    f = self.levels[-1]
+    f = self._lead()
     xst, zst = f._xz(xs, zs)
     m = xst.shape[0]
     res = {'score': torch.empty((m,), dtype=torch.float64, device=f.device)}
@@ -1038,19 +1103,54 @@ class StackedGP:
       for k in ('mean', 'stddev', 'linf_distance'):
         res[k] = torch.empty((m,), dtype=torch.float64, device=f.device)
     f._stream.wait_stream(torch.cuda.current_stream(f.device))
-    self.levels[0]._use_acq(acq)          # multi-handle calls take the acquisition of hs[0]
+    self._members(self.levels[0])[0]._use_acq(acq)          # multi-handle calls take the acquisition of hs[0]
     a, keep = acq._c()
-    _lib.check('vzgp_score_stack', f._lib.vzgp_score_stack(
-        self._handles(), len(self.levels), self._alphas(), _ptr(xst), _ptr(zst), m, C.byref(a), _ptr(res['score']),
-        _ptr(res.get('mean')), _ptr(res.get('stddev')), _ptr(res.get('linf_distance'))))
+    outs = (_ptr(res['score']), _ptr(res.get('mean')), _ptr(res.get('stddev')), _ptr(res.get('linf_distance')))
+    if self.ensemble_size == 1:
+      _lib.check('vzgp_score_stack', f._lib.vzgp_score_stack(
+          self._handles(), len(self.levels), self._alphas(), _ptr(xst), _ptr(zst), m, C.byref(a), *outs))
+    else:
+      _lib.check('vzgp_score_stack_ensemble', f._lib.vzgp_score_stack_ensemble(
+          self._handles(), len(self.levels), self.ensemble_size, self._alphas(), _ptr(xst), _ptr(zst), m, C.byref(a),
+          *outs))
     res['_inputs'] = (xst, zst, keep)
     return res
 
-  def eagle_run(self, cfg, acq: Acquisition, count: int, seed: int, prior=None, prior_z=None, cat_sizes=None, other=None):
+  def score_multi(self, xs, acq: ScalarizedUcbAcquisition, zs=None, with_aux: bool = False) -> dict:
+    """Scalarised UCB of a stack of multi-metric levels; returns device tensors {'score' [M], ['mean' [n_metrics, M],
+    'stddev' [M]]}."""
+    f = self._lead()
+    xst, zst = f._xz(xs, zs)
+    m = xst.shape[0]
+    res = {'score': torch.empty((m,), dtype=torch.float64, device=f.device)}
+    if with_aux:
+      res['mean'] = torch.empty((self.n_metrics, m), dtype=torch.float64, device=f.device)
+      res['stddev'] = torch.empty((m,), dtype=torch.float64, device=f.device)
+    f._stream.wait_stream(torch.cuda.current_stream(f.device))
+    sc, keep = acq._c()
+    _lib.check('vzgp_score_stack_multi', f._lib.vzgp_score_stack_multi(
+        self._handles(), len(self.levels), self._alphas(), _ptr(xst), _ptr(zst), m, C.byref(sc), _ptr(res['score']),
+        _ptr(res.get('mean')), _ptr(res.get('stddev'))))
+    res['_inputs'] = (xst, zst, keep)
+    return res
+
+  def eagle_run(self, cfg, acq, count: int, seed: int, prior=None, prior_z=None, cat_sizes=None, other=None):
+    """The device Eagle loop on the stacked acquisition: `Acquisition` (single-metric levels) or
+    `ScalarizedUcbAcquisition` (multi-metric levels)."""
     assert other is None
-    f = self.levels[-1]
-    self.levels[0]._use_acq(acq)
-    a, keep = acq._c()
+    f = self._lead()
+    if isinstance(acq, ScalarizedUcbAcquisition):
+      a, keep = acq._c()
+      fn, args = 'vzgp_eagle_run_stack_multi', (self._handles(), len(self.levels), self._alphas(), C.byref(cfg),
+                                                C.byref(a))
+    else:
+      self._members(self.levels[0])[0]._use_acq(acq)
+      a, keep = acq._c()
+      if self.ensemble_size == 1:
+        fn, args = 'vzgp_eagle_run_stack', (self._handles(), len(self.levels), self._alphas(), C.byref(cfg), C.byref(a))
+      else:
+        fn, args = 'vzgp_eagle_run_stack_ensemble', (self._handles(), len(self.levels), self.ensemble_size,
+                                                     self._alphas(), C.byref(cfg), C.byref(a))
     n_prior = 0 if prior is None else len(prior)
     pt = f._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
     pz = f._dev(prior_z, torch.int32) if n_prior > 0 and self.dk > 0 else None
@@ -1058,17 +1158,16 @@ class StackedGP:
     bz = np.zeros((count, self.dk), np.int32)
     bs = np.zeros(count, np.float64)
     sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
-    _lib.check('vzgp_eagle_run_stack', f._lib.vzgp_eagle_run_stack(
-        self._handles(), len(self.levels), self._alphas(), C.byref(cfg), C.byref(a), _ptr(pt), _ptr(pz), n_prior,
-        sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None, count, seed,
-        bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
+    _lib.check(fn, getattr(f._lib, fn)(
+        *args, _ptr(pt), _ptr(pz), n_prior, sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None,
+        count, seed, bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
         bs.ctypes.data_as(C.POINTER(C.c_double))))
     del keep
     return bx, bz, bs
 
   def random_search(self, m: int, acq: Acquisition, count: int, seed: int, index_base: int = 0, cat_sizes=None):
     """RandomVectorizedStrategy over the stack: Philox pool -> combined score -> device top-k."""
-    f = self.levels[-1]
+    f = self._lead()
     xs = f.random_pool(m, self.dc, seed, index_base) if self.dc else torch.zeros((m, 0), dtype=torch.float64, device=f.device)
     zs = f.random_pool_cat(m, cat_sizes, seed, index_base) if self.dk else None
     out = self.score(xs, acq, zs=zs)
@@ -1078,8 +1177,14 @@ class StackedGP:
     bz = zs[it].cpu().numpy() if zs is not None else np.zeros((count, 0), np.int32)
     return bx, bz, val, idx + index_base
 
+  def random_pool(self, m: int, dc: int, seed: int, index_base: int = 0) -> torch.Tensor:
+    return self._lead().random_pool(m, dc, seed, index_base)
+
+  def random_pool_cat(self, m: int, cat_sizes, seed: int, index_base: int = 0) -> torch.Tensor:
+    return self._lead().random_pool_cat(m, cat_sizes, seed, index_base)
+
   def topk(self, score, count: int):
-    return self.levels[-1].topk(score, count)
+    return self._lead().topk(score, count)
 
 
 class _DevView:
