@@ -543,7 +543,7 @@ int vzgp_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int3
  * (members summed in index order: repeated calls are bit-identical), and the acquisition is vzgp_score_pe's on the
  * mixtures: UCB = mean_A + c sigma_B, PE = sigma_B + p min(mean_A + e sigma_A - threshold, 0), then the strict trust
  * region against the first tr_rows trials of hBs[0].  mu / sigma (mixture of A) and sigma_all (mixture of B) are
- * optional device outputs [M].  E = 1 computes what vzgp_score_pe computes. */
+ * optional device outputs [M].  E = 1 computes what vzgp_score_pe computes (vzgp_score_pe is this scorer at E = 1). */
 int vzgp_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const double* Xs, const int32_t* Zs,
                            int M, const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all);
 /* vzgp_eagle_run with vzgp_score_pe_ensemble as the scoring function.  Forms (vzgp_get_int "eagle_route" on hAs[0]):
@@ -573,11 +573,12 @@ int vzgp_eagle_run_stack(vzgp_handle* const* hs, int E, const double* alphas, co
  * vzgp_score_pe_ensemble), and the levels are stacked as in vzgp_score_stack: mean = sum_l mean_l, s = sd_l^alphas[l] *
  * s^(1 - alphas[l]) bottom-up.  The acquisition (vzgp_set_acquisition of hs[0]) and the trust region follow, the trust
  * region measured against the trials of the top level's member 0, hs[(n_levels - 1) * E], which also computes linf.
- * mu / sigma / linf are optional device outputs [M].  E = 1 calls vzgp_score_stack (bit-identical results). */
+ * mu / sigma / linf are optional device outputs [M].  E = 1 computes what vzgp_score_stack computes (vzgp_score_stack
+ * is this scorer at E = 1, without the single-metric requirement). */
 int vzgp_score_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, const double* alphas, const double* Xs,
                               const int32_t* Zs, int M, const vzgp_acq* acq, double* score, double* mu, double* sigma,
                               double* linf);
-/* vzgp_eagle_run with vzgp_score_stack_ensemble as the scoring function; E = 1 calls vzgp_eagle_run_stack.  The loop
+/* vzgp_eagle_run with vzgp_score_stack_ensemble as the scoring function (E = 1: vzgp_eagle_run_stack).  The loop
  * runs as the replayed graph (the persistent and cooperative forms evaluate single models only); "eagle_route" is
  * recorded on hs[(n_levels - 1) * E]. */
 int vzgp_eagle_run_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, const double* alphas,

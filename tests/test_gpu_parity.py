@@ -290,7 +290,7 @@ def test_random_search_matches_oracle(dev):
 
 # The last two rows are BASELINE C3's shape (P = B = 1000 fireflies, N = 1000 trials, D = 20) and a
 # batch-600 case: batches above 512 take the replayed CUDA-graph form of the loop (c_abi.cu,
-# eagle_run_impl) with k_eagle_suggest / k_eagle_update at 1000 flies and the large-pool k_score.  The form each row
+# eagle_run_impl over the Model descriptor) with k_eagle_suggest / k_eagle_update at 1000 flies and the large-pool k_score.  The form each row
 # takes is asserted.  At every size here the trust radius is above 0.5 (the region is off) and no fly is visited often
 # enough to be trimmed: tests/test_gpu_eagle_steps.py covers the active region, trimming, ties and non-finite rewards.
 @pytest.mark.parametrize('n,d,pool,batch,steps', [(30, 4, 25, 25, 6), (60, 5, 20, 5, 14), (130, 3, 50, 25, 7),

@@ -41,7 +41,7 @@ def _kernel_split(fn):
   for ev in prof.key_averages():
     if ev.device_type is not None and 'CUDA' in str(ev.device_type) and ev.count > 0:
       name = ev.key
-      for k in ('k_score_finalize', 'k_score', 'k_mean_multi', 'k_pe_multi_combine', 'k_pe_combine'):
+      for k in ('k_score_finalize', 'k_score', 'k_mean_multi', 'k_pe_multi_combine'):
         if k in name:
           name = k
           break

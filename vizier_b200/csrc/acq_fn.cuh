@@ -1,8 +1,8 @@
 // Pointwise acquisition functions of the posterior (mean, stddev) at one candidate: UCB, LCB, EI, PI and the
 // thresholded pair of AcquisitionTrustRegion (vizier/_src/algorithms/designers/gp/acquisitions.py:213-274,
 // :390-492), and the L-inf trust region applied after them.  Every pointwise scoring epilogue (emit_score,
-// k_general_finalize, k_stack_combine, k_ensemble_combine, score_batch64) evaluates acq_value on its final
-// (mean, stddev); those and the GP-UCB-PE combines (k_pe_combine, k_pe_multi_combine, score_batch64, k_eagle_grid)
+// k_general_finalize, k_stack_ensemble_combine, k_ensemble_combine, score_batch64) evaluates acq_value on its final
+// (mean, stddev); those and the GP-UCB-PE combines (k_pe_ensemble_combine, k_pe_multi_combine, score_batch64, k_eagle_grid)
 // then call tr_apply.  The set scorers (k_set_pe_combine, k_qacq_mc) add tr_set_term per point instead.
 #pragma once
 #include <cuda_runtime.h>

@@ -521,15 +521,47 @@ static int shared_shift(int m, int* k, F eval) {
   }
 }
 
+// What the handles of one group of a multi-handle model share besides the feature dimensions.
+enum class Trials { kAny, kSameNValid, kSameFit };   // kSameFit: n_valid and the padded size np
+
+// The handles of a multi-handle model, `groups` groups of `per`: hs[g * per + i].  Each is non-null, fitted and on the
+// device, stream and feature dimensions of hs[0]; `trials` says what the handles of one group share.
+static int check_handles(vzgp_handle* const* hs, int groups, int per, Trials trials) {
+  for (int k = 0; k < groups * per; ++k) {
+    const vzgp_handle* h = hs[k];
+    const vzgp_handle* first = hs[k / per * per];
+    VZ_ARG(h != nullptr, "handle");
+    if (!h->fitted) { set_error("scoring needs every handle fitted"); return VZGP_ERR_STATE; }
+    VZ_ARG(h->device == hs[0]->device && h->stream == hs[0]->stream, "all handles must share device and stream");
+    VZ_ARG(h->dc == hs[0]->dc && h->dk == hs[0]->dk, "all handles must have the same feature dimensions");
+    VZ_ARG(trials == Trials::kAny ||
+               (h->n_valid == first->n_valid && (trials == Trials::kSameNValid || h->np == first->np)),
+           "the handles of a model must be fitted on the same trials");
+  }
+  return 0;
+}
+
+// A pool of M candidates for models with the features of h (nothing is read or written when M = 0).
+static int check_pool(const vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const double* score) {
+  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
+  VZ_ARG(M == 0 || Xs != nullptr || h->dc == 0, "Xs");
+  VZ_ARG(M == 0 || Zs != nullptr || h->dk == 0, "Zs");
+  return 0;
+}
+
+// GP-UCB-PE: model A and model B (P: vzgp_pe_params or vzgp_pe_multi_params).
+template <class P>
+static int check_pe(vzgp_handle* hA, vzgp_handle* hB, const P* pe) {
+  VZ_ARG(hA && hB && pe, "handles / pe");
+  vzgp_handle* const hs[2] = {hA, hB};
+  VZ_TRY(check_handles(hs, 2, 1, Trials::kAny));
+  VZ_ARG(pe->mode == 0 || pe->mode == 1, "mode");
+  return 0;
+}
+
 static int check_separable(vzgp_handle* const* hs, int M) {
   VZ_ARG(hs != nullptr && M >= 1 && M <= kMaxMetrics, "1 <= M <= 8 member handles");
-  for (int j = 0; j < M; ++j) {
-    VZ_ARG(hs[j] != nullptr, "handle");
-    if (!hs[j]->fitted) { set_error("separable model used before vzgp_fit_separable"); return VZGP_ERR_STATE; }
-    VZ_ARG(hs[j]->device == hs[0]->device && hs[j]->stream == hs[0]->stream, "members must share device and stream");
-    VZ_ARG(hs[j]->dc == hs[0]->dc && hs[j]->dk == hs[0]->dk && hs[j]->n_valid == hs[0]->n_valid,
-           "members must be fitted on the same trials");
-  }
+  VZ_TRY(check_handles(hs, 1, M, Trials::kSameNValid));
   if (hs[0]->sep_m != M) { set_error("hs[0] does not hold a separable fit with M tasks"); return VZGP_ERR_STATE; }
   return 0;
 }
@@ -1110,31 +1142,59 @@ static int eagle_check_config(const vzgp_handle* h, const vzgp_eagle_config* cfg
   return 0;
 }
 
-static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_config* cfg, const vzgp_acq* acq,
-                          const vzgp_pe_params* pe, const double* prior, const int32_t* prior_z, int n_prior,
-                          const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
-                          double* best_score, vzgp_handle* const* ens = nullptr, int n_ens = 0,
-                          const vzgp_scalarization* scal = nullptr, const double* stack_alphas = nullptr,
-                          const vzgp_pe_multi_params* pem = nullptr, vzgp_handle* const* sep = nullptr,
-                          int n_sep = 0, vzgp_handle* const* ens_b = nullptr, int stack_members = 1) {
-  VZ_ARG(h && cfg && (acq || pe || scal || pem) && best_score, "handle / pointers");
-  const AcqFn* fn = (pe || scal || pem) ? nullptr : handle_acq(ens ? ens[0] : h);   // multi-handle calls: the setting of hs[0]
-  // GP-UCB-PE ensembles: ens = the E members of model A (h = ens[0]), ens_b those of model B (hB = ens_b[0])
-  // Stacks: ens = the handles of n_ens levels (stack_members each, level-major), h = the top level's (first) handle
-  auto score_batch = [&](const double* xs, const int32_t* zs, int m, double* out) -> int {
-    if (pe && ens_b) return launch_score_pe_ensemble(ens, ens_b, n_ens, xs, zs, m, pe, out, nullptr, nullptr, nullptr);
-    if (stack_alphas && scal) return launch_score_stack_multi(ens, n_ens, stack_alphas, xs, zs, m, out, nullptr, nullptr);
-    if (stack_alphas && stack_members > 1)
-      return launch_score_stack_ensemble(ens, n_ens, stack_members, stack_alphas, xs, zs, m, acq, out, nullptr, nullptr,
-                                         nullptr, fn);
-    if (pem) return launch_score_pe_multi(h, hB, xs, zs, m, pem, out, nullptr, nullptr, nullptr);
-    if (sep) return launch_score_separable(sep, n_sep, xs, zs, m, out, nullptr, nullptr);
-    if (scal) return launch_score_multi(h, xs, zs, m, out, nullptr, nullptr);
-    if (pe) return launch_score_pe(h, hB, xs, zs, m, pe, out, nullptr, nullptr, nullptr);
-    if (stack_alphas) return launch_score_stack(ens, n_ens, stack_alphas, xs, zs, m, acq, out, nullptr, nullptr, nullptr, fn);
-    if (n_ens > 1) return launch_score_ensemble(ens, n_ens, xs, zs, m, acq, out, nullptr, nullptr, nullptr, fn);
-    return launch_score(h, xs, zs, m, acq, out, nullptr, nullptr, nullptr, fn);
-  };
+// What an Eagle run scores its batches against: the kind of model, its handles and the one request that kind takes.
+// The vzgp_eagle_run_* entry points fill it after validation.
+struct Model {
+  enum Kind { kSingle, kEnsemble, kStack, kPe, kPeMulti, kMulti, kStackMulti, kSeparable };
+  Kind kind;
+  vzgp_handle* owner;                         // holds the Eagle state
+  vzgp_handle* const* hs;                     // model A of GP-UCB-PE; stacks level-major, hs[l * E + e]
+  vzgp_handle* const* hBs = nullptr;          // GP-UCB-PE: model B
+  int n = 1;                                  // levels of a stack, tasks of a separable model
+  int E = 1;                                  // members per level (ensembles, stacks) or per model (GP-UCB-PE)
+  const double* alphas = nullptr;             // stacks
+  const vzgp_acq* acq = nullptr;              // single, ensemble, stack: with the acquisition function of hs[0]
+  const vzgp_pe_params* pe = nullptr;         // GP-UCB-PE
+  const vzgp_pe_multi_params* pem = nullptr;  // multi-metric GP-UCB-PE
+  const vzgp_scalarization* sc = nullptr;     // multi, stacked multi, separable
+
+  const AcqFn* fn() const { return acq ? handle_acq(hs[0]) : nullptr; }
+  // The persistent and cooperative single-model loops score one GP, or one GP-UCB-PE pair, inside the kernel.
+  bool single_form() const { return kind == kSingle || (kind == kPe && E == 1); }
+  // prepare: the one-time set-up before the loop; otherwise the scores of M candidates into out (capturable).
+  int run(bool prepare, const double* xs = nullptr, const int32_t* zs = nullptr, int M = 0, double* out = nullptr) const {
+    switch (kind) {
+      case kSingle:
+        return prepare ? 0 : launch_score(hs[0], xs, zs, M, acq, out, nullptr, nullptr, nullptr, fn());
+      case kEnsemble:
+        return prepare ? 0 : launch_score_ensemble(hs, E, xs, zs, M, acq, out, nullptr, nullptr, nullptr, fn());
+      case kStack:
+        return prepare ? 0
+                       : launch_score_stack_ensemble(hs, n, E, alphas, xs, zs, M, acq, out, nullptr, nullptr, nullptr,
+                                                     fn());
+      case kPe:
+        return prepare ? 0 : launch_score_pe_ensemble(hs, hBs, E, xs, zs, M, pe, out, nullptr, nullptr, nullptr);
+      case kPeMulti:
+        return prepare ? prepare_score_pe_multi(hs[0], pem)
+                       : launch_score_pe_multi(hs[0], hBs[0], xs, zs, M, pem, out, nullptr, nullptr, nullptr);
+      case kMulti:
+        return prepare ? prepare_scalarization(hs[0], sc) : launch_score_multi(hs[0], xs, zs, M, out, nullptr, nullptr);
+      case kStackMulti:
+        return prepare ? prepare_scalarization(owner, sc)
+                       : launch_score_stack_multi(hs, n, alphas, xs, zs, M, out, nullptr, nullptr);
+      case kSeparable:
+        return prepare ? prepare_scalarization(hs[0], sc, n)
+                       : launch_score_separable(hs, n, xs, zs, M, out, nullptr, nullptr);
+    }
+    return VZGP_ERR_ARG;
+  }
+};
+
+static int eagle_run_impl(const Model& m, const vzgp_eagle_config* cfg, const double* prior, const int32_t* prior_z,
+                          int n_prior, const int32_t* cat_sizes, int count, uint64_t seed, double* best_x,
+                          int32_t* best_z, double* best_score) {
+  vzgp_handle* h = m.owner;
+  VZ_ARG(h && cfg && best_score, "handle / pointers");
   if (!h->fitted) { set_error("vzgp_eagle_run before vzgp_fit"); return VZGP_ERR_STATE; }
   VZ_ARG(best_x != nullptr || h->dc == 0, "best_x");
   VZ_ARG(best_z != nullptr || h->dk == 0, "best_z");
@@ -1151,17 +1211,16 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
   double* prior_r = es.prior_r;
   double* chosen_r = es.chosen_r;
   int* ord = es.ord;
-  if (scal) VZ_TRY(prepare_scalarization(h, scal, sep ? n_sep : 0));
-  if (pem) VZ_TRY(prepare_score_pe_multi(h, pem));
+  VZ_TRY(m.run(true));
   VZ_TRY(launch_eagle_init(h, e));
   if (n_prior > 0) {
-    VZ_TRY(score_batch(prior, Dk > 0 ? prior_z : nullptr, n_prior, prior_r));
+    VZ_TRY(m.run(false, prior, Dk > 0 ? prior_z : nullptr, n_prior, prior_r));
     VZ_TRY(launch_eagle_seed_priors(h, e, prior, prior_z, prior_r, n_prior, ord, chosen_r));
   }
   const int steps = (cfg->max_evaluations - 1) / B + 1;
   auto one_step = [&]() -> int {
     VZ_TRY(launch_eagle_suggest(h, e));
-    VZ_TRY(score_batch(e.batch, Dk > 0 ? e.batch_z : nullptr, B, e.batch_r));
+    VZ_TRY(m.run(false, e.batch, Dk > 0 ? e.batch_z : nullptr, B, e.batch_r));
     VZ_TRY(launch_eagle_update(h, e));
     return 0;
   };
@@ -1169,22 +1228,21 @@ static int eagle_run_impl(vzgp_handle* h, vzgp_handle* hB, const vzgp_eagle_conf
   // CUDA graph of the suggest -> score -> update sequence: the iteration counter and all state
   // live in device memory, so the launches are identical and the host only enqueues graphs.
   bool done = false;
-  // the persistent and cooperative forms evaluate single-metric acquisitions only
-  const bool fused_ok = n_ens <= 1 && !scal && !stack_alphas && !pem;
-  if (fused_ok && eagle_persistent_eligible(h, pe ? hB : nullptr, e)) {
+  vzgp_handle* hB = m.kind == Model::kPe ? m.hBs[0] : nullptr;
+  if (m.single_form() && eagle_persistent_eligible(h, hB, e)) {
     // small study: the whole loop is one persistent single-CTA kernel
-    VZ_TRY(launch_eagle_persistent64(h, pe ? hB : nullptr, e, acq, pe, steps, fn));
+    VZ_TRY(launch_eagle_persistent64(h, hB, e, m.acq, m.pe, steps, m.fn()));
     h->eagle_route = VZGP_EAGLE_PERSISTENT;
     done = true;
-  } else if (fused_ok && eagle_grid_eligible(h, pe ? hB : nullptr, e)) {
+  } else if (m.single_form() && eagle_grid_eligible(h, hB, e)) {
     // mid-size study: one cooperative launch, phases separated by grid barriers.  If the cooperative
     // launch is refused (nothing has run then) the launch-per-phase loop below takes over.
-    done = launch_eagle_grid(h, pe ? hB : nullptr, e, acq, pe, steps, fn) == 0;
+    done = launch_eagle_grid(h, hB, e, m.acq, m.pe, steps, m.fn()) == 0;
     if (done) h->eagle_route = VZGP_EAGLE_COOPERATIVE;
     else cudaGetLastError();
-  } else if (pe && ens_b && eagle_grid_pe_ensemble_eligible(ens, ens_b, n_ens, e)) {
-    // the same cooperative loop over the 2E member models (E = 1 took the single-model forms above)
-    done = launch_eagle_grid_pe_ensemble(ens, ens_b, n_ens, e, pe, steps) == 0;
+  } else if (m.kind == Model::kPe && eagle_grid_pe_ensemble_eligible(m.hs, m.hBs, m.E, e)) {
+    // the same cooperative loop over the 2E member models (2 <= E; E = 1 took the single-model forms above)
+    done = launch_eagle_grid_pe_ensemble(m.hs, m.hBs, m.E, e, m.pe, steps) == 0;
     if (done) h->eagle_route = VZGP_EAGLE_COOPERATIVE;
     else cudaGetLastError();
   }
@@ -1318,37 +1376,28 @@ int vzgp_eagle_run(vzgp_handle* h, const vzgp_eagle_config* cfg, const vzgp_acq*
                    const int32_t* prior_z, int n_prior, const int32_t* cat_sizes, int count, uint64_t seed,
                    double* best_x, int32_t* best_z, double* best_score) {
   VZ_ARG(acq != nullptr, "acq");
-  return eagle_run_impl(h, nullptr, cfg, acq, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
-                        best_z, best_score);
+  Model m{Model::kSingle, h, &h};
+  m.acq = acq;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 int vzgp_eagle_run_multi(vzgp_handle* h, const vzgp_eagle_config* cfg, const vzgp_scalarization* sc,
                          const double* prior, const int32_t* prior_z, int n_prior, const int32_t* cat_sizes,
                          int count, uint64_t seed, double* best_x, int32_t* best_z, double* best_score) {
   VZ_ARG(sc != nullptr, "scalarization");
-  return eagle_run_impl(h, nullptr, cfg, nullptr, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
-                        best_z, best_score, nullptr, 0, sc);
+  Model m{Model::kMulti, h, &h};
+  m.sc = sc;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 int vzgp_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_scalarization* sc,
                      double* score, double* mu, double* sigma) {
   VZ_ARG(h != nullptr && sc != nullptr, "handle / scalarization");
   if (!h->fitted) { set_error("vzgp_score_multi before vzgp_fit_multi"); return VZGP_ERR_STATE; }
-  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
-  VZ_ARG(M == 0 || Xs != nullptr || h->dc == 0, "Xs");
-  VZ_ARG(M == 0 || Zs != nullptr || h->dk == 0, "Zs");
+  VZ_TRY(check_pool(h, Xs, Zs, M, score));
   Guard g(h->device);
   VZ_TRY(prepare_scalarization(h, sc));
   return launch_score_multi(h, Xs, Zs, M, score, mu, sigma);
-}
-
-static int check_pe(vzgp_handle* hA, vzgp_handle* hB, const vzgp_pe_params* pe) {
-  VZ_ARG(hA && hB && pe, "handles / pe");
-  if (!hA->fitted || !hB->fitted) { set_error("GP-UCB-PE scoring needs both models fitted"); return VZGP_ERR_STATE; }
-  VZ_ARG(hA->device == hB->device && hA->stream == hB->stream, "both models must share device and stream");
-  VZ_ARG(hA->dc == hB->dc && hA->dk == hB->dk, "both models must have the same feature dimensions");
-  VZ_ARG(pe->mode == 0 || pe->mode == 1, "mode");
-  return 0;
 }
 
 int vzgp_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
@@ -1356,7 +1405,7 @@ int vzgp_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int3
   VZ_TRY(check_pe(hA, hB, pe));
   VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
   Guard g(hA->device);
-  return launch_score_pe(hA, hB, Xs, Zs, M, pe, score, mu, sigma, sigma_all);
+  return launch_score_pe_ensemble(&hA, &hB, 1, Xs, Zs, M, pe, score, mu, sigma, sigma_all);
 }
 
 int vzgp_score_set_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, int n_sets, int q, const vzgp_pe_params* pe,
@@ -1392,16 +1441,13 @@ int vzgp_eagle_run_pe(vzgp_handle* hA, vzgp_handle* hB, const vzgp_eagle_config*
                       const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
                       double* best_score) {
   VZ_TRY(check_pe(hA, hB, pe));
-  return eagle_run_impl(hA, hB, cfg, nullptr, pe, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z,
-                        best_score);
+  Model m{Model::kPe, hA, &hA};
+  m.hBs = &hB; m.pe = pe;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 static int check_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const vzgp_pe_multi_params* pe) {
-  VZ_ARG(hA && hB && pe, "handles / pe");
-  if (!hA->fitted || !hB->fitted) { set_error("GP-UCB-PE scoring needs both models fitted"); return VZGP_ERR_STATE; }
-  VZ_ARG(hA->device == hB->device && hA->stream == hB->stream, "both models must share device and stream");
-  VZ_ARG(hA->dc == hB->dc && hA->dk == hB->dk, "both models must have the same feature dimensions");
-  VZ_ARG(pe->mode == 0 || pe->mode == 1, "mode");
+  VZ_TRY(check_pe(hA, hB, pe));
   VZ_ARG(pe->n_metrics >= 1 && pe->n_metrics <= kMaxMetrics, "1 <= n_metrics <= 8");
   VZ_ARG(pe->n_metrics == hA->n_metrics, "n_metrics must equal the metrics model A was fitted with (vzgp_fit_multi)");
   VZ_ARG(pe->mode != 1 || pe->thresholds != nullptr, "thresholds (mode 1)");
@@ -1414,9 +1460,7 @@ static int check_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const vzgp_pe_multi_
 int vzgp_score_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
                         const vzgp_pe_multi_params* pe, double* score, double* mu, double* sigma, double* sigma_all) {
   VZ_TRY(check_pe_multi(hA, hB, pe));
-  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
-  VZ_ARG(M == 0 || Xs != nullptr || hA->dc == 0, "Xs");
-  VZ_ARG(M == 0 || Zs != nullptr || hA->dk == 0, "Zs");
+  VZ_TRY(check_pool(hA, Xs, Zs, M, score));
   Guard g(hA->device);
   VZ_TRY(prepare_score_pe_multi(hA, pe));
   return launch_score_pe_multi(hA, hB, Xs, Zs, M, pe, score, mu, sigma, sigma_all);
@@ -1427,29 +1471,21 @@ int vzgp_eagle_run_pe_multi(vzgp_handle* hA, vzgp_handle* hB, const vzgp_eagle_c
                             const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
                             double* best_score) {
   VZ_TRY(check_pe_multi(hA, hB, pe));
-  return eagle_run_impl(hA, hB, cfg, nullptr, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z,
-                        best_score, nullptr, 0, nullptr, nullptr, pe);
+  Model m{Model::kPeMulti, hA, &hA};
+  m.hBs = &hB; m.pem = pe;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 static int check_ensemble(vzgp_handle* const* hs, int E) {
   VZ_ARG(hs != nullptr && E >= 1 && E <= 16, "1 <= E <= 16 handles");
-  for (int e = 0; e < E; ++e) {
-    VZ_ARG(hs[e] != nullptr, "handle");
-    if (!hs[e]->fitted) { set_error("ensemble scoring needs every member fitted"); return VZGP_ERR_STATE; }
-    VZ_ARG(hs[e]->device == hs[0]->device && hs[e]->stream == hs[0]->stream, "members must share device and stream");
-    VZ_ARG(hs[e]->dc == hs[0]->dc && hs[e]->dk == hs[0]->dk && hs[e]->n_valid == hs[0]->n_valid,
-           "members must be fitted on the same trials");
-  }
-  return 0;
+  return check_handles(hs, 1, E, Trials::kSameNValid);
 }
 
 int vzgp_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int M,
                         const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf) {
   VZ_TRY(check_ensemble(hs, E));
   VZ_ARG(acq != nullptr, "acq");
-  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
-  VZ_ARG(M == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
-  VZ_ARG(M == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
+  VZ_TRY(check_pool(hs[0], Xs, Zs, M, score));
   Guard g(hs[0]->device);
   return launch_score_ensemble(hs, E, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(hs[0]));
 }
@@ -1459,23 +1495,19 @@ int vzgp_eagle_run_ensemble(vzgp_handle* const* hs, int E, const vzgp_eagle_conf
                             int count, uint64_t seed, double* best_x, int32_t* best_z, double* best_score) {
   VZ_TRY(check_ensemble(hs, E));
   VZ_ARG(acq != nullptr, "acq");
-  return eagle_run_impl(hs[0], nullptr, cfg, acq, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
-                        best_z, best_score, hs, E);
+  // the loop scores a one-member ensemble as the single model it is, without the mixture
+  Model m{E == 1 ? Model::kSingle : Model::kEnsemble, hs[0], hs};
+  m.E = E; m.acq = acq;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 static int check_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const vzgp_pe_params* pe) {
   VZ_ARG(hAs != nullptr && hBs != nullptr && pe != nullptr, "handles / pe");
   VZ_ARG(E >= 1 && E <= kMaxPeEnsemble, "1 <= E <= 8 members per model");
-  for (int k = 0; k < 2 * E; ++k) {
-    vzgp_handle* h = k < E ? hAs[k] : hBs[k - E];
-    VZ_ARG(h != nullptr, "handle");
-    if (!h->fitted) { set_error("GP-UCB-PE ensemble scoring needs every member of both models fitted"); return VZGP_ERR_STATE; }
-    VZ_ARG(h->device == hAs[0]->device && h->stream == hAs[0]->stream, "all members must share device and stream");
-    VZ_ARG(h->dc == hAs[0]->dc && h->dk == hAs[0]->dk, "all members must have the same feature dimensions");
-    VZ_ARG(h->n_metrics == 1, "GP-UCB-PE ensembles: single-metric members");
-    const vzgp_handle* first = k < E ? hAs[0] : hBs[0];
-    VZ_ARG(h->n_valid == first->n_valid && h->np == first->np, "the members of a model must be fitted on the same trials");
-  }
+  vzgp_handle* hs[2 * kMaxPeEnsemble];
+  for (int e = 0; e < E; ++e) { hs[e] = hAs[e]; hs[E + e] = hBs[e]; }
+  VZ_TRY(check_handles(hs, 2, E, Trials::kSameFit));
+  for (int k = 0; k < 2 * E; ++k) VZ_ARG(hs[k]->n_metrics == 1, "GP-UCB-PE ensembles: single-metric members");
   VZ_ARG(pe->mode == 0 || pe->mode == 1, "mode");
   return 0;
 }
@@ -1483,9 +1515,7 @@ static int check_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, i
 int vzgp_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const double* Xs, const int32_t* Zs,
                            int M, const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all) {
   VZ_TRY(check_pe_ensemble(hAs, hBs, E, pe));
-  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
-  VZ_ARG(M == 0 || Xs != nullptr || hAs[0]->dc == 0, "Xs");
-  VZ_ARG(M == 0 || Zs != nullptr || hAs[0]->dk == 0, "Zs");
+  VZ_TRY(check_pool(hAs[0], Xs, Zs, M, score));
   Guard g(hAs[0]->device);
   return launch_score_pe_ensemble(hAs, hBs, E, Xs, Zs, M, pe, score, mu, sigma, sigma_all);
 }
@@ -1495,8 +1525,9 @@ int vzgp_eagle_run_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs,
                                const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
                                double* best_score) {
   VZ_TRY(check_pe_ensemble(hAs, hBs, E, pe));
-  return eagle_run_impl(hAs[0], hBs[0], cfg, nullptr, pe, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
-                        best_z, best_score, hAs, E, nullptr, nullptr, nullptr, nullptr, 0, hBs);
+  Model m{Model::kPe, hAs[0], hAs};
+  m.hBs = hBs; m.E = E; m.pe = pe;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 static int check_qacq(const vzgp_qacq* qa, int n_sets, int q) {
@@ -1514,9 +1545,7 @@ int vzgp_score_qsets(vzgp_handle* const* hs, int E, const double* Xs, const int3
   VZ_TRY(check_qacq(qa, n_sets, q));
   for (int e = 0; e < E; ++e) VZ_ARG(hs[e]->n_metrics == 1, "q-acquisitions: single-metric models");
   VZ_ARG(hs[0]->dc <= kMaxDc && hs[0]->dk <= kMaxDk, "Dc <= 64, Dk <= 32");
-  VZ_ARG(n_sets == 0 || score != nullptr, "score");
-  VZ_ARG(n_sets == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
-  VZ_ARG(n_sets == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
+  VZ_TRY(check_pool(hs[0], Xs, Zs, n_sets, score));
   if (n_sets == 0) return 0;
   Guard g(hs[0]->device);
   return launch_score_qsets(hs, E, Xs, Zs, n_sets, q, qa, seed, score, mu, sigma, linf);
@@ -1533,66 +1562,26 @@ int vzgp_qacq_from_moments(vzgp_handle* h, int n_sets, int q, int E, const doubl
   return launch_qacq_mc(h, n_sets, q, E, mean, cov, nullptr, qa, seed, score, nullptr, nullptr);
 }
 
-static int check_stack(vzgp_handle* const* hs, int E, const double* alphas) {
-  VZ_ARG(hs != nullptr && alphas != nullptr && E >= 1 && E <= 16, "1 <= E <= 16 handles, alphas");
-  for (int e = 0; e < E; ++e) {
-    VZ_ARG(hs[e] != nullptr, "handle");
-    if (!hs[e]->fitted) { set_error("stacked scoring needs every level fitted"); return VZGP_ERR_STATE; }
-    VZ_ARG(hs[e]->device == hs[0]->device && hs[e]->stream == hs[0]->stream, "levels must share device and stream");
-    VZ_ARG(hs[e]->dc == hs[0]->dc && hs[e]->dk == hs[0]->dk, "levels must have the same feature dimensions");
-    VZ_ARG(e == 0 || (alphas[e] >= 0.0 && alphas[e] <= 1.0), "0 <= alpha <= 1");
-  }
-  return 0;
-}
-
-int vzgp_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const double* Xs, const int32_t* Zs, int M,
-                     const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf) {
-  VZ_TRY(check_stack(hs, E, alphas));
-  VZ_ARG(acq != nullptr, "acq");
-  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
-  VZ_ARG(M == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
-  VZ_ARG(M == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
-  Guard g(hs[0]->device);
-  return launch_score_stack(hs, E, alphas, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(hs[0]));
-}
-
-int vzgp_eagle_run_stack(vzgp_handle* const* hs, int E, const double* alphas, const vzgp_eagle_config* cfg,
-                         const vzgp_acq* acq, const double* prior, const int32_t* prior_z, int n_prior,
-                         const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
-                         double* best_score) {
-  VZ_TRY(check_stack(hs, E, alphas));
-  VZ_ARG(acq != nullptr, "acq");
-  return eagle_run_impl(hs[E - 1], nullptr, cfg, acq, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
-                        best_z, best_score, hs, E, nullptr, alphas);
-}
-
-// Stacks of uniform ensembles and of independent multi-metric levels: every handle fitted, on one device and stream,
-// with the same feature dimensions; the members of a level (hs[l * E .. l * E + E)) fitted on the same trials.
-static int check_stack_levels(vzgp_handle* const* hs, int L, int E, const double* alphas) {
+// Stacks of L levels of E members, hs[l * E + e] (E = 1: single GPs, or the independent multi-metric levels of
+// vzgp_score_stack_multi): every handle fitted, on one device and stream, with the same feature dimensions; the
+// members of a level fitted on the same trials.
+static int check_stack(vzgp_handle* const* hs, int L, int E, const double* alphas) {
   VZ_ARG(hs != nullptr && alphas != nullptr, "handles / alphas");
   VZ_ARG(L >= 1 && L <= kMaxStackLevels, "1 <= n_levels <= 16");
   VZ_ARG(E >= 1 && E <= kMaxPeEnsemble, "1 <= E <= 8 members per level");
-  for (int k = 0; k < L * E; ++k) VZ_ARG(hs[k] != nullptr, "handle");
-  for (int k = 0; k < L * E; ++k) {
-    vzgp_handle* h = hs[k];
-    if (!h->fitted) { set_error("stacked scoring needs every member of every level fitted"); return VZGP_ERR_STATE; }
-    VZ_ARG(h->device == hs[0]->device && h->stream == hs[0]->stream, "levels must share device and stream");
-    VZ_ARG(h->dc == hs[0]->dc && h->dk == hs[0]->dk, "levels must have the same feature dimensions");
-    const vzgp_handle* first = hs[(k / E) * E];
-    VZ_ARG(h->n_valid == first->n_valid && h->np == first->np, "the members of a level must be fitted on the same trials");
-  }
+  VZ_TRY(check_handles(hs, L, E, Trials::kSameFit));
   for (int l = 1; l < L; ++l) VZ_ARG(alphas[l] >= 0.0 && alphas[l] <= 1.0, "0 <= alpha <= 1");
   return 0;
 }
 
 static int check_stack_ensemble(vzgp_handle* const* hs, int L, int E, const double* alphas) {
-  VZ_TRY(check_stack_levels(hs, L, E, alphas));
+  VZ_TRY(check_stack(hs, L, E, alphas));
   for (int k = 0; k < L * E; ++k) VZ_ARG(hs[k]->n_metrics == 1, "stacked ensembles: single-metric members");
   return 0;
 }
 
 static int check_stack_multi(vzgp_handle* const* hs, int L, const double* alphas, const vzgp_scalarization* sc) {
-  VZ_TRY(check_stack_levels(hs, L, 1, alphas));
+  VZ_TRY(check_stack(hs, L, 1, alphas));
   VZ_ARG(sc != nullptr, "scalarization");
   for (int l = 0; l < L; ++l) {
     VZ_ARG(hs[l]->n_metrics >= 2 && hs[l]->n_metrics == hs[0]->n_metrics,
@@ -1602,15 +1591,32 @@ static int check_stack_multi(vzgp_handle* const* hs, int L, const double* alphas
   return 0;
 }
 
+int vzgp_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const double* Xs, const int32_t* Zs, int M,
+                     const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf) {
+  VZ_TRY(check_stack(hs, E, 1, alphas));
+  VZ_ARG(acq != nullptr, "acq");
+  VZ_TRY(check_pool(hs[0], Xs, Zs, M, score));
+  Guard g(hs[0]->device);
+  return launch_score_stack_ensemble(hs, E, 1, alphas, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(hs[0]));
+}
+
+int vzgp_eagle_run_stack(vzgp_handle* const* hs, int E, const double* alphas, const vzgp_eagle_config* cfg,
+                         const vzgp_acq* acq, const double* prior, const int32_t* prior_z, int n_prior,
+                         const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
+                         double* best_score) {
+  VZ_TRY(check_stack(hs, E, 1, alphas));
+  VZ_ARG(acq != nullptr, "acq");
+  Model m{Model::kStack, hs[E - 1], hs};
+  m.n = E; m.alphas = alphas; m.acq = acq;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
+}
+
 int vzgp_score_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, const double* alphas, const double* Xs,
                               const int32_t* Zs, int M, const vzgp_acq* acq, double* score, double* mu, double* sigma,
                               double* linf) {
   VZ_TRY(check_stack_ensemble(hs, n_levels, E, alphas));
-  if (E == 1) return vzgp_score_stack(hs, n_levels, alphas, Xs, Zs, M, acq, score, mu, sigma, linf);
   VZ_ARG(acq != nullptr, "acq");
-  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
-  VZ_ARG(M == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
-  VZ_ARG(M == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
+  VZ_TRY(check_pool(hs[0], Xs, Zs, M, score));
   Guard g(hs[0]->device);
   return launch_score_stack_ensemble(hs, n_levels, E, alphas, Xs, Zs, M, acq, score, mu, sigma, linf,
                                      handle_acq(hs[0]));
@@ -1621,21 +1627,17 @@ int vzgp_eagle_run_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, c
                                   const int32_t* prior_z, int n_prior, const int32_t* cat_sizes, int count,
                                   uint64_t seed, double* best_x, int32_t* best_z, double* best_score) {
   VZ_TRY(check_stack_ensemble(hs, n_levels, E, alphas));
-  if (E == 1)
-    return vzgp_eagle_run_stack(hs, n_levels, alphas, cfg, acq, prior, prior_z, n_prior, cat_sizes, count, seed,
-                                best_x, best_z, best_score);
   VZ_ARG(acq != nullptr, "acq");
-  return eagle_run_impl(hs[(n_levels - 1) * E], nullptr, cfg, acq, nullptr, prior, prior_z, n_prior, cat_sizes, count,
-                        seed, best_x, best_z, best_score, hs, n_levels, nullptr, alphas, nullptr, nullptr, 0, nullptr, E);
+  Model m{Model::kStack, hs[(n_levels - 1) * E], hs};
+  m.n = n_levels; m.E = E; m.alphas = alphas; m.acq = acq;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 int vzgp_score_stack_multi(vzgp_handle* const* hs, int n_levels, const double* alphas, const double* Xs,
                            const int32_t* Zs, int M, const vzgp_scalarization* sc, double* score, double* mu,
                            double* sigma) {
   VZ_TRY(check_stack_multi(hs, n_levels, alphas, sc));
-  VZ_ARG(M >= 0 && (M == 0 || score != nullptr), "M / score");
-  VZ_ARG(M == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
-  VZ_ARG(M == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
+  VZ_TRY(check_pool(hs[0], Xs, Zs, M, score));
   Guard g(hs[0]->device);
   VZ_TRY(prepare_scalarization(hs[n_levels - 1], sc));
   return launch_score_stack_multi(hs, n_levels, alphas, Xs, Zs, M, score, mu, sigma);
@@ -1646,8 +1648,9 @@ int vzgp_eagle_run_stack_multi(vzgp_handle* const* hs, int n_levels, const doubl
                                const int32_t* cat_sizes, int count, uint64_t seed, double* best_x, int32_t* best_z,
                                double* best_score) {
   VZ_TRY(check_stack_multi(hs, n_levels, alphas, sc));
-  return eagle_run_impl(hs[n_levels - 1], nullptr, cfg, nullptr, nullptr, prior, prior_z, n_prior, cat_sizes, count,
-                        seed, best_x, best_z, best_score, hs, n_levels, sc, alphas);
+  Model m{Model::kStackMulti, hs[n_levels - 1], hs};
+  m.n = n_levels; m.alphas = alphas; m.sc = sc;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 // The graph-batched evaluation behind vzgp_nll_grad_batch and vzgp_nll_grad_separable_batch: branch r evaluates
@@ -2116,9 +2119,7 @@ int vzgp_score_separable(vzgp_handle* const* hs, int M, const double* Xs, const 
                          const vzgp_scalarization* sc, double* score, double* mu, double* sigma) {
   VZ_TRY(check_separable(hs, M));
   VZ_ARG(sc != nullptr, "scalarization");
-  VZ_ARG(n >= 0 && (n == 0 || score != nullptr), "n / score");
-  VZ_ARG(n == 0 || Xs != nullptr || hs[0]->dc == 0, "Xs");
-  VZ_ARG(n == 0 || Zs != nullptr || hs[0]->dk == 0, "Zs");
+  VZ_TRY(check_pool(hs[0], Xs, Zs, n, score));
   Guard g(hs[0]->device);
   VZ_TRY(prepare_scalarization(hs[0], sc, M));
   return launch_score_separable(hs, M, Xs, Zs, n, score, mu, sigma);
@@ -2129,8 +2130,9 @@ int vzgp_eagle_run_separable(vzgp_handle* const* hs, int M, const vzgp_eagle_con
                              int count, uint64_t seed, double* best_x, int32_t* best_z, double* best_score) {
   VZ_TRY(check_separable(hs, M));
   VZ_ARG(sc != nullptr, "scalarization");
-  return eagle_run_impl(hs[0], nullptr, cfg, nullptr, nullptr, prior, prior_z, n_prior, cat_sizes, count, seed, best_x,
-                        best_z, best_score, nullptr, 0, sc, nullptr, nullptr, hs, M);
+  Model m{Model::kSeparable, hs[0], hs};
+  m.n = M; m.sc = sc;
+  return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
 }
 
 int vzgp_posterior_separable(vzgp_handle* const* hs, int M, const double* Xs, const int32_t* Zs, int n, int add_noise,

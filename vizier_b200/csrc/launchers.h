@@ -109,17 +109,12 @@ int launch_score_i8(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
 // CUtensorMap (void*) of a u8 tensor of `rank` <= 3 dims (innermost first), byte strides of dims 1.., 128-byte swizzle.
 int make_tensor_map_u8(void* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
                        const uint32_t* box, bool promote_256 = true);
-int launch_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
-                    const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all);
-// GP-UCB-PE over uniform ensembles of E members per model (pe_ensemble.cuh; score.cu).
+// GP-UCB-PE over uniform ensembles of E members per model, E = 1 for two single models (pe_ensemble.cuh; score.cu).
 int launch_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const double* Xs,
                              const int32_t* Zs, int M, const vzgp_pe_params* pe, double* score, double* mu,
                              double* sigma, double* sigma_all);
-int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const double* Xs, const int32_t* Zs, int M,
-                       const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf,
-                       const AcqFn* fn = nullptr);
-// Stacks whose levels are uniform ensembles of E members (hs[l * E + e], score.cu) or independent multi-metric GPs
-// scored with the scalarisation prepared on the top level (multi.cu).
+// Stacks whose levels are uniform ensembles of E members (hs[l * E + e]; E = 1 for single GPs, score.cu) or
+// independent multi-metric GPs scored with the scalarisation prepared on the top level (multi.cu).
 constexpr int kMaxStackLevels = 16;
 int launch_score_stack_ensemble(vzgp_handle* const* hs, int L, int E, const double* alphas, const double* Xs,
                                 const int32_t* Zs, int M, const vzgp_acq* acq, double* score, double* mu, double* sigma,

@@ -236,7 +236,7 @@ int launch_score_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int 
 
 // Stacked residual GPs of independent multi-task levels (transfer learning with several metrics): every level has one
 // factor, so its stddev is shared by the metrics, and one alpha per metric.  mean_m = sum_l mu_l,m; the stddevs are
-// stacked bottom-up as in k_stack_combine, s <- sd_l^alpha_l * s^(1 - alpha_l); then u_m = mean_m + c s and the
+// stacked bottom-up as in k_stack_ensemble_combine, s <- sd_l^alpha_l * s^(1 - alpha_l); then u_m = mean_m + c s and the
 // floored HV scalarisation of k_scalarize, without a trust region (gp_bandit.py:242).
 // mu: [L][n_metrics][M], sd: [L][M]; mu_out optional [n_metrics][M], sigma_out optional [M].
 struct StackMultiCombine {

@@ -950,6 +950,32 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
 }
 
 // ---------------------------------------------------------------------------
+// The member loop of the multi-model launchers (ensembles, stacks, GP-UCB-PE): groups[g][e] (g < n_groups, e < per)
+// is scored by launch_score on its own route, mean and stddev, into owner->pe_tmp, which launch_score does not
+// touch: [2 n_groups per + 2][M] = per group mu | sd (per rows each), then linf | dummy.  Every member asks for
+// `req`; member `dist` of the last group asks for `req_dist` and, when want_linf, writes the trust-region distance
+// to *linf (the linf plane when *linf is null).  *planes = the first plane.  Asynchronous, capturable.
+// ---------------------------------------------------------------------------
+static int score_members(vzgp_handle* owner, vzgp_handle* const* const* groups, int n_groups, int per,
+                         const double* Xs, const int32_t* Zs, int M, const vzgp_acq& req, int dist,
+                         const vzgp_acq& req_dist, bool want_linf, double** planes, double** linf) {
+  const size_t n = (size_t)n_groups * per;
+  VZ_TRY(owner->pe_tmp.reserve(sizeof(double) * (2 * n + 2) * (size_t)M));
+  double* t = owner->pe_tmp.as<double>();
+  if (*linf == nullptr) *linf = t + 2 * n * M;
+  double* dummy = t + (2 * n + 1) * M;
+  for (int g = 0; g < n_groups; ++g)
+    for (int e = 0; e < per; ++e) {
+      const bool d = g == n_groups - 1 && e == dist;
+      double* mu = t + (2 * (size_t)g * per + e) * M;
+      VZ_TRY(launch_score(groups[g][e], Xs, Zs, M, d ? &req_dist : &req, dummy, mu, mu + (size_t)per * M,
+                          d && want_linf ? *linf : nullptr));
+    }
+  *planes = t;
+  return 0;
+}
+
+// ---------------------------------------------------------------------------
 // GP-UCB-PE acquisition from the pieces of two models (gp_ucb_pe.py:344-381, :434-492, :221-242).
 // ---------------------------------------------------------------------------
 struct PeCombine {
@@ -957,105 +983,17 @@ struct PeCombine {
   double ucb, explore, penalty, threshold;
   TrustRegion tr;
 };
-__global__ void k_pe_combine(int M, PeCombine p, const double* __restrict__ mu, const double* __restrict__ sd,
-                             const double* __restrict__ sd_all, const double* __restrict__ linf,
-                             double* __restrict__ score) {
-  const int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= M) return;
-  double acq;
-  if (p.mode == 0) {
-    acq = fma(p.ucb, sd_all[m], mu[m]);
-  } else {
-    const double explore_ucb = fma(sd[m], p.explore, mu[m]);
-    acq = sd_all[m] + p.penalty * fmin(explore_ucb - p.threshold, 0.0);
-  }
-  score[m] = tr_apply(p.tr, acq, linf[m]);
-}
-
-int launch_score_pe(vzgp_handle* hA, vzgp_handle* hB, const double* Xs, const int32_t* Zs, int M,
-                    const vzgp_pe_params* pe, double* score, double* mu, double* sigma, double* sigma_all) {
-  if (M <= 0) return 0;
-  VZ_TRY(hA->pe_tmp.reserve(sizeof(double) * 6 * (size_t)M));
-  double* t = hA->pe_tmp.as<double>();
-  double* mu_a = mu ? mu : t;
-  double* sd_a = sigma ? sigma : t + M;
-  double* sd_b = sigma_all ? sigma_all : t + 2 * (size_t)M;
-  double* linf_b = t + 3 * (size_t)M;
-  double* dummy_a = t + 4 * (size_t)M;
-  double* dummy_b = t + 5 * (size_t)M;
-  const vzgp_acq none = posterior_request(), accb = posterior_request(pe->tr_dim_mask, pe->tr_rows);
-  PeCombine p;
-  p.mode = pe->mode; p.ucb = pe->ucb_coefficient; p.explore = pe->explore_coefficient;
-  p.penalty = pe->penalty_coefficient; p.threshold = pe->threshold;
-  p.tr = trust_region_of(hB, *pe, true);
-  VZ_TRY(launch_score(hA, Xs, Zs, M, &none, dummy_a, mu_a, sd_a, nullptr));
-  VZ_TRY(launch_score(hB, Xs, Zs, M, &accb, dummy_b, nullptr, sd_b, tr_needs_distance(p.tr) ? linf_b : nullptr));
-  k_pe_combine<<<(M + 255) / 256, 256, 0, hA->stream>>>(M, p, mu_a, sd_a, sd_b, linf_b, score);
-  VZ_CHECK_LAUNCH();
-  hA->launches++;
-  return 0;
-}
 
 // ---------------------------------------------------------------------------
 // Stacked residual GPs of transfer learning (StackedResidualGP, gp/gp_models.py:91-140; combine_predictions_with_aux,
 // gp/transfer_learning.py:62-152): level 0 is the first prior study's GP, every further level is trained on the
-// residuals of the stack below it, the last level on the current study.  mean = sum of the level means; the stddevs
-// are combined bottom-up by weighted geometric means  s <- sd_e^alpha_e * s^(1 - alpha_e)  (alpha_e from the degrees
-// of freedom of the two levels, computed by the caller).  UCB and the trust region (distances to the TOP level's
-// trials) on the combined prediction.
-// ---------------------------------------------------------------------------
-struct StackCombine {
-  int E;
-  double alpha[16];
-  AcqFn acq;
-  TrustRegion tr;
-};
-__global__ void k_stack_combine(int M, StackCombine p, const double* __restrict__ mu_e, const double* __restrict__ sd_e,
-                                const double* __restrict__ linf, double* __restrict__ score, double* __restrict__ mu,
-                                double* __restrict__ sigma) {
-  const int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= M) return;
-  double mean = mu_e[m], sd = sd_e[m];
-  for (int e = 1; e < p.E; ++e) {
-    mean += mu_e[(size_t)e * M + m];
-    sd = pow(sd_e[(size_t)e * M + m], p.alpha[e]) * pow(sd, 1.0 - p.alpha[e]);
-  }
-  score[m] = tr_apply(p.tr, acq_value(p.acq, mean, sd), linf[m]);
-  if (mu) mu[m] = mean;
-  if (sigma) sigma[m] = sd;
-}
-
-int launch_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const double* Xs, const int32_t* Zs, int M,
-                       const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf, const AcqFn* fn) {
-  if (M <= 0) return 0;
-  vzgp_handle* top = hs[E - 1];
-  VZ_TRY(top->pe_tmp.reserve(sizeof(double) * (2 * (size_t)E + 2) * (size_t)M));
-  double* t = top->pe_tmp.as<double>();
-  double* mu_e = t;
-  double* sd_e = t + (size_t)E * M;
-  double* linf_buf = linf ? linf : t + 2 * (size_t)E * M;
-  double* dummy = t + (2 * (size_t)E + 1) * M;
-  StackCombine p;
-  p.E = E; p.acq = acq_fn_of(acq, fn);
-  p.tr = trust_region_of(top, *acq, acq->tr_strict);   // measured against the trials of the top level (the current study)
-  const bool want_linf = tr_needs_distance(p.tr) || linf != nullptr;
-  const vzgp_acq none = posterior_request(acq->tr_dim_mask, acq->tr_rows);
-  for (int e = 0; e < E; ++e)
-    VZ_TRY(launch_score(hs[e], Xs, Zs, M, &none, dummy, mu_e + (size_t)e * M, sd_e + (size_t)e * M,
-                        (e == E - 1 && want_linf) ? linf_buf : nullptr));
-  for (int e = 0; e < 16; ++e) p.alpha[e] = e < E ? alphas[e] : 0.0;
-  k_stack_combine<<<(M + 255) / 256, 256, 0, top->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma);
-  VZ_CHECK_LAUNCH();
-  top->launches++;
-  return 0;
-}
-
-// ---------------------------------------------------------------------------
-// Stacked levels of uniform ensembles (VizierGPBandit(ensemble_size=E).set_priors: every level of the stack is trained
-// with the designer's spec, gp_bandit.py:402-447).  Per candidate, each level's prediction is the two-pass mixture of
-// its E members (pe_mixture), then the stack of k_stack_combine over the level mixtures: mean = sum of the level
-// means, s <- sd_l^alpha_l * s^(1 - alpha_l) bottom-up.  The acquisition and the non-strict trust region (distances to
-// the top level's trials) follow.  mu_e / sd_e: [L][E][M], level-major like the handles.
+// residuals of the stack below it, the last level on the current study.  Every level is a uniform ensemble of E
+// members (VizierGPBandit(ensemble_size=E).set_priors trains each level with the designer's spec,
+// gp_bandit.py:402-447; E = 1 is a single GP).  Per candidate, each level's prediction is the two-pass mixture of its
+// members (pe_mixture: with E = 1 exactly the member's mean and stddev), then mean = sum of the level means and the
+// stddevs are combined bottom-up by weighted geometric means  s <- sd_l^alpha_l * s^(1 - alpha_l)  (alpha_l from the
+// degrees of freedom of the two levels, computed by the caller).  The acquisition and the non-strict trust region
+// (distances to the TOP level's trials) follow.  mu_e / sd_e: [L][E][M], level-major like the handles.
 // ---------------------------------------------------------------------------
 struct StackEnsCombine {
   int L, E;
@@ -1085,32 +1023,24 @@ __global__ void __launch_bounds__(256) k_stack_ensemble_combine(int M, StackEnsC
   if (sigma) sigma[m] = sd;
 }
 
-// hs[l * E + e] = member e of level l.  Every member is scored by launch_score on its own route (mean and stddev);
-// top-level member 0 also gives the trust-region distance (the members of a level share its trials).  The pieces
-// live in the top handle's pe_tmp, which launch_score does not touch: [2 L E + 2][M] = mu | sd (L E rows each) |
-// linf | dummy.  Asynchronous, capturable.
+// hs[l * E + e] = member e of level l, all L E members one group of score_members in the top handle's pe_tmp;
+// top-level member 0 gives the trust-region distance (the members of a level share its trials).
 int launch_score_stack_ensemble(vzgp_handle* const* hs, int L, int E, const double* alphas, const double* Xs,
                                 const int32_t* Zs, int M, const vzgp_acq* acq, double* score, double* mu, double* sigma,
                                 double* linf, const AcqFn* fn) {
   if (M <= 0) return 0;
   const int n = L * E;
   vzgp_handle* top = hs[(L - 1) * E];
-  VZ_TRY(top->pe_tmp.reserve(sizeof(double) * (2 * (size_t)n + 2) * (size_t)M));
-  double* t = top->pe_tmp.as<double>();
-  double* mu_e = t;
-  double* sd_e = t + (size_t)n * M;
-  double* linf_buf = linf ? linf : t + 2 * (size_t)n * M;
-  double* dummy = t + (2 * (size_t)n + 1) * M;
   StackEnsCombine p;
   p.L = L; p.E = E; p.acq = acq_fn_of(acq, fn);
   p.tr = trust_region_of(top, *acq, acq->tr_strict);
-  const bool want_linf = tr_needs_distance(p.tr) || linf != nullptr;
-  const vzgp_acq none = posterior_request(acq->tr_dim_mask, acq->tr_rows);
-  for (int k = 0; k < n; ++k)
-    VZ_TRY(launch_score(hs[k], Xs, Zs, M, &none, dummy, mu_e + (size_t)k * M, sd_e + (size_t)k * M,
-                        (k == (L - 1) * E && want_linf) ? linf_buf : nullptr));
+  const vzgp_acq req = posterior_request(acq->tr_dim_mask, acq->tr_rows);
+  double *t, *linf_buf = linf;
+  VZ_TRY(score_members(top, &hs, 1, n, Xs, Zs, M, req, (L - 1) * E, req, tr_needs_distance(p.tr) || linf != nullptr,
+                       &t, &linf_buf));
   for (int l = 0; l < kMaxStackLevels; ++l) p.alpha[l] = l < L ? alphas[l] : 0.0;
-  k_stack_ensemble_combine<<<(M + 255) / 256, 256, 0, top->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma);
+  k_stack_ensemble_combine<<<(M + 255) / 256, 256, 0, top->stream>>>(M, p, t, t + (size_t)n * M, linf_buf, score, mu,
+                                                                     sigma);
   VZ_CHECK_LAUNCH();
   top->launches++;
   return 0;
@@ -1209,21 +1139,15 @@ int launch_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const
                           const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf, const AcqFn* fn) {
   if (M <= 0) return 0;
   vzgp_handle* h0 = hs[0];
-  VZ_TRY(h0->pe_tmp.reserve(sizeof(double) * (2 * (size_t)E + 2) * (size_t)M));
-  double* t = h0->pe_tmp.as<double>();
-  double* mu_e = t;
-  double* sd_e = t + (size_t)E * M;
-  double* linf_buf = linf ? linf : t + 2 * (size_t)E * M;
-  double* dummy = t + (2 * (size_t)E + 1) * M;
   EnsCombine p;
   p.E = E; p.acq = acq_fn_of(acq, fn);
   p.tr = trust_region_of(h0, *acq, acq->tr_strict);
-  const bool want_linf = tr_needs_distance(p.tr) || linf != nullptr;
-  const vzgp_acq none = posterior_request(acq->tr_dim_mask, acq->tr_rows);
-  for (int e = 0; e < E; ++e)   // all members share the trials: the distance is computed once
-    VZ_TRY(launch_score(hs[e], Xs, Zs, M, &none, dummy, mu_e + (size_t)e * M, sd_e + (size_t)e * M,
-                        (e == 0 && want_linf) ? linf_buf : nullptr));
-  k_ensemble_combine<<<(M + 255) / 256, 256, 0, h0->stream>>>(M, p, mu_e, sd_e, linf_buf, score, mu, sigma, h0->small.as<int>());
+  const vzgp_acq req = posterior_request(acq->tr_dim_mask, acq->tr_rows);
+  double *t, *linf_buf = linf;
+  // all members share the trials: member 0 gives the distance
+  VZ_TRY(score_members(h0, &hs, 1, E, Xs, Zs, M, req, 0, req, tr_needs_distance(p.tr) || linf != nullptr, &t, &linf_buf));
+  k_ensemble_combine<<<(M + 255) / 256, 256, 0, h0->stream>>>(M, p, t, t + (size_t)E * M, linf_buf, score, mu, sigma,
+                                                              h0->small.as<int>());
   VZ_CHECK_LAUNCH();
   h0->launches++;
   return 0;
@@ -1252,31 +1176,22 @@ __global__ void __launch_bounds__(256) k_pe_ensemble_combine(int M, PeEnsCombine
   if (sigma_all) sigma_all[m] = s_b;
 }
 
-// Every member is scored by launch_score (its own route): A members give mean and stddev, B members mean and stddev,
-// B member 0 also the trust-region distance (all B members share the trials).  The pieces live in hAs[0]->pe_tmp,
-// which launch_score does not touch: [4E + 2][M] = mu_a | sd_a | mu_b | sd_b (E rows each) | linf | dummy.
+// The A members, then the B members, as the two groups of score_members in hAs[0]->pe_tmp: [4E + 2][M] =
+// mu_a | sd_a | mu_b | sd_b (E rows each) | linf | dummy.  B member 0 gives the trust-region distance (all B members
+// share the trials).  E = 1 is the GP-UCB-PE of two single models (vzgp_score_pe).
 int launch_score_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const double* Xs,
                              const int32_t* Zs, int M, const vzgp_pe_params* pe, double* score, double* mu,
                              double* sigma, double* sigma_all) {
   if (M <= 0) return 0;
   vzgp_handle* h0 = hAs[0];
-  VZ_TRY(h0->pe_tmp.reserve(sizeof(double) * (4 * (size_t)E + 2) * (size_t)M));
-  double* t = h0->pe_tmp.as<double>();
-  double* mu_a = t;
-  double* sd_a = t + (size_t)E * M;
-  double* mu_b = t + 2 * (size_t)E * M;
-  double* sd_b = t + 3 * (size_t)E * M;
-  double* linf_b = t + 4 * (size_t)E * M;
-  double* dummy = t + (4 * (size_t)E + 1) * M;
   const PeEnsCombine p = pe_ensemble_args(hBs[0], E, pe);
   const vzgp_acq none = posterior_request(), accb = posterior_request(pe->tr_dim_mask, pe->tr_rows);
-  for (int e = 0; e < E; ++e)
-    VZ_TRY(launch_score(hAs[e], Xs, Zs, M, &none, dummy, mu_a + (size_t)e * M, sd_a + (size_t)e * M, nullptr));
-  for (int e = 0; e < E; ++e)
-    VZ_TRY(launch_score(hBs[e], Xs, Zs, M, e == 0 ? &accb : &none, dummy, mu_b + (size_t)e * M, sd_b + (size_t)e * M,
-                        (e == 0 && tr_needs_distance(p.tr)) ? linf_b : nullptr));
-  k_pe_ensemble_combine<<<(M + 255) / 256, 256, 0, h0->stream>>>(M, p, mu_a, sd_a, mu_b, sd_b, linf_b, score, mu,
-                                                                 sigma, sigma_all);
+  vzgp_handle* const* const groups[2] = {hAs, hBs};
+  double *t, *linf_b = nullptr;
+  VZ_TRY(score_members(h0, groups, 2, E, Xs, Zs, M, none, 0, accb, tr_needs_distance(p.tr), &t, &linf_b));
+  const size_t em = (size_t)E * M;
+  k_pe_ensemble_combine<<<(M + 255) / 256, 256, 0, h0->stream>>>(M, p, t, t + em, t + 2 * em, t + 3 * em, linf_b, score,
+                                                                 mu, sigma, sigma_all);
   VZ_CHECK_LAUNCH();
   h0->launches++;
   return 0;

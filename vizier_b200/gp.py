@@ -361,6 +361,26 @@ def _ptr(t: Optional[torch.Tensor]):
   return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def _eagle_run(dev, fn: str, args: tuple, cfg: '_lib.EagleConfig', req, count: int, seed: int, prior, prior_z,
+               cat_sizes, _keep):
+  """One `vzgp_eagle_run*` call: `args` are the entry point's model arguments (handles, counts, alphas) and `req` its
+  request, passed around the config; the prior trials go to `dev`'s device.  `_keep` (what `req` points into) is held
+  until the call returns.  Returns (best_x [count,Dc], best_z [count,Dk], best_score [count])."""
+  n_prior = 0 if prior is None else len(prior)
+  pt = dev._dev(prior, torch.float64) if n_prior > 0 and dev.dc > 0 else None
+  pz = dev._dev(prior_z, torch.int32) if n_prior > 0 and dev.dk > 0 else None
+  bx = np.zeros((count, dev.dc), np.float64)
+  bz = np.zeros((count, dev.dk), np.int32)
+  bs = np.zeros(count, np.float64)
+  sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
+  _lib.check(fn, getattr(dev._lib, fn)(
+      *args, C.byref(cfg), req, _ptr(pt), _ptr(pz), n_prior,
+      sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None, count, seed,
+      bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
+      bs.ctypes.data_as(C.POINTER(C.c_double))))
+  return bx, bz, bs
+
+
 class DeviceGP:
   """One libvzgp handle = one study's GP on one GPU."""
 
@@ -909,44 +929,16 @@ class DeviceGP:
     UcbPeAcquisition the GP-UCB-PE acquisition is optimised (vzgp_eagle_run_pe), with a UcbPeMultiAcquisition its
     multi-metric form (vzgp_eagle_run_pe_multi)."""
     if isinstance(acq, (UcbPeAcquisition, UcbPeMultiAcquisition)):
-      return self._eagle_run_pe(cfg, acq, count, seed, prior, prior_z, cat_sizes, other)
-    multi = isinstance(acq, ScalarizedUcbAcquisition)
-    if not multi:
+      fn = 'vzgp_eagle_run_pe_multi' if isinstance(acq, UcbPeMultiAcquisition) else 'vzgp_eagle_run_pe'
+      args = (self._h, other._h)
+    elif isinstance(acq, ScalarizedUcbAcquisition):
+      fn, args = 'vzgp_eagle_run_multi', (self._h,)
+    else:
       self._use_acq(acq)
+      fn, args = 'vzgp_eagle_run', (self._h,)
     a, keep = acq._c()
-    n_prior = 0 if prior is None else len(prior)
-    pt = self._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
-    pz = self._dev(prior_z, torch.int32) if n_prior > 0 and self.dk > 0 else None
-    bx = np.zeros((count, self.dc), np.float64)
-    bz = np.zeros((count, self.dk), np.int32)
-    bs = np.zeros(count, np.float64)
-    sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
-    fn_name = 'vzgp_eagle_run_multi' if multi else 'vzgp_eagle_run'
-    _lib.check(fn_name, getattr(self._lib, fn_name)(
-        self._h, C.byref(cfg), C.byref(a), _ptr(pt), _ptr(pz), n_prior,
-        sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None, count, seed,
-        bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
-        bs.ctypes.data_as(C.POINTER(C.c_double))))
-    del keep
-    return bx, bz, bs
+    return _eagle_run(self, fn, args, cfg, C.byref(a), count, seed, prior, prior_z, cat_sizes, keep)
 
-  def _eagle_run_pe(self, cfg, pe, count, seed, prior, prior_z, cat_sizes, other):
-    fn_name = 'vzgp_eagle_run_pe_multi' if isinstance(pe, UcbPeMultiAcquisition) else 'vzgp_eagle_run_pe'
-    p, keep = pe._c()
-    n_prior = 0 if prior is None else len(prior)
-    pt = self._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
-    pz = self._dev(prior_z, torch.int32) if n_prior > 0 and self.dk > 0 else None
-    bx = np.zeros((count, self.dc), np.float64)
-    bz = np.zeros((count, self.dk), np.int32)
-    bs = np.zeros(count, np.float64)
-    sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
-    _lib.check(fn_name, getattr(self._lib, fn_name)(
-        self._h, other._h, C.byref(cfg), C.byref(p), _ptr(pt), _ptr(pz), n_prior,
-        sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None, count, seed,
-        bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
-        bs.ctypes.data_as(C.POINTER(C.c_double))))
-    del keep
-    return bx, bz, bs
 
 def transfer_dof(n: int, num_hyperparameters: int) -> float:
   """gp/transfer_learning.py:38-59 (_compute_dof)."""
@@ -960,7 +952,78 @@ def transfer_alpha(n_top: int, n_base: int, num_hyperparameters: int, expected_b
   return beta2 / (1.0 + beta2)
 
 
-class StackedGP:
+class _MultiHandle:
+  """A model of several libvzgp handles on ONE stream (`EnsembleGP`, `StackedGP`, `SeparableGP`).  The calls that take
+  one handle go to the lead handle `_lead()`, which also carries the state of the host-stepped Eagle loop
+  (`SteppedEagle` drives `_h`, `_lib`, `_stream` and `_dev`)."""
+
+  def _devices(self) -> list:
+    """Every handle's DeviceGP, in the order of the library's handle arrays."""
+    return self.members
+
+  def _lead(self) -> 'DeviceGP':
+    return self._devices()[0]
+
+  def _handles(self):
+    hs = [d._h for d in self._devices()]
+    return (C.c_void_p * len(hs))(*hs)
+
+  @property
+  def _h(self):
+    return self._lead()._h
+
+  @property
+  def _lib(self):
+    return self._lead()._lib
+
+  @property
+  def _stream(self):
+    return self._lead()._stream
+
+  @property
+  def stream(self):
+    return self._lead().stream
+
+  def _dev(self, a, dtype):
+    return self._lead()._dev(a, dtype)
+
+  @property
+  def launch_count(self) -> int:
+    return sum(d.launch_count for d in self._devices())
+
+  def synchronize(self):
+    self._lead().synchronize()
+
+  def close(self):
+    for d in self._devices():
+      d.close()
+
+  def random_pool(self, m: int, dc: int, seed: int, index_base: int = 0) -> torch.Tensor:
+    return self._lead().random_pool(m, dc, seed, index_base)
+
+  def random_pool_cat(self, m: int, cat_sizes, seed: int, index_base: int = 0) -> torch.Tensor:
+    return self._lead().random_pool_cat(m, cat_sizes, seed, index_base)
+
+  def topk(self, score: torch.Tensor, count: int):
+    return self._lead().topk(score, count)
+
+
+def _random_search_by_scoring(model, m: int, acq: 'Acquisition', count: int, seed: int, index_base: int = 0,
+                              cat_sizes=None):
+  """RandomVectorizedStrategy over a multi-handle model: Philox pool -> the model's score -> device top-k.  Returns
+  (best_x [count,Dc], best_z [count,Dk], best_score [count], best_index [count])."""
+  dev = model.device
+  xs = model.random_pool(m, model.dc, seed, index_base) if model.dc else torch.zeros((m, 0), dtype=torch.float64, device=dev)
+  zs = model.random_pool_cat(m, cat_sizes, seed, index_base) if model.dk else None
+  out = model.score(xs, acq, zs=zs)
+  idx, val = model.topk(out['score'], count)
+  it = torch.from_numpy(np.maximum(idx, 0)).to(dev)
+  bx = xs[it].cpu().numpy()
+  bz = zs[it].cpu().numpy() if zs is not None else np.zeros((count, 0), np.int32)
+  return bx, bz, val, idx + index_base
+
+
+class StackedGP(_MultiHandle):
   """Stack of residual GPs for transfer learning (`VizierGPBandit.set_priors`, gp_bandit.py:289-318; StackedResidualGP,
   gp/gp_models.py:91-140, :245-300): level 0 is fitted on the first prior study, each further level on the residuals
   of the next study against the stack below it, the last level on the current study.  The levels are libvzgp handles
@@ -1002,40 +1065,15 @@ class StackedGP:
   def n_metrics(self) -> int:
     return self._kind(self.levels[0])[1] if self.levels else 1
 
+  def _devices(self) -> list:
+    return [m for level in self.levels for m in self._members(level)]   # level-major: hs[l * E + e]
+
   def _lead(self) -> 'DeviceGP':
     """The top level's (first) handle: it owns the Eagle state and the scratch of the combine."""
     return self._members(self.levels[-1])[0]
 
-  # the lead handle carries the state of the host-stepped Eagle loop (SteppedEagle drives these)
-  @property
-  def _h(self):
-    return self._lead()._h
-
-  @property
-  def _lib(self):
-    return self._lead()._lib
-
-  @property
-  def _stream(self):
-    return self._lead()._stream
-
-  def _dev(self, a, dtype):
-    return self._lead()._dev(a, dtype)
-
-  @property
-  def stream(self):
-    return self.levels[0].stream
-
-  @property
-  def launch_count(self) -> int:
-    return sum(m.launch_count for m in self.levels)
-
-  def synchronize(self):
-    self.levels[0].synchronize()
-
   def close(self):
-    for m in self.levels:
-      m.close()
+    super().close()
     self.levels = []
 
   def truncate(self, n_levels: int) -> None:
@@ -1087,10 +1125,6 @@ class StackedGP:
     self.counts.append(int(n_points))
     self.device, self.dc, self.dk, self.n = level.device, level.dc, level.dk, level.n
 
-  def _handles(self):
-    hs = [m._h for level in self.levels for m in self._members(level)]   # level-major: hs[l * E + e]
-    return (C.c_void_p * len(hs))(*hs)
-
   def _alphas(self):
     return (C.c_double * len(self.levels))(*self.alphas)
 
@@ -1138,53 +1172,19 @@ class StackedGP:
     """The device Eagle loop on the stacked acquisition: `Acquisition` (single-metric levels) or
     `ScalarizedUcbAcquisition` (multi-metric levels)."""
     assert other is None
-    f = self._lead()
     if isinstance(acq, ScalarizedUcbAcquisition):
-      a, keep = acq._c()
-      fn, args = 'vzgp_eagle_run_stack_multi', (self._handles(), len(self.levels), self._alphas(), C.byref(cfg),
-                                                C.byref(a))
+      fn, args = 'vzgp_eagle_run_stack_multi', (self._handles(), len(self.levels), self._alphas())
     else:
       self._members(self.levels[0])[0]._use_acq(acq)
-      a, keep = acq._c()
       if self.ensemble_size == 1:
-        fn, args = 'vzgp_eagle_run_stack', (self._handles(), len(self.levels), self._alphas(), C.byref(cfg), C.byref(a))
+        fn, args = 'vzgp_eagle_run_stack', (self._handles(), len(self.levels), self._alphas())
       else:
         fn, args = 'vzgp_eagle_run_stack_ensemble', (self._handles(), len(self.levels), self.ensemble_size,
-                                                     self._alphas(), C.byref(cfg), C.byref(a))
-    n_prior = 0 if prior is None else len(prior)
-    pt = f._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
-    pz = f._dev(prior_z, torch.int32) if n_prior > 0 and self.dk > 0 else None
-    bx = np.zeros((count, self.dc), np.float64)
-    bz = np.zeros((count, self.dk), np.int32)
-    bs = np.zeros(count, np.float64)
-    sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
-    _lib.check(fn, getattr(f._lib, fn)(
-        *args, _ptr(pt), _ptr(pz), n_prior, sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None,
-        count, seed, bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
-        bs.ctypes.data_as(C.POINTER(C.c_double))))
-    del keep
-    return bx, bz, bs
+                                                     self._alphas())
+    a, keep = acq._c()
+    return _eagle_run(self, fn, args, cfg, C.byref(a), count, seed, prior, prior_z, cat_sizes, keep)
 
-  def random_search(self, m: int, acq: Acquisition, count: int, seed: int, index_base: int = 0, cat_sizes=None):
-    """RandomVectorizedStrategy over the stack: Philox pool -> combined score -> device top-k."""
-    f = self._lead()
-    xs = f.random_pool(m, self.dc, seed, index_base) if self.dc else torch.zeros((m, 0), dtype=torch.float64, device=f.device)
-    zs = f.random_pool_cat(m, cat_sizes, seed, index_base) if self.dk else None
-    out = self.score(xs, acq, zs=zs)
-    idx, val = f.topk(out['score'], count)
-    it = torch.from_numpy(np.maximum(idx, 0)).to(f.device)
-    bx = xs[it].cpu().numpy()
-    bz = zs[it].cpu().numpy() if zs is not None else np.zeros((count, 0), np.int32)
-    return bx, bz, val, idx + index_base
-
-  def random_pool(self, m: int, dc: int, seed: int, index_base: int = 0) -> torch.Tensor:
-    return self._lead().random_pool(m, dc, seed, index_base)
-
-  def random_pool_cat(self, m: int, cat_sizes, seed: int, index_base: int = 0) -> torch.Tensor:
-    return self._lead().random_pool_cat(m, cat_sizes, seed, index_base)
-
-  def topk(self, score, count: int):
-    return self._lead().topk(score, count)
+  random_search = _random_search_by_scoring
 
 
 class _DevView:
@@ -1249,7 +1249,7 @@ class SteppedEagle:
     return bx, bz, bs
 
 
-class EnsembleGP:
+class EnsembleGP(_MultiHandle):
   """Uniform ensemble of E GPs fitted on the same trials with different hyper-parameters
   (`VizierGPBandit(ensemble_size=E)`: the E best ARD restarts, gp_models.py:200-223; predictive =
   UniformEnsemblePredictive, stochastic_process_model.py:836-868).  The members are E libvzgp handles on
@@ -1263,39 +1263,7 @@ class EnsembleGP:
     first = DeviceGP(device, stream=stream)
     self.members = [first] + [DeviceGP(device, stream=first.stream) for _ in range(size - 1)]
     self.device = first.device
-    self._lib = first._lib
     self.n = self.dc = self.dk = 0
-
-  @property
-  def stream(self):
-    return self.members[0].stream
-
-  # member 0 carries the state of the host-stepped Eagle loop (SteppedEagle drives these)
-  @property
-  def _h(self):
-    return self.members[0]._h
-
-  @property
-  def _stream(self):
-    return self.members[0]._stream
-
-  def _dev(self, a, dtype):
-    return self.members[0]._dev(a, dtype)
-
-  def close(self):
-    for m in self.members:
-      m.close()
-
-  @property
-  def launch_count(self) -> int:
-    return sum(m.launch_count for m in self.members)
-
-  def synchronize(self):
-    self.members[0].synchronize()
-
-  def _handles(self):
-    arr = (C.c_void_p * len(self.members))(*[m._h for m in self.members])
-    return arr
 
   def fit(self, x, y, params: Sequence[GPHyperParams], z=None, n_valid=None) -> int:
     assert len(params) == len(self.members)
@@ -1353,48 +1321,23 @@ class EnsembleGP:
                 other=None):
     """`DeviceGP.eagle_run` on the mixture; with `other` (an EnsembleGP) and a UcbPeAcquisition the GP-UCB-PE
     acquisition of the two mixtures is optimised (vzgp_eagle_run_pe_ensemble)."""
-    f = self.members[0]
     if isinstance(acq, UcbPeAcquisition):
-      p, keep = acq._c()
-      ha, hb = self._pe_handles(other)
-      fn, args = 'vzgp_eagle_run_pe_ensemble', (ha, hb, len(self.members), C.byref(cfg), C.byref(p))
+      fn, args = 'vzgp_eagle_run_pe_ensemble', (*self._pe_handles(other), len(self.members))
     else:
       assert other is None
-      f._use_acq(acq)
-      a, keep = acq._c()
-      fn, args = 'vzgp_eagle_run_ensemble', (self._handles(), len(self.members), C.byref(cfg), C.byref(a))
-    n_prior = 0 if prior is None else len(prior)
-    pt = f._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
-    pz = f._dev(prior_z, torch.int32) if n_prior > 0 and self.dk > 0 else None
-    bx = np.zeros((count, self.dc), np.float64)
-    bz = np.zeros((count, self.dk), np.int32)
-    bs = np.zeros(count, np.float64)
-    sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
-    _lib.check(fn, getattr(self._lib, fn)(
-        *args, _ptr(pt), _ptr(pz), n_prior, sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None,
-        count, seed, bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
-        bs.ctypes.data_as(C.POINTER(C.c_double))))
-    del keep
-    return bx, bz, bs
+      self.members[0]._use_acq(acq)
+      fn, args = 'vzgp_eagle_run_ensemble', (self._handles(), len(self.members))
+    a, keep = acq._c()
+    return _eagle_run(self, fn, args, cfg, C.byref(a), count, seed, prior, prior_z, cat_sizes, keep)
 
-  def random_search(self, m: int, acq: Acquisition, count: int, seed: int, index_base: int = 0, cat_sizes=None):
-    """RandomVectorizedStrategy over the ensemble: Philox pool -> mixture score -> device top-k."""
-    f = self.members[0]
-    xs = f.random_pool(m, self.dc, seed, index_base) if self.dc else torch.zeros((m, 0), dtype=torch.float64, device=self.device)
-    zs = f.random_pool_cat(m, cat_sizes, seed, index_base) if self.dk else None
-    out = self.score(xs, acq, zs=zs)
-    idx, val = f.topk(out['score'], count)
-    it = torch.from_numpy(np.maximum(idx, 0)).to(self.device)
-    bx = xs[it].cpu().numpy()
-    bz = zs[it].cpu().numpy() if zs is not None else np.zeros((count, 0), np.int32)
-    return bx, bz, val, idx + index_base
+  random_search = _random_search_by_scoring
 
   def posterior(self, xs, zs=None, add_noise: bool = True):
     """Per-member joint posteriors [(mean [M], cov [M, M])] (the mixture components)."""
     return [m.posterior(xs, zs, add_noise) for m in self.members]
 
 
-class SeparableGP:
+class SeparableGP(_MultiHandle):
   """Separable multi-task GP (`VizierGPBandit(multitask_type=SEPARABLE_*)`; tuned_gp_models.py:282-305): the prior
   covariance of the labels is K_s (x) T + sn2 I.  Diagonalising T = Q diag(lambda) Q^T splits it into M single-metric
   GPs (eigen-tasks) with signal variances s^2 lambda_j and labels Y Q[:, j]; `members` holds one libvzgp handle per
@@ -1406,28 +1349,9 @@ class SeparableGP:
     first = DeviceGP(device)
     self.members = [first] + [DeviceGP(device, stream=first.stream) for _ in range(n_metrics - 1)]
     self.device = first.device
-    self._lib = first._lib
     self.n_metrics = n_metrics
     self.n = self.dc = self.dk = 0
     self.cholesky_failed = False
-
-  @property
-  def stream(self):
-    return self.members[0].stream
-
-  @property
-  def launch_count(self) -> int:
-    return sum(m.launch_count for m in self.members)
-
-  def synchronize(self):
-    self.members[0].synchronize()
-
-  def close(self):
-    for m in self.members:
-      m.close()
-
-  def _handles(self):
-    return (C.c_void_p * len(self.members))(*[m._h for m in self.members])
 
   def fit(self, x, y, params: GPHyperParams, z=None, n_valid=None) -> int:
     """y [N, M]; params carries the task parameters (params.multitask_type).  Returns the shared Cholesky retries."""
@@ -1472,31 +1396,9 @@ class SeparableGP:
   def eagle_run(self, cfg, acq: ScalarizedUcbAcquisition, count: int, seed: int, prior=None, prior_z=None,
                 cat_sizes=None, other=None):
     assert other is None and isinstance(acq, ScalarizedUcbAcquisition)
-    f = self.members[0]
     sc, keep = acq._c()
-    n_prior = 0 if prior is None else len(prior)
-    pt = f._dev(prior, torch.float64) if n_prior > 0 and self.dc > 0 else None
-    pz = f._dev(prior_z, torch.int32) if n_prior > 0 and self.dk > 0 else None
-    bx = np.zeros((count, self.dc), np.float64)
-    bz = np.zeros((count, self.dk), np.int32)
-    bs = np.zeros(count, np.float64)
-    sizes = np.ascontiguousarray(np.asarray(cat_sizes if cat_sizes is not None else [], np.int32))
-    _lib.check('vzgp_eagle_run_separable', self._lib.vzgp_eagle_run_separable(
-        self._handles(), self.n_metrics, C.byref(cfg), C.byref(sc), _ptr(pt), _ptr(pz), n_prior,
-        sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes.size else None, count, seed,
-        bx.ctypes.data_as(C.POINTER(C.c_double)), bz.ctypes.data_as(C.POINTER(C.c_int32)),
-        bs.ctypes.data_as(C.POINTER(C.c_double))))
-    del keep
-    return bx, bz, bs
-
-  def random_pool(self, m: int, dc: int, seed: int, index_base: int = 0) -> torch.Tensor:
-    return self.members[0].random_pool(m, dc, seed, index_base)
-
-  def random_pool_cat(self, m: int, cat_sizes, seed: int, index_base: int = 0) -> torch.Tensor:
-    return self.members[0].random_pool_cat(m, cat_sizes, seed, index_base)
-
-  def topk(self, score: torch.Tensor, count: int):
-    return self.members[0].topk(score, count)
+    return _eagle_run(self, 'vzgp_eagle_run_separable', (self._handles(), self.n_metrics), cfg, C.byref(sc), count,
+                      seed, prior, prior_z, cat_sizes, keep)
 
   def posterior(self, xs, zs=None, add_noise: bool = True):
     """Joint posterior over the n points and M metrics: mean [M, n] and covariance [M n, M n] in metric-major blocks
