@@ -423,6 +423,25 @@ int vzgp_score_topk(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, 
 int vzgp_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int M,
                         const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf);
 
+/* The acquisition of vzgp_score and its gradient with respect to the candidates' continuous features, for
+ * gradient-based acquisition optimisers (L-BFGS-B, lbfgsb_optimizer.py).  Xs [M x Dc] device; score [M] and
+ * grad [M x Dc] row-major device (required); mu, sigma, linf [M] device, optional.  Asynchronous on the handle's
+ * stream.  The handle's acquisition function (vzgp_set_acquisition) is applied to (mu, sigma), then the trust
+ * region; a point outside the region scores -1e4 - linf and its gradient is -d linf / dx (one coordinate: the
+ * nearest trial, lowest index on ties, and its first coordinate attaining the maximum, lowest index on ties; 0 at
+ * linf = 0).  A clamped variance (counted as in vzgp_score) contributes no stddev gradient.  No limit on the trial
+ * count beyond the fit's.  VZGP_ERR_ARG for models with categorical features, VZGP_ERR_STATE before a fit. */
+int vzgp_score_grad(vzgp_handle* h, const double* Xs, int M, const vzgp_acq* acq, double* score, double* grad,
+                    double* mu, double* sigma, double* linf);
+
+/* The same for a uniform ensemble of E <= 16 members (fitted on the same valid trials, possibly padded to different
+ * sizes, as for vzgp_score_ensemble; one device and stream), scored as
+ * the two-pass mixture  mean = avg mu_e,  var = avg sigma_e^2 + avg (mu_e - mean)^2  with the acquisition function
+ * of hs[0].  Its gradient is that of the same formula; the value agrees with vzgp_score_ensemble (one-pass variance)
+ * to round-off. */
+int vzgp_score_grad_ensemble(vzgp_handle* const* hs, int E, const double* Xs, int M, const vzgp_acq* acq,
+                             double* score, double* grad, double* mu, double* sigma, double* linf);
+
 /* Candidate-pool shards over several GPUs (SURVEY 8e; the reference is single-process, its
  * counterpart is the arg-partition over ONE pool, vectorized_base.py:575-587).
  * vzgp_score_topk_pack: score this rank's shard, select its top `count` and write them to the DEVICE

@@ -223,6 +223,8 @@ SIGNATURES = {
     'vzgp_topk': (_i, [_vp, _vp, _i64, _i, _pi64, _pd]),
     'vzgp_score_topk': (_i, [_vp, _vp, _vp, _i, _pA, _i, _vp, _pd, _pd, _pi64]),
     'vzgp_score_ensemble': (_i, [C.POINTER(_vp), _i, _vp, _vp, _i, _pA, _vp, _vp, _vp, _vp]),
+    'vzgp_score_grad': (_i, [_vp, _vp, _i, _pA, _vp, _vp, _vp, _vp, _vp]),
+    'vzgp_score_grad_ensemble': (_i, [C.POINTER(_vp), _i, _vp, _i, _pA, _vp, _vp, _vp, _vp, _vp]),
     'vzgp_eagle_run_ensemble': (_i, [C.POINTER(_vp), _i, C.POINTER(EagleConfig), _pA, _vp, _vp, _i, _pi32, _i, C.c_uint64, _pd, _pi32, _pd]),
     'vzgp_score_topk_pack': (_i, [_vp, _vp, _vp, _i, _pA, _i, _i64, _vp, _vp]),
     'vzgp_merge_topk': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),

@@ -105,11 +105,12 @@ def _lean_lbfgsb(fun, x0: np.ndarray, bounds, **kw):
     return done.value
 
 
-def _lockstep(batch_fn, inits, bounds, **kw):
+def _lockstep(batch_fn, inits, bounds, stop_nonfinite: bool = False, **kw):
   """All restarts at once: every round collects the point each unfinished restart asks for and evaluates
   them with ONE call of `batch_fn(indices, points) -> (losses, grads)` (one CUDA graph launch for all
   restarts, gp.DeviceGP.make_batch_loss_fn).  Each restart's sequence of iterates is exactly the one it
-  would have had alone."""
+  would have had alone.  With stop_nonfinite, a restart sent a non-finite loss or gradient ends at that point
+  with that loss."""
   gens = [_lean_lbfgsb_steps(np.asarray(t0, np.float64), bounds, **kw) for t0 in inits]
   pending, results = {}, {}
   for i, gen in enumerate(gens):
@@ -121,6 +122,10 @@ def _lockstep(batch_fn, inits, bounds, **kw):
     idx = sorted(pending)
     losses, grads = batch_fn(idx, [pending[i] for i in idx])
     for k, i in enumerate(idx):
+      if stop_nonfinite and not (np.isfinite(losses[k]) and np.all(np.isfinite(grads[k]))):
+        results[i] = (np.array(pending[i], np.float64), float(losses[k]))
+        del pending[i]
+        continue
       try:
         pending[i] = gens[i].send((losses[k], grads[k]))
       except StopIteration as done:

@@ -1490,6 +1490,32 @@ int vzgp_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const i
   return launch_score_ensemble(hs, E, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(hs[0]));
 }
 
+// Continuous features only: the gradient is taken in them and the reference's L-BFGS-B optimiser rejects the rest.
+static int check_score_grad(vzgp_handle* const* hs, int E, const double* Xs, int M, const vzgp_acq* acq, double* score,
+                           double* grad) {
+  VZ_ARG(acq != nullptr, "acq");
+  VZ_TRY(check_pool(hs[0], Xs, nullptr, M, score));
+  VZ_ARG(hs[0]->dk == 0, "the gradient needs continuous features only (Dk = 0)");
+  VZ_ARG(M == 0 || grad != nullptr || hs[0]->dc == 0, "grad");
+  return 0;
+}
+
+int vzgp_score_grad(vzgp_handle* h, const double* Xs, int M, const vzgp_acq* acq, double* score, double* grad,
+                    double* mu, double* sigma, double* linf) {
+  VZ_TRY(check_handles(&h, 1, 1, Trials::kAny));
+  VZ_TRY(check_score_grad(&h, 1, Xs, M, acq, score, grad));
+  Guard g(h->device);
+  return launch_score_grad(&h, 1, Xs, M, acq, handle_acq(h), score, grad, mu, sigma, linf);
+}
+
+int vzgp_score_grad_ensemble(vzgp_handle* const* hs, int E, const double* Xs, int M, const vzgp_acq* acq,
+                             double* score, double* grad, double* mu, double* sigma, double* linf) {
+  VZ_TRY(check_ensemble(hs, E));
+  VZ_TRY(check_score_grad(hs, E, Xs, M, acq, score, grad));
+  Guard g(hs[0]->device);
+  return launch_score_grad(hs, E, Xs, M, acq, handle_acq(hs[0]), score, grad, mu, sigma, linf);
+}
+
 int vzgp_eagle_run_ensemble(vzgp_handle* const* hs, int E, const vzgp_eagle_config* cfg, const vzgp_acq* acq,
                             const double* prior, const int32_t* prior_z, int n_prior, const int32_t* cat_sizes,
                             int count, uint64_t seed, double* best_x, int32_t* best_z, double* best_score) {

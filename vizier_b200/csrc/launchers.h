@@ -169,6 +169,10 @@ int launch_gather_rows(vzgp_handle* h, const double* X, int dc, const long long*
 
 int launch_nll_grad_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int n_valid,
                           const KernelParams& kp, double sn2, double jitter0, int max_iters, double* out);
+// The acquisition and its gradient in the continuous features (score_grad.cu): hs[0..E), E = 1 for one model, scored
+// as the two-pass mixture; continuous features only.  grad is [M x Dc].
+int launch_score_grad(vzgp_handle* const* hs, int E, const double* Xs, int M, const vzgp_acq* acq, const AcqFn* fn,
+                      double* score, double* grad, double* mu, double* sigma, double* linf);
 int launch_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int M,
                           const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf,
                           const AcqFn* fn = nullptr);

@@ -25,6 +25,12 @@ uniform mixture of its E best restarts (`vzgp_score_stack_ensemble`), `linear_co
 multi-metric problem stacks independent multi-task levels on [N, M] residuals, scored by the scalarised UCB
 (`vzgp_score_stack_multi`).  Separable multi-task types and parallel scoring functions with priors raise
 NotImplementedError.
+`acquisition_optimizer_factory=optimizers.LBFGSBOptimizerFactory()` optimises the acquisition with L-BFGS-B
+(lbfgsb_optimizer.py) instead of Eagle: single-metric studies with continuous parameters (categorical ones raise
+ValueError at construction), single models, ensembles and `linear_coef`, every lowered acquisition, with or without
+the trust region.  The acquisition and its gradient come from `vzgp_score_grad` (csrc/score_grad.cu), one batched
+call per round of the lock-stepped restarts.  With multi-metric studies, parallel scoring functions or `set_priors`
+it raises NotImplementedError.
 `scoring_function_factory` (e.g. `acquisitions.bayesian_scoring_function_factory(lambda d: EI(get_best_labels(d.labels)))`
 or `AcquisitionTrustRegion.default_ucb_pi`) selects UCB, LCB, EI, PI or a thresholded pair of those; the device
 scoring kernels evaluate it (`acquisitions.lower_acquisition`).  Multi-metric problems keep their scalarised UCB.
@@ -162,7 +168,14 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     self._output_warper = output_warper or output_warpers.create_default_warper()
     self._rng = np.random.default_rng(_seed_from(rng))
     self._converter = converters.TrialToModelInputConverter.from_problem(problem)
-    self._acquisition_optimizer = acquisition_optimizer_factory(self._converter)
+    self._lbfgsb = isinstance(acquisition_optimizer_factory, vb.LBFGSBOptimizerFactory)
+    if self._lbfgsb and self._n_metrics > 1:
+      raise NotImplementedError('the L-BFGS-B acquisition optimiser with multi-metric studies (the gradient of the '
+                                'scalarised UCB) is not implemented.')
+    if self._lbfgsb and self._parallel:
+      raise NotImplementedError('the L-BFGS-B acquisition optimiser with parallel (q-) scoring functions is not '
+                                'implemented.')
+    self._acquisition_optimizer = acquisition_optimizer_factory(self._converter)   # L-BFGS-B: ValueError if categorical
     if self._scoring_function_factory is not None:
       empty = acq_lib.ModelData(features=None, labels=acq_lib.PaddedArray.as_padded(np.zeros((0, self._n_metrics))))
       acq_lib.check_supported(self._scoring_function(empty).acquisition_fn, parallel=self._parallel)
@@ -196,6 +209,8 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     retrains the prior stack from scratch on what it is given."""
     if self._parallel:
       raise NotImplementedError('transfer-learning priors with parallel (q-) scoring functions are not implemented.')
+    if self._lbfgsb:
+      raise NotImplementedError('transfer-learning priors with the L-BFGS-B acquisition optimiser are not implemented.')
     if self._multitask_type:
       raise NotImplementedError(f'transfer-learning priors with the separable multi-task type {self._multitask_type} '
                                 'are not implemented.')

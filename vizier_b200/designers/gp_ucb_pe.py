@@ -164,6 +164,8 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
                metadata_ns: str = 'google_gp_ucb_pe_bandit', device: int = 0):
     if problem.search_space.is_conditional:
       raise ValueError(f'{type(self)} does not support conditional search.')
+    if isinstance(acquisition_optimizer_factory, vb.LBFGSBOptimizerFactory):
+      raise NotImplementedError('GP-UCB-PE with the L-BFGS-B acquisition optimiser is not implemented.')
     self._n_metrics = len(problem.metric_information)
     if self._n_metrics > 1:
       # gp_ucb_pe.py:701-722

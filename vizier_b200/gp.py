@@ -381,6 +381,29 @@ def _eagle_run(dev, fn: str, args: tuple, cfg: '_lib.EagleConfig', req, count: i
   return bx, bz, bs
 
 
+def _score_grad(lead: 'DeviceGP', members: Sequence['DeviceGP'], xs, acq: 'Acquisition', with_aux: bool) -> dict:
+  xst = lead._dev(xs, torch.float64)
+  m, dc = xst.shape[0], xst.shape[1]
+  flat = torch.empty((m * (1 + dc),), dtype=torch.float64, device=lead.device)   # one copy brings both back
+  res = {'score': flat[:m], 'grad': flat[m:].view(m, dc), '_flat': flat}
+  if with_aux:
+    for k in ('mean', 'stddev', 'linf_distance'):
+      res[k] = torch.empty((m,), dtype=torch.float64, device=lead.device)
+  lead._stream.wait_stream(torch.cuda.current_stream(lead.device))
+  lead._use_acq(acq)                      # multi-handle calls take the acquisition of hs[0]
+  a, keep = acq._c()
+  outs = (_ptr(res['score']), _ptr(res['grad']), _ptr(res.get('mean')), _ptr(res.get('stddev')),
+          _ptr(res.get('linf_distance')))
+  if len(members) == 1:
+    _lib.check('vzgp_score_grad', lead._lib.vzgp_score_grad(lead._h, _ptr(xst), m, C.byref(a), *outs))
+  else:
+    hs = (C.c_void_p * len(members))(*[d._h for d in members])
+    _lib.check('vzgp_score_grad_ensemble', lead._lib.vzgp_score_grad_ensemble(hs, len(members), _ptr(xst), m,
+                                                                               C.byref(a), *outs))
+  res['_inputs'] = (xst, keep)
+  return res
+
+
 class DeviceGP:
   """One libvzgp handle = one study's GP on one GPU."""
 
@@ -696,6 +719,12 @@ class DeviceGP:
         _ptr(res.get('stddev')), _ptr(res.get('linf_distance'))))
     res['_inputs'] = (xst, zst, keep)  # keep alive until the caller synchronises
     return res
+
+  def score_grad(self, xs, acq: Acquisition, with_aux: bool = False) -> dict:
+    """The acquisition of `score` and its gradient in the continuous features (`vzgp_score_grad`; continuous models
+    only).  Asynchronous on self.stream; returns device tensors {'score' [M], 'grad' [M, Dc],
+    ['mean', 'stddev', 'linf_distance' [M]]}."""
+    return _score_grad(self, [self], xs, acq, with_aux)
 
   def score_multi(self, xs, acq: ScalarizedUcbAcquisition, zs=None, with_aux: bool = False) -> dict:
     """Multi-metric scalarised UCB; returns device tensors {'score' [M], ['mean' [n_metrics, M], 'stddev' [M]]}."""
@@ -1289,6 +1318,10 @@ class EnsembleGP(_MultiHandle):
         _ptr(res.get('mean')), _ptr(res.get('stddev')), _ptr(res.get('linf_distance'))))
     res['_inputs'] = (xst, zst, keep)
     return res
+
+  def score_grad(self, xs, acq: Acquisition, with_aux: bool = False) -> dict:
+    """`DeviceGP.score_grad` of the two-pass mixture of the members (`vzgp_score_grad_ensemble`)."""
+    return _score_grad(self.members[0], self.members, xs, acq, with_aux)
 
   def score_qsets(self, xs_sets, q: int, qacq: QAcquisition, seed: int, zs=None, period: int = 0,
                   with_aux: bool = False, with_cov: bool = False) -> dict:

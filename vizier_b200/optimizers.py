@@ -5,9 +5,12 @@ Mirrors
     (vizier/_src/algorithms/optimizers/vectorized_base.py:668-710, :278-542, :125-131),
   * `EagleStrategyConfig` / `VectorizedEagleStrategyFactory`
     (vizier/_src/algorithms/optimizers/eagle_strategy.py:111-167, :325-407),
-  * `random_strategy_factory` (random_vectorized_optimizer.py:114-123).
-Calling the optimiser runs the whole ask-evaluate-tell loop inside libvzgp
-(`vzgp_eagle_run` / `vzgp_random_search`); only the `count` winners come back to the host.
+  * `random_strategy_factory` (random_vectorized_optimizer.py:114-123),
+  * `LBFGSBOptimizerFactory` / `LBFGSBOptimizer` (lbfgsb_optimizer.py:48-250).
+Calling a vectorised optimiser runs the whole ask-evaluate-tell loop inside libvzgp
+(`vzgp_eagle_run` / `vzgp_random_search`); only the `count` winners come back to the host.  The L-BFGS-B
+optimiser drives SciPy's L-BFGS-B on the host, all restarts in lock step, with the acquisition and its gradient
+evaluated on the device (`vzgp_score_grad`), one batched call per round.
 """
 
 from __future__ import annotations
@@ -18,7 +21,7 @@ from typing import Callable, Dict, Optional, Union
 
 import numpy as np
 
-from vizier_b200 import _lib, gp
+from vizier_b200 import _lib, ard, gp
 
 
 @dataclasses.dataclass(frozen=True)
@@ -290,21 +293,28 @@ class VectorizedOptimizer:
       return VectorizedStrategyResults(bx, bs, pe_aux(bx, bz), categorical=bz)
     if is_multi:   # no trust region -> no aux (acquisitions.py:190-207)
       return VectorizedStrategyResults(bx, bs, {}, categorical=bz)
-    # score_with_aux on the winners (vectorized_base.py:504-526)
-    out = dev.score(bx, acq, zs=bz if self.n_categorical else None, with_aux=True)
-    dev.synchronize()
-    aux = {
-        'mean': out['mean'].cpu().numpy(), 'stddev': out['stddev'].cpu().numpy(),
-        'linf_distance': out['linf_distance'].cpu().numpy(),
-        'radius': np.full(count, acq.trust_radius),
-    }
-    if not acq.use_trust_region:
-      return VectorizedStrategyResults(bx, bs, {}, categorical=bz)
-    # the acquisition before the trust region, evaluated by the same device epilogue as the scores
-    raw = dev.score(bx, dataclasses.replace(acq, use_trust_region=False), zs=bz if self.n_categorical else None)
-    dev.synchronize()
-    aux['raw_acquisition'] = raw['score'].cpu().numpy()
+    _, aux = _score_with_aux(dev, acq, bx, bz if self.n_categorical else None)
     return VectorizedStrategyResults(bx, bs, aux, categorical=bz)
+
+
+def _score_with_aux(dev, acq: gp.Acquisition, bx: np.ndarray, bz: Optional[np.ndarray]):
+  """score_with_aux on the winners (vectorized_base.py:504-526): their scores and, with the trust region, the aux
+  arrays of acquisitions.py:190-207.  Returns (scores [count], aux)."""
+  out = dev.score(bx, acq, zs=bz, with_aux=True)
+  dev.synchronize()
+  scores = out['score'].cpu().numpy()
+  if not acq.use_trust_region:
+    return scores, {}
+  aux = {
+      'mean': out['mean'].cpu().numpy(), 'stddev': out['stddev'].cpu().numpy(),
+      'linf_distance': out['linf_distance'].cpu().numpy(),
+      'radius': np.full(len(bx), acq.trust_radius),
+  }
+  # the acquisition before the trust region, evaluated by the same device epilogue as the scores
+  raw = dev.score(bx, dataclasses.replace(acq, use_trust_region=False), zs=bz)
+  dev.synchronize()
+  aux['raw_acquisition'] = raw['score'].cpu().numpy()
+  return scores, aux
 
 
 @dataclasses.dataclass
@@ -317,3 +327,108 @@ class VectorizedOptimizerFactory:
   def __call__(self, converter) -> VectorizedOptimizer:
     return VectorizedOptimizer(self.strategy_factory, converter.n_continuous, converter.n_categorical,
                                self.suggestion_batch_size, self.max_evaluations, tuple(converter.categorical_sizes))
+
+
+@dataclasses.dataclass
+class LBFGSBOptimizer:
+  """L-BFGS-B over the continuous features (lbfgsb_optimizer.py:48-230): `random_restarts` uniform initial points
+  clipped into `bounds`, each minimised on -score by SciPy's L-BFGS-B (gtol 1e-8, maxls 20, `maxiter`), all restarts
+  advancing in lock step (`ard._lockstep`); the `count` lowest final losses win.  Prior features are ignored.  A
+  restart whose value or gradient is not finite stops at that point and keeps its value."""
+
+  bounds: tuple                 # ((low, high),) per continuous feature: (0, 1), or (0.5, 0.5) for a fixed one
+  random_restarts: int = 25
+  maxiter: int = 50
+  gtol: float = 1e-8
+  maxls: int = 20
+  rounds: int = dataclasses.field(default=0, init=False)   # batched evaluations of the last device run
+  final_losses: Optional[np.ndarray] = dataclasses.field(default=None, init=False)   # the winners' last -score
+
+  @property
+  def n_continuous(self) -> int:
+    return len(self.bounds)
+
+  def _check(self, count: int, n_parallel: Optional[int]):
+    if n_parallel and count > 1:
+      raise ValueError("LBFGSBOptimizer doesn't support batch of batches (count > 1 is disallowed when n_parallel "
+                       'is set).')
+    if not 1 <= count <= self.random_restarts:
+      raise ValueError(f'count must be in [1, random_restarts = {self.random_restarts}], got {count}.')
+
+  def _run(self, batch_fn, q: int, count: int, seed: int) -> np.ndarray:
+    """The `count` best final points [count, q * Dc] of the restarts from uniform inits drawn with `seed`."""
+    inits = np.random.default_rng(seed).uniform(size=(self.random_restarts, q * self.n_continuous))
+    bounds = list(self.bounds) * q
+    if ard._setulb is None:  # pylint: disable=protected-access
+      raise NotImplementedError("LBFGSBOptimizer needs SciPy's reverse-communication L-BFGS-B routine (the C "
+                                'setulb of SciPy >= 1.15), which drives the restarts in lock step.')
+    results = ard._lockstep(batch_fn, inits, bounds, stop_nonfinite=True, maxiter=self.maxiter,  # pylint: disable=protected-access
+                            gtol=self.gtol, maxls=self.maxls)
+    losses = np.asarray([r[1] for r in results])
+    order = np.argsort(losses, kind='stable')[:count]    # NaN losses sort last
+    self.final_losses = losses[order]
+    return np.stack([np.asarray(results[i][0], np.float64) for i in order])
+
+  def optimize_host(self, value_and_grad: Callable, *, count: int = 1, n_parallel: Optional[int] = None,
+                    seed: int = 0) -> VectorizedStrategyResults:
+    """The optimiser on a host function: `value_and_grad(points) -> (values [B], grads)` with points [B, Dc], or
+    [B, n_parallel, Dc] when a value rates a set of n_parallel points (grads have the points' shape).  Returns
+    features [count, Dc] and their values, or with n_parallel the best set [n_parallel, Dc] with its value repeated."""
+    self._check(count, n_parallel)
+    q, dc = int(n_parallel or 1), self.n_continuous
+
+    def shaped(pts):
+      return pts.reshape(-1, q, dc) if n_parallel else pts.reshape(-1, dc)
+
+    def batch_fn(idx, pts):
+      del idx
+      values, grads = value_and_grad(shaped(np.stack(pts)))
+      return -np.asarray(values, np.float64), -np.asarray(grads, np.float64).reshape(len(pts), -1)
+
+    best = self._run(batch_fn, q, count, seed)
+    values = np.asarray(value_and_grad(shaped(best))[0], np.float64).reshape(-1)
+    if n_parallel:
+      return VectorizedStrategyResults(best.reshape(q, dc), np.full(q, values[0]), {},
+                                       categorical=np.zeros((q, 0), np.int32))
+    return VectorizedStrategyResults(best, values, {}, categorical=np.zeros((count, 0), np.int32))
+
+  def __call__(self, dev, acq, *, count: int = 1, prior_features: Optional[np.ndarray] = None,
+               prior_categorical: Optional[np.ndarray] = None, seed: int = 0) -> VectorizedStrategyResults:
+    """`VectorizedOptimizer.__call__` on a single-metric GP (`gp.DeviceGP` or `gp.EnsembleGP`) and a
+    `gp.Acquisition`: every round scores the unfinished restarts with one `score_grad` call.  Rewards and aux are
+    those of `dev.score` at the winners, as for the Eagle optimiser."""
+    import torch
+    del prior_features, prior_categorical
+    if not isinstance(acq, gp.Acquisition) or not isinstance(dev, (gp.DeviceGP, gp.EnsembleGP)):
+      raise NotImplementedError('LBFGSBOptimizer optimises single-metric acquisitions of one GP or a uniform '
+                                f'ensemble, not {type(acq).__name__} on {type(dev).__name__}.')
+    self._check(count, None)
+    self.rounds = 0
+
+    def batch_fn(idx, pts):
+      del idx
+      out = dev.score_grad(np.stack(pts), acq)
+      with torch.cuda.stream(dev.stream):
+        flat = out['_flat'].cpu().numpy()        # score [k] then grad [k, Dc]: one copy per round
+      k = len(pts)
+      self.rounds += 1
+      return -flat[:k], -flat[k:].reshape(k, self.n_continuous)
+
+    bx = self._run(batch_fn, 1, count, seed)
+    scores, aux = _score_with_aux(dev, acq, bx, None)
+    return VectorizedStrategyResults(bx, scores, aux, categorical=np.zeros((count, 0), np.int32))
+
+
+@dataclasses.dataclass(frozen=True)
+class LBFGSBOptimizerFactory:
+  """lbfgsb_optimizer.py:233-270."""
+
+  random_restarts: int = 25
+  maxiter: int = 100
+
+  def __call__(self, converter) -> LBFGSBOptimizer:
+    if converter.n_categorical > 0:
+      raise ValueError("LBFGSBOptimizer doesn't support categorical features.")
+    # the scaled specs' bounds (converters/core.py:441): a parameter with low == high maps to 0.5
+    bounds = tuple((0.5, 0.5) if s.low == s.high else (0.0, 1.0) for s in converter.continuous_specs)
+    return LBFGSBOptimizer(bounds, self.random_restarts, self.maxiter)
