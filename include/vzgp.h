@@ -86,7 +86,10 @@ typedef struct vzgp_acq {
  * use_threshold (AcquisitionTrustRegion): where the `thresholding` value t is not >= threshold the score is
  * bad_acq_value - t, elsewhere the `main` acquisition.  The caller resolves a NaN threshold and apply_tr_after by
  * passing use_threshold = 0. */
-typedef enum vzgp_acq_kind { VZGP_ACQ_UCB = 0, VZGP_ACQ_LCB = 1, VZGP_ACQ_EI = 2, VZGP_ACQ_PI = 3 } vzgp_acq_kind;
+typedef enum vzgp_acq_kind {
+  VZGP_ACQ_UCB = 0, VZGP_ACQ_LCB = 1, VZGP_ACQ_EI = 2, VZGP_ACQ_PI = 3,
+  VZGP_ACQ_MES = 4   /* set by vzgp_mes_fit / vzgp_set_mes only; vzgp_set_acquisition rejects it */
+} vzgp_acq_kind;
 typedef struct vzgp_acq_term {
   int kind;               /* vzgp_acq_kind */
   double coefficient;     /* UCB / LCB */
@@ -106,6 +109,24 @@ typedef struct vzgp_acq_fn {
  * of hs[0].  GP-UCB-PE (single- and multi-metric), set-PE and multi-metric calls ignore it.  Unknown kinds and a non-finite best_label for EI
  * or PI are rejected with VZGP_ERR_ARG. */
 int vzgp_set_acquisition(vzgp_handle* h, const vzgp_acq_fn* fn);
+
+/* MaxValueEntropySearch (acquisitions.py:293-365; Wang & Jegelka, ICML 2017, §3.1) as the acquisition of h, until the
+ * next vzgp_set_acquisition.  Its value at (mu, sd) is (1/K) sum_k [g_k phi(g_k) / (2 Phi(g_k)) - log Phi(g_k)],
+ * g_k = (y*_k - mu) / sd, over K max-value samples y*_k (sd = 0: a sample above mu adds 0, one equal to it log 2, one
+ * below +inf), followed by the trust region.  It is single-model: the ensemble and stack scoring and Eagle calls and
+ * vzgp_score_grad_ensemble return VZGP_ERR_ARG when hs[0] has it; GP-UCB-PE, set-PE and multi-metric calls ignore it.
+ * The samples belong to the fit they were drawn for: after a refit every scoring call on h returns VZGP_ERR_ARG until
+ * vzgp_mes_fit or vzgp_set_mes (or vzgp_set_acquisition) runs again.
+ *
+ * vzgp_mes_fit draws them on the device (k_mes_fit) from h's posterior at its valid trials (mu_i, sd_i as vzgp_score
+ * computes them, sd^2 including the noise): P(y) = prod_i Phi((y - mu_i) / sd_i); floor = best_label + 5 sqrt(sn2);
+ * P(best_label) >= 0.25 makes every sample `floor`; otherwise a Gumbel fit to the quartiles of P (bisection, fixed
+ * iteration count) gives y*_k = max(a - b log(-log u_k), floor), u_k = Philox stream 14 of `seed`, element k.
+ * max_values_out: optional device copy [num_samples].  Continuous models only (Dk = 0), 1 <= num_samples <= 256,
+ * finite best_label, else VZGP_ERR_ARG; VZGP_ERR_STATE before a fit.  Asynchronous on h's stream.
+ * vzgp_set_mes takes given samples (host [num_samples], finite) instead. */
+int vzgp_mes_fit(vzgp_handle* h, double best_label, int num_samples, uint64_t seed, double* max_values_out);
+int vzgp_set_mes(vzgp_handle* h, const double* host_values, int num_samples);
 
 /* GP-UCB-PE acquisition (vizier/_src/algorithms/designers/gp_ucb_pe.py:282-492) built from two
  * fitted models: A = completed trials (mean, stddev), B = completed + pending trials

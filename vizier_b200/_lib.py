@@ -53,7 +53,8 @@ class Acq(C.Structure):
   ]
 
 
-ACQ_UCB, ACQ_LCB, ACQ_EI, ACQ_PI = 0, 1, 2, 3   # vzgp_acq_kind
+ACQ_UCB, ACQ_LCB, ACQ_EI, ACQ_PI, ACQ_MES = 0, 1, 2, 3, 4   # vzgp_acq_kind
+MES_MAX_SAMPLES = 256
 
 
 class AcqTerm(C.Structure):
@@ -194,6 +195,8 @@ SIGNATURES = {
     'vzgp_set_int': (_i, [_vp, C.c_char_p, _i]),
     'vzgp_get_int': (_i, [_vp, C.c_char_p, C.POINTER(C.c_int64)]),
     'vzgp_set_acquisition': (_i, [_vp, C.POINTER(AcqFn)]),
+    'vzgp_mes_fit': (_i, [_vp, C.c_double, _i, C.c_uint64, _vp]),
+    'vzgp_set_mes': (_i, [_vp, _vp, _i]),
     'vzgp_kernel_matrix': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _pP, _d, _vp, _i]),
     'vzgp_cross_kernel': (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _pP, _vp, _i]),
     'vzgp_cholesky_retry': (_i, [_vp, _vp, _i, _i, _d, _i, _vp, _i, _pd]),

@@ -155,6 +155,40 @@ def bayesian_scoring_function_factory(acquisition_fn_factory: Callable[[ModelDat
   return f
 
 
+def _num_categorical(features) -> int:
+  """Categorical feature dimensions of `ModelData.features`: a (continuous, categorical) pair as the designer passes
+  it, or an object with a `categorical` array (vizier's ModelInput)."""
+  if features is None:
+    return 0
+  cat = features[1] if isinstance(features, tuple) else getattr(features, 'categorical', None)
+  cat = getattr(cat, 'padded_array', cat)
+  return 0 if cat is None else int(np.shape(cat)[-1])
+
+
+@dataclasses.dataclass
+class MaxValueEntropySearch:
+  """MaxValueEntropySearch scoring function (acquisitions.py:293-365): the MES of Wang & Jegelka (ICML 2017) over
+  `num_max_value_samples` Gumbel-fitted max values seeded by `seed`, then the trust region.  The designer draws the
+  max values on the device after each fit (`gp.DeviceGP.mes_fit`) from its model and `best_label`, the best warped
+  label (-inf without observations).  Continuous features only."""
+
+  best_label: float
+  use_trust_region: bool = False
+  num_max_value_samples: int = 100
+  seed: int = 123
+
+  @classmethod
+  def scoring_fn_factory(cls, data: ModelData, predictive, continuous_feasible_values,
+                         use_trust_region: bool = False) -> 'MaxValueEntropySearch':
+    """acquisitions.py:299-344: raises ValueError for categorical features."""
+    del predictive, continuous_feasible_values
+    if _num_categorical(data.features) > 0:
+      raise ValueError('Categorical data is not supported.')
+    labels = np.asarray(data.labels.padded_array, np.float64)
+    best = float(np.max(labels)) if labels.size else -np.inf
+    return cls(best, bool(use_trust_region))
+
+
 def _best_label(best_labels) -> float:
   b = np.asarray(best_labels, np.float64).reshape(-1)
   if b.size != 1:

@@ -4,6 +4,8 @@
 // k_general_finalize, k_stack_ensemble_combine, k_ensemble_combine, score_batch64) evaluates acq_value on its final
 // (mean, stddev); those and the GP-UCB-PE combines (k_pe_ensemble_combine, k_pe_multi_combine, score_batch64, k_eagle_grid)
 // then call tr_apply.  The set scorers (k_set_pe_combine, k_qacq_mc) add tr_set_term per point instead.
+// MaxValueEntropySearch (acquisitions.py:293-365) is the main acquisition only, over the handle's max-value samples
+// (vzgp_mes_fit / vzgp_set_mes, DESIGN §6k).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -13,6 +15,7 @@
 namespace vzgp {
 
 constexpr int kMaxDc = 64;     // continuous feature dims supported by the tile kernels
+constexpr int kMaxMesSamples = 256;   // max-value samples of MaxValueEntropySearch
 
 struct AcqTerm {
   int kind;             // vzgp_acq_kind
@@ -26,6 +29,8 @@ struct AcqFn {
   AcqTerm thr;          // AcquisitionTrustRegion: the thresholding acquisition
   int use_thr;          // 0: main only (also when the host resolved a NaN threshold or apply_tr_after)
   double threshold, bad_value;
+  const double* mes;    // main.kind == VZGP_ACQ_MES: the handle's max-value samples (device) ...
+  int mes_k;            // ... and their count
 };
 
 // Plain UCB with coefficient c: what every call computes unless the handle was given another acquisition.
@@ -35,6 +40,7 @@ inline AcqFn ucb_acq_fn(double c) {
   f.thr = f.main;
   f.use_thr = 0;
   f.threshold = 0.0; f.bad_value = 0.0;
+  f.mes = nullptr; f.mes_k = 0;
   return f;
 }
 
@@ -57,10 +63,98 @@ __device__ __forceinline__ double acq_term(const AcqTerm& t, double mean, double
   return fma(t.coefficient, sd, mean);   // UCB: the same expression as the UCB-only epilogues had
 }
 
+// One max-value sample's MES term t(g) = g r / 2 - log Phi(g), r = phi(g) / Phi(g), and dt/dg = -(r/2)(1 + g^2 + g r),
+// at g = (y* - mean) / sd (Wang & Jegelka 2017, eq. 6).  g r / 2 and -log Phi both grow like g^2 / 2 as g -> -inf,
+// so c = g + r is formed without cancelling them: directly from erfcx down to g = -12, and below from the
+// asymptotic series S = 1 - sqrt(pi) x erfcx(x) = sum_m (-1)^(m+1) (2m-1)!! z^m, x = -g / sqrt 2, z = 1 / g^2, where
+// r = |g| / (1 - S), c = |g| S / (1 - S) and 1 + g c = U / (1 - S), U = sum_m (-1)^(m+1) 2m (2m-1)!! z^m.
+// tests/mes_oracle.py restates it; tests/test_mes_host.py holds it to mpmath.
+constexpr double kMesSeriesG = -12.0;
+constexpr int kMesSeriesTerms = 24;
+
+__device__ __forceinline__ void mes_term(double g, double& t, double& dt) {
+  if (g >= 0.0) {
+    const double ec = erfc(g * 0.7071067811865476);
+    const double r = 0.3989422804014327 * exp(-0.5 * g * g) / (1.0 - 0.5 * ec);
+    t = 0.5 * g * r - log1p(-0.5 * ec);
+    dt = -0.5 * r * (1.0 + g * g + g * r);
+  } else if (g >= kMesSeriesG) {
+    const double E = erfcx(-g * 0.7071067811865476);
+    const double r = 0.7978845608028654 / E, c = g + r;
+    t = 0.5 * g * c - log(0.5 * E);
+    dt = -0.5 * r * (1.0 + g * c);
+  } else {
+    const double z = 1.0 / (g * g);
+    double s = z, S = 0.0, U = 0.0;
+    for (int m = 1; m <= kMesSeriesTerms; ++m) {
+      S += s;
+      U += (2.0 * m) * s;
+      s *= -(2.0 * m + 1.0) * z;
+    }
+    const double a = -g, r = a / (1.0 - S), c = a * S / (1.0 - S);
+    t = 0.5 * g * c - log1p(-S) + (log(a) + 0.9189385332046728);
+    dt = -0.5 * r * (U / (1.0 - S));
+  }
+}
+
+// MES at (mean, sd): the samples' terms summed in index order over K, the same order on every route, so a given
+// (mean, sd) scores bit-identically everywhere.  With SLOPES also d/dmean and d/dsd.  sd = 0 (clamped variance) takes
+// the limits - a sample above the mean adds 0, one equal to it log 2, one below +inf - and no slope.
+template <bool SLOPES>
+__device__ __forceinline__ double mes_value(const AcqFn& f, double mean, double sd, double* s_mu = nullptr,
+                                            double* s_sd = nullptr) {
+  double v = 0.0, a_mu = 0.0, a_sd = 0.0;
+  if (sd > 0.0) {
+    for (int k = 0; k < f.mes_k; ++k) {
+      const double g = (f.mes[k] - mean) / sd;
+      double t, dt;
+      mes_term(g, t, dt);
+      v += t;
+      if (SLOPES) { a_mu -= dt / sd; a_sd -= dt * g / sd; }
+    }
+  } else {
+    for (int k = 0; k < f.mes_k; ++k) {
+      const double y = f.mes[k];
+      v += y > mean ? 0.0 : (y == mean ? 0.6931471805599453 : INFINITY);
+    }
+  }
+  if (SLOPES) { *s_mu = a_mu / f.mes_k; *s_sd = a_sd / f.mes_k; }
+  return v / f.mes_k;
+}
+
+// mes_value on a group of eight consecutive lanes, for epilogues with idle lanes: lane p of the group evaluates the
+// terms of samples k0 + p, eight at a time, and every lane then adds the eight in index order, so the sum is
+// mes_value's bit for bit while the costly terms run in parallel.  Every lane of the warp takes part; each group may
+// hold its own candidate.
+__device__ __forceinline__ double mes_value_8(const AcqFn& f, double mean, double sd, int p) {
+  const int base = (threadIdx.x & 31) & ~7;
+  double v = 0.0;
+  for (int k0 = 0; k0 < f.mes_k; k0 += 8) {
+    double t = 0.0;
+    if (k0 + p < f.mes_k) {
+      const double y = f.mes[k0 + p];
+      if (sd > 0.0) {
+        double dt;
+        mes_term((y - mean) / sd, t, dt);
+      } else {
+        t = y > mean ? 0.0 : (y == mean ? 0.6931471805599453 : INFINITY);
+      }
+    }
+    const int n = f.mes_k - k0 < 8 ? f.mes_k - k0 : 8;
+    for (int j = 0; j < 8; ++j) {
+      const double tj = __shfl_sync(0xffffffffu, t, base + j);
+      if (j < n) v += tj;
+    }
+  }
+  return v / f.mes_k;
+}
+
 // AcquisitionTrustRegion.__call__ (:466-492): where the thresholding value is not >= threshold (NaN included) the
-// score is bad_value - thresholding value, otherwise the main acquisition.
+// score is bad_value - thresholding value, otherwise the main acquisition.  MES = false leaves MaxValueEntropySearch
+// out, for kernels that never see it (multi-model combines) or have an instance of their own for it.
+template <bool MES = true>
 __device__ __forceinline__ double acq_value(const AcqFn& f, double mean, double sd) {
-  const double v = acq_term(f.main, mean, sd);
+  const double v = MES && f.main.kind == VZGP_ACQ_MES ? mes_value<false>(f, mean, sd) : acq_term(f.main, mean, sd);
   if (f.use_thr) {
     const double t = acq_term(f.thr, mean, sd);
     if (!(t >= f.threshold)) return f.bad_value - t;
@@ -70,9 +164,9 @@ __device__ __forceinline__ double acq_value(const AcqFn& f, double mean, double 
 
 // The scoring kernels on the default path are instantiated twice: GENERIC = false evaluates only UCB with the
 // main coefficient (the default keeps its register budget), GENERIC = true every acquisition.
-template <bool GENERIC>
+template <bool GENERIC, bool MES = true>
 __device__ __forceinline__ double acq_eval(const AcqFn& f, double mean, double sd) {
-  return GENERIC ? acq_value(f, mean, sd) : fma(f.main.coefficient, sd, mean);
+  return GENERIC ? acq_value<MES>(f, mean, sd) : fma(f.main.coefficient, sd, mean);
 }
 
 // L-inf trust region (acquisitions.py:152-174, :779-820), resolved on the host by trust_region_of (launchers.h).

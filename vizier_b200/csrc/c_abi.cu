@@ -184,7 +184,7 @@ static int fit_common(vzgp_handle* h, const double* X, const int32_t* Z, const d
   VZ_TRY(fill_kernel_params(p, dc, dk, &kp));
   const int np = round_up(N, kBlk);
   VZ_TRY(ensure_model_buffers(h, np, dc, dk, n_metrics));
-  h->fitted = false; h->i8_ready = false;
+  h->fitted = false; h->i8_ready = false; h->model_gen++;
   h->n = N; h->np = np; h->dc = dc; h->dk = dk; h->n_valid = n_valid; h->n_metrics = n_metrics;
   h->kp = kp; h->sn2 = p->observation_noise_variance;
   h->mean_const = p->linear_coef != 0.0 ? p->linear_coef * p->mean_constant : 0.0;
@@ -265,7 +265,7 @@ static int nll_graph_eval(vzgp_handle* h, const double* X, const int32_t* Z, con
              h->nll_key_dims[3] == n_valid && h->nll_key_dims[4] == n_metrics;
   hit = hit && (h->df_nb[1] == 0 || h->df_nb[1] == np / 64);   // another call re-planned the dataflow tasks
   for (int q = 0; hit && q < kNllBufs; ++q) hit = cur[q] == h->nll_bufs[q];   // a workspace was reallocated since the capture
-  h->fitted = false; h->i8_ready = false;
+  h->fitted = false; h->i8_ready = false; h->model_gen++;
   if (!hit) {
     nll_graph_drop(h);
     VZ_TRY(ensure_model_buffers(h, np, dc, dk, n_metrics));
@@ -440,6 +440,17 @@ static int ensure_pinned(vzgp_handle* h, size_t bytes) {
 
 // The acquisition function the scoring calls on h evaluate (nullptr: UCB with the call's coefficient).
 static const AcqFn* handle_acq(const vzgp_handle* h) { return h->has_acq_fn ? &h->acq_fn : nullptr; }
+
+// MaxValueEntropySearch is a single-model acquisition, and its samples belong to the model they were drawn for.
+static int check_acq(const vzgp_handle* h, bool multi) {
+  if (!h->has_acq_fn || h->acq_fn.main.kind != VZGP_ACQ_MES) return 0;
+  VZ_ARG(!multi, "MaxValueEntropySearch scores single models only (not ensembles or stacks)");
+  VZ_ARG(h->mes_gen == h->model_gen, "MaxValueEntropySearch samples are stale: the model was refitted since "
+         "vzgp_mes_fit / vzgp_set_mes");
+  return 0;
+}
+
+static int check_acq(vzgp_handle* const* hs) { return check_acq(hs[0], true); }
 
 static int acq_term_from(const vzgp_acq_term& t, AcqTerm* out) {
   VZ_ARG(t.kind >= VZGP_ACQ_UCB && t.kind <= VZGP_ACQ_PI, "unknown vzgp_acq_kind");
@@ -679,6 +690,44 @@ int vzgp_set_acquisition(vzgp_handle* h, const vzgp_acq_fn* fn) {
   return 0;
 }
 
+static void use_mes(vzgp_handle* h, int K) {
+  AcqFn f = ucb_acq_fn(0.0);
+  f.main.kind = VZGP_ACQ_MES;
+  f.thr = f.main;
+  f.mes = h->mes.as<double>();
+  f.mes_k = K;
+  h->acq_fn = f;
+  h->has_acq_fn = true;
+  h->mes_gen = h->model_gen;
+}
+
+int vzgp_mes_fit(vzgp_handle* h, double best_label, int num_samples, uint64_t seed, double* max_values_out) {
+  VZ_ARG(h != nullptr, "handle");
+  if (!h->fitted) { set_error("vzgp_mes_fit before vzgp_fit"); return VZGP_ERR_STATE; }
+  VZ_ARG(h->dk == 0 && h->n_metrics == 1, "MaxValueEntropySearch needs a single-metric model of continuous features");
+  VZ_ARG(num_samples >= 1 && num_samples <= kMaxMesSamples, "1 <= num_samples <= 256");
+  VZ_ARG(std::isfinite(best_label), "finite best_label");
+  Guard g(h->device);
+  VZ_TRY(launch_mes_fit(h, best_label, num_samples, seed));
+  if (max_values_out)
+    VZ_CUDA(cudaMemcpyAsync(max_values_out, h->mes.ptr, sizeof(double) * num_samples, cudaMemcpyDeviceToDevice,
+                            h->stream));
+  use_mes(h, num_samples);
+  return 0;
+}
+
+int vzgp_set_mes(vzgp_handle* h, const double* host_values, int num_samples) {
+  VZ_ARG(h != nullptr && host_values != nullptr, "handle / values");
+  VZ_ARG(num_samples >= 1 && num_samples <= kMaxMesSamples, "1 <= num_samples <= 256");
+  for (int k = 0; k < num_samples; ++k) VZ_ARG(std::isfinite(host_values[k]), "finite max values");
+  Guard g(h->device);
+  VZ_TRY(h->mes.reserve(sizeof(double) * kMaxMesSamples));
+  // pageable source: the copy has left host_values when the call returns
+  VZ_CUDA(cudaMemcpyAsync(h->mes.ptr, host_values, sizeof(double) * num_samples, cudaMemcpyHostToDevice, h->stream));
+  use_mes(h, num_samples);
+  return 0;
+}
+
 int vzgp_get_int(const vzgp_handle* h, const char* key, int64_t* value) {
   VZ_ARG(h && key && value, "handle / key / value");
   if (std::strcmp(key, "launches") == 0) { *value = h->launches; return 0; }
@@ -749,7 +798,7 @@ int vzgp_factor_inverse(vzgp_handle* h, const double* A, int N, int lda, double*
   Guard g(h->device);
   const int np = round_up(N, kBlk);
   VZ_TRY(ensure_model_buffers(h, np, 1, 0));
-  h->fitted = false; h->i8_ready = false;
+  h->fitted = false; h->i8_ready = false; h->model_gen++;
   const bool want_kinv = Kinv != nullptr;
   if (want_kinv) VZ_TRY(h->Kinv.reserve(sizeof(double) * (size_t)np * np * kLauumSplit));
   int* flag = reinterpret_cast<int*>(h->small.as<char>() + kOffFlag);
@@ -899,7 +948,7 @@ static int check_scoring(vzgp_handle* h, const double* Xs, const int32_t* Zs, in
   VZ_ARG(score != nullptr, "score");
   VZ_ARG(Xs != nullptr || h->dc == 0, "Xs");
   VZ_ARG(Zs != nullptr || h->dk == 0, "Zs");
-  return 0;
+  return check_acq(h, false);
 }
 
 int vzgp_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const vzgp_acq* acq,
@@ -1050,6 +1099,7 @@ int vzgp_random_search(vzgp_handle* h, int64_t M, int64_t index_base, const vzgp
                        double* best_score, int64_t* best_index) {
   VZ_ARG(h && acq && best_score, "handle / pointers");
   if (!h->fitted) { set_error("vzgp_random_search before vzgp_fit"); return VZGP_ERR_STATE; }
+  VZ_TRY(check_acq(h, false));
   VZ_ARG(M >= 1 && M <= INT_MAX, "1 <= M < 2^31 per call");
   VZ_ARG(best_x != nullptr || h->dc == 0, "best_x");
   VZ_ARG(best_z != nullptr || h->dk == 0, "best_z");
@@ -1376,6 +1426,7 @@ int vzgp_eagle_run(vzgp_handle* h, const vzgp_eagle_config* cfg, const vzgp_acq*
                    const int32_t* prior_z, int n_prior, const int32_t* cat_sizes, int count, uint64_t seed,
                    double* best_x, int32_t* best_z, double* best_score) {
   VZ_ARG(acq != nullptr, "acq");
+  if (h != nullptr) VZ_TRY(check_acq(h, false));
   Model m{Model::kSingle, h, &h};
   m.acq = acq;
   return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
@@ -1485,6 +1536,7 @@ int vzgp_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const i
                         const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf) {
   VZ_TRY(check_ensemble(hs, E));
   VZ_ARG(acq != nullptr, "acq");
+  VZ_TRY(check_acq(hs));
   VZ_TRY(check_pool(hs[0], Xs, Zs, M, score));
   Guard g(hs[0]->device);
   return launch_score_ensemble(hs, E, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(hs[0]));
@@ -1504,6 +1556,7 @@ int vzgp_score_grad(vzgp_handle* h, const double* Xs, int M, const vzgp_acq* acq
                     double* mu, double* sigma, double* linf) {
   VZ_TRY(check_handles(&h, 1, 1, Trials::kAny));
   VZ_TRY(check_score_grad(&h, 1, Xs, M, acq, score, grad));
+  VZ_TRY(check_acq(h, false));
   Guard g(h->device);
   return launch_score_grad(&h, 1, Xs, M, acq, handle_acq(h), score, grad, mu, sigma, linf);
 }
@@ -1512,6 +1565,7 @@ int vzgp_score_grad_ensemble(vzgp_handle* const* hs, int E, const double* Xs, in
                              double* score, double* grad, double* mu, double* sigma, double* linf) {
   VZ_TRY(check_ensemble(hs, E));
   VZ_TRY(check_score_grad(hs, E, Xs, M, acq, score, grad));
+  VZ_TRY(check_acq(hs));
   Guard g(hs[0]->device);
   return launch_score_grad(hs, E, Xs, M, acq, handle_acq(hs[0]), score, grad, mu, sigma, linf);
 }
@@ -1521,6 +1575,7 @@ int vzgp_eagle_run_ensemble(vzgp_handle* const* hs, int E, const vzgp_eagle_conf
                             int count, uint64_t seed, double* best_x, int32_t* best_z, double* best_score) {
   VZ_TRY(check_ensemble(hs, E));
   VZ_ARG(acq != nullptr, "acq");
+  VZ_TRY(check_acq(hs));
   // the loop scores a one-member ensemble as the single model it is, without the mixture
   Model m{E == 1 ? Model::kSingle : Model::kEnsemble, hs[0], hs};
   m.E = E; m.acq = acq;
@@ -1621,6 +1676,7 @@ int vzgp_score_stack(vzgp_handle* const* hs, int E, const double* alphas, const 
                      const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf) {
   VZ_TRY(check_stack(hs, E, 1, alphas));
   VZ_ARG(acq != nullptr, "acq");
+  VZ_TRY(check_acq(hs));
   VZ_TRY(check_pool(hs[0], Xs, Zs, M, score));
   Guard g(hs[0]->device);
   return launch_score_stack_ensemble(hs, E, 1, alphas, Xs, Zs, M, acq, score, mu, sigma, linf, handle_acq(hs[0]));
@@ -1632,6 +1688,7 @@ int vzgp_eagle_run_stack(vzgp_handle* const* hs, int E, const double* alphas, co
                          double* best_score) {
   VZ_TRY(check_stack(hs, E, 1, alphas));
   VZ_ARG(acq != nullptr, "acq");
+  VZ_TRY(check_acq(hs));
   Model m{Model::kStack, hs[E - 1], hs};
   m.n = E; m.alphas = alphas; m.acq = acq;
   return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
@@ -1642,6 +1699,7 @@ int vzgp_score_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, const
                               double* linf) {
   VZ_TRY(check_stack_ensemble(hs, n_levels, E, alphas));
   VZ_ARG(acq != nullptr, "acq");
+  VZ_TRY(check_acq(hs));
   VZ_TRY(check_pool(hs[0], Xs, Zs, M, score));
   Guard g(hs[0]->device);
   return launch_score_stack_ensemble(hs, n_levels, E, alphas, Xs, Zs, M, acq, score, mu, sigma, linf,
@@ -1654,6 +1712,7 @@ int vzgp_eagle_run_stack_ensemble(vzgp_handle* const* hs, int n_levels, int E, c
                                   uint64_t seed, double* best_x, int32_t* best_z, double* best_score) {
   VZ_TRY(check_stack_ensemble(hs, n_levels, E, alphas));
   VZ_ARG(acq != nullptr, "acq");
+  VZ_TRY(check_acq(hs));
   Model m{Model::kStack, hs[(n_levels - 1) * E], hs};
   m.n = n_levels; m.E = E; m.alphas = alphas; m.acq = acq;
   return eagle_run_impl(m, cfg, prior, prior_z, n_prior, cat_sizes, count, seed, best_x, best_z, best_score);
@@ -1728,7 +1787,7 @@ static int nll_batch_eval(vzgp_handle* const* hs, int R, const double* X, const 
       VZ_TRY(h->Tws.reserve(sizeof(double) * (size_t)np * np));
       VZ_TRY(chol_dataflow_prepare(h, np, true));
       VZ_TRY(ensure_pinned(h, res_bytes));
-      h->fitted = false; h->i8_ready = false;
+      h->fitted = false; h->i8_ready = false; h->model_gen++;
       h->n = N; h->np = np; h->dc = Dc; h->dk = Dk; h->n_valid = n_valid; h->n_metrics = n_metrics;
       h->mean_const = 0.0;   // captured by the label-padding node (see nll_graph_eval)
       VZ_CUDA(cudaStreamSynchronize(h->stream));
@@ -1803,7 +1862,7 @@ static int nll_batch_eval(vzgp_handle* const* hs, int R, const double* X, const 
   for (int r = 0; r < R; ++r) {
     if (active && !active[r]) continue;
     sn2s[r] = ps[r].observation_noise_variance;
-    hs[r]->kp = kps[r]; hs[r]->sn2 = sn2s[r]; hs[r]->mean_const = 0.0; hs[r]->fitted = false; hs[r]->i8_ready = false;
+    hs[r]->kp = kps[r]; hs[r]->sn2 = sn2s[r]; hs[r]->mean_const = 0.0; hs[r]->fitted = false; hs[r]->i8_ready = false; hs[r]->model_gen++;
     for (int q = 0; q < 3; ++q) {
       if (!b->nodes[r][q]) continue;
       cudaKernelNodeParams kpar;

@@ -202,4 +202,10 @@ struct vzgp_handle {
   // vzgp_acq.ucb_coefficient.  Read at every call: no launch state is built from it.
   bool has_acq_fn = false;
   vzgp::AcqFn acq_fn;
+
+  // MaxValueEntropySearch (mes.cu): the max-value samples, allocated once at kMaxMesSamples so that launches and
+  // captured graphs see one address, the fit's scratch (trial moments), and the model they were drawn for: every
+  // change of the fitted model bumps model_gen, and samples with mes_gen != model_gen are stale.
+  vzgp::DevBuf mes, mes_tmp;
+  int64_t model_gen = 0, mes_gen = -1;
 };

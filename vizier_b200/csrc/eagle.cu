@@ -289,7 +289,16 @@ __device__ __forceinline__ void score_batch64(const SmallModel& ma, const SmallM
   stage_candidates64(sm, ma.kp.dc, ma.kp.dk, cand, candz, B);
   if (q.pe_mode < 0) {
     posterior_tile64(ma, sm.a, sm, B, q, sm.mu, sm.sd, q.want_linf ? sm.linf : nullptr, clamp_count);
-    if (tid < B) out_score[tid] = tr_apply(q.tr, acq_eval<GENERIC>(q.fn, sm.mu[tid], sm.sd[tid]), sm.linf[tid]);
+    if (GENERIC && q.fn.main.kind == VZGP_ACQ_MES) {
+      // eight lanes per candidate share its K samples (mes_value_8); every thread takes part in the shuffles
+      for (int c0 = 0; c0 < B; c0 += kPThreads / 8) {
+        const int c = c0 + (tid >> 3), cc = c < B ? c : B - 1;
+        const double v = mes_value_8(q.fn, sm.mu[cc], sm.sd[cc], tid & 7);
+        if (c < B && (tid & 7) == 0) out_score[c] = tr_apply(q.tr, v, sm.linf[c]);
+      }
+    } else if (tid < B) {
+      out_score[tid] = tr_apply(q.tr, acq_eval<GENERIC>(q.fn, sm.mu[tid], sm.sd[tid]), sm.linf[tid]);
+    }
   } else {
     posterior_tile64(ma, sm.a, sm, B, q, sm.mu, sm.sd, nullptr, clamp_count);
     posterior_tile64(mb, sm.b, sm, B, q, sm.mu + 64, sm.sd + 64, q.want_linf ? sm.linf : nullptr, clamp_count);

@@ -13,6 +13,8 @@ constexpr uint32_t kStreamInitCat = 4, kStreamCatLaplace = 5, kStreamCatGumbel =
                    kStreamPullRand = 9, kStreamPushRand = 10, kStreamSetLaplace = 11;
 // Monte Carlo draws of the q-acquisitions (score_q.cu): Box-Muller normals and mixture members.
 constexpr uint32_t kStreamQacqNormal = 12, kStreamQacqMember = 13;
+// Uniforms of the MaxValueEntropySearch max-value samples (mes.cu).
+constexpr uint32_t kStreamMes = 14;
 
 __device__ __forceinline__ double laplace_from_uniform(double u) {
   const double v = u - 0.5;

@@ -173,6 +173,8 @@ int launch_nll_grad_small(vzgp_handle* h, const double* X, const int32_t* Z, con
 // as the two-pass mixture; continuous features only.  grad is [M x Dc].
 int launch_score_grad(vzgp_handle* const* hs, int E, const double* Xs, int M, const vzgp_acq* acq, const AcqFn* fn,
                       double* score, double* grad, double* mu, double* sigma, double* linf);
+// MaxValueEntropySearch max values of h's fitted model into h->mes [K] (mes.cu).
+int launch_mes_fit(vzgp_handle* h, double best_label, int K, uint64_t seed);
 int launch_score_ensemble(vzgp_handle* const* hs, int E, const double* Xs, const int32_t* Zs, int M,
                           const vzgp_acq* acq, double* score, double* mu, double* sigma, double* linf,
                           const AcqFn* fn = nullptr);

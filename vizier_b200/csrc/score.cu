@@ -538,14 +538,17 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   if (ncta > 1) cluster_sync();   // no CTA exits while a peer can still multicast into it or arrive on its barriers
 }
 
-// nsplit > 1: sums the partial row sums in a fixed order and emits the scores.
+// nsplit > 1: sums the partial row sums in a fixed order and emits the scores.  MES: the MaxValueEntropySearch
+// instance (the UCB / LCB / EI / PI one keeps its register budget).
+template <bool MES>
 __global__ void k_score_finalize(const ScoreArgs a) {
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   int clamped = 0;
   if (m < a.M) {
     double rs = 0.0;
     for (int s = 0; s < a.nsplit; ++s) rs += a.part[(size_t)s * a.mpad + m];
-    emit_score(a, m, rs, a.part[(size_t)a.nsplit * a.mpad + m], a.part[(size_t)(a.nsplit + 1) * a.mpad + m], clamped);
+    emit_score<true, MES>(a, m, rs, a.part[(size_t)a.nsplit * a.mpad + m], a.part[(size_t)(a.nsplit + 1) * a.mpad + m],
+                          clamped);
   }
   if (clamped) atomicAdd(a.clamp_count, clamped);
 }
@@ -560,11 +563,11 @@ __global__ void __launch_bounds__(kSmallThreads) k_var_small(const __grid_consta
   extern __shared__ double smem_raw[];
   var_small_dispatch(a, blockIdx.x, blockIdx.y, smem_raw);
 }
-template <bool WITH_LINF>
+template <bool WITH_LINF, bool MES>
 __global__ void __launch_bounds__(256) k_small_finalize(const ScoreArgs a) {
   const int m = blockIdx.x * 32 + (threadIdx.x >> 3);
   int clamped = 0;
-  small_finalize_8<WITH_LINF>(a, m, threadIdx.x & 7, m < a.M, clamped);
+  small_finalize_8<WITH_LINF, true, MES>(a, m, threadIdx.x & 7, m < a.M, clamped);
   if (clamped) atomicAdd(a.clamp_count, clamped);
 }
 
@@ -764,6 +767,8 @@ struct GeneralArgs {
   int* clamp_count;
 };
 
+// One warp per candidate.  MES: the MaxValueEntropySearch instance, its K samples split over lanes 0-7.
+template <bool MES>
 __global__ void __launch_bounds__(256) k_general_finalize(GeneralArgs a) {
   const int m = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32, lane = threadIdx.x & 31;
   if (m >= a.mc) return;
@@ -779,7 +784,7 @@ __global__ void __launch_bounds__(256) k_general_finalize(GeneralArgs a) {
     rs += __shfl_xor_sync(0xffffffffu, rs, o);
     dist = fmin(dist, __shfl_xor_sync(0xffffffffu, dist, o));
   }
-  if (lane != 0) return;
+  if (!MES && lane != 0) return;
   double kss = a.kp.sf2;
   if (a.kp.use_linear) {
     double uu = 0.0;
@@ -791,9 +796,16 @@ __global__ void __launch_bounds__(256) k_general_finalize(GeneralArgs a) {
   }
   mean += a.mean_const;
   double var = kss - rs + a.sn2;
-  if (var < 0.0) { var = 0.0; atomicAdd(a.clamp_count, 1); }
+  if (var < 0.0) { var = 0.0; if (lane == 0) atomicAdd(a.clamp_count, 1); }
   const double sd = sqrt(var);
-  a.score[m] = tr_apply(a.tr, acq_value(a.acq, mean, sd), dist);
+  double acq;
+  if (MES) {
+    acq = mes_value_8(a.acq, mean, sd, lane & 7);
+    if (lane != 0) return;
+  } else {
+    acq = acq_value<false>(a.acq, mean, sd);
+  }
+  a.score[m] = tr_apply(a.tr, acq, dist);
   if (a.mu) a.mu[m] = mean;
   if (a.sigma) a.sigma[m] = sd;
   if (a.linf) a.linf[m] = dist;
@@ -837,7 +849,8 @@ static int launch_score_general(vzgp_handle* h, const double* Xs, const int32_t*
     a.mc = mc;
     a.score = score + m0; a.mu = mu ? mu + m0 : nullptr; a.sigma = sigma ? sigma + m0 : nullptr;
     a.linf = linf ? linf + m0 : nullptr;
-    k_general_finalize<<<(mc + 7) / 8, 256, 0, h->stream>>>(a);
+    if (a.acq.main.kind == VZGP_ACQ_MES) k_general_finalize<true><<<(mc + 7) / 8, 256, 0, h->stream>>>(a);
+    else k_general_finalize<false><<<(mc + 7) / 8, 256, 0, h->stream>>>(a);
     VZ_CHECK_LAUNCH();
     h->launches++;
   }
@@ -879,8 +892,9 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
     VZ_TRY(raise_dyn_smem((const void*)k_var_small, sm2));
     k_var_small<<<g2, kSmallThreads, sm2, h->stream>>>(a);
     VZ_CHECK_LAUNCH();
-    if (with_linf) k_small_finalize<true><<<(M + 31) / 32, 256, 0, h->stream>>>(a);
-    else k_small_finalize<false><<<(M + 31) / 32, 256, 0, h->stream>>>(a);
+    const bool mes = a.acq.main.kind == VZGP_ACQ_MES;
+    if (with_linf) (mes ? k_small_finalize<true, true> : k_small_finalize<true, false>)<<<(M + 31) / 32, 256, 0, h->stream>>>(a);
+    else (mes ? k_small_finalize<false, true> : k_small_finalize<false, false>)<<<(M + 31) / 32, 256, 0, h->stream>>>(a);
     VZ_CHECK_LAUNCH();
     h->launches += 3;
     return 0;
@@ -942,7 +956,8 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
   VZ_CHECK_LAUNCH();
   h->launches++;
   if (nsplit > 1) {
-    k_score_finalize<<<(M + 255) / 256, 256, 0, h->stream>>>(a);
+    if (a.acq.main.kind == VZGP_ACQ_MES) k_score_finalize<true><<<(M + 255) / 256, 256, 0, h->stream>>>(a);
+    else k_score_finalize<false><<<(M + 255) / 256, 256, 0, h->stream>>>(a);
     VZ_CHECK_LAUNCH();
     h->launches++;
   }
@@ -1018,7 +1033,7 @@ __global__ void __launch_bounds__(256) k_stack_ensemble_combine(int M, StackEnsC
     mean += mean_l;
     sd = pow(sd_l, p.alpha[l]) * pow(sd, 1.0 - p.alpha[l]);
   }
-  score[m] = tr_apply(p.tr, acq_value(p.acq, mean, sd), linf[m]);
+  score[m] = tr_apply(p.tr, acq_value<false>(p.acq, mean, sd), linf[m]);
   if (mu) mu[m] = mean;
   if (sigma) sigma[m] = sd;
 }
@@ -1130,7 +1145,7 @@ __global__ void k_ensemble_combine(int M, EnsCombine p, const double* __restrict
   double var = s2 / p.E - mean * mean;
   if (var < 0.0) { var = 0.0; atomicAdd(clamp_count, 1); }
   const double sd = sqrt(var);
-  score[m] = tr_apply(p.tr, acq_value(p.acq, mean, sd), linf[m]);
+  score[m] = tr_apply(p.tr, acq_value<false>(p.acq, mean, sd), linf[m]);
   if (mu) mu[m] = mean;
   if (sigma) sigma[m] = sd;
 }

@@ -243,7 +243,8 @@ __global__ void __launch_bounds__(256) k_grad_combine(int mc, GradCombine p, con
     return;
   }
   double s_mu, s_sd;
-  acq_term_slopes(p.acq.main, mean, sd, s_mu, s_sd);
+  if (p.acq.main.kind == VZGP_ACQ_MES) mes_value<true>(p.acq, mean, sd, &s_mu, &s_sd);   // sd = 0: no slope
+  else acq_term_slopes(p.acq.main, mean, sd, s_mu, s_sd);
   if (p.acq.use_thr) {
     const double t = acq_term(p.acq.thr, mean, sd);
     if (!(t >= p.acq.threshold)) {   // bad_value - t

@@ -49,14 +49,15 @@ struct ScoreArgs {
   AcqFn acq;          // acquisition function of (mean, stddev)
 };
 
-// Final score from the reduced pieces (shared by the fused epilogue and the split finalize kernel).
-template <bool GENERIC = true>
+// Final score from the reduced pieces (shared by the fused epilogue and the split finalize kernel); `acq`: the
+// acquisition value when the caller evaluated it already (MES split over lanes).
+template <bool GENERIC = true, bool MES = true>
 __device__ __forceinline__ void emit_score(const ScoreArgs& a, int m, double rs, double mean, double dist,
-                                           int& clamped) {
+                                           int& clamped, const double* acq = nullptr) {
   double var = a.kp.sf2 - rs + a.sn2;
   if (var < 0.0) { var = 0.0; ++clamped; }
   const double sd = sqrt(var);
-  a.score[m] = tr_apply(a.tr, acq_eval<GENERIC>(a.acq, mean, sd), dist);
+  a.score[m] = tr_apply(a.tr, acq ? *acq : acq_eval<GENERIC, MES>(a.acq, mean, sd), dist);
   if (a.mu) a.mu[m] = mean;
   if (a.sigma) a.sigma[m] = sd;
   if (a.linf) a.linf[m] = dist;
@@ -353,7 +354,7 @@ __device__ __forceinline__ void var_small_dispatch(const ScoreArgs& a, int b, in
 
 // EIGHT lanes per candidate m (lane group p = 0..7 sums partials p, p + 8, ... then a fixed shuffle tree):
 // deterministic, and a 25-candidate batch finalises in one pass of 200 threads.
-template <bool WITH_LINF, bool GENERIC = true>
+template <bool WITH_LINF, bool GENERIC = true, bool MES = true>
 __device__ __forceinline__ void small_finalize_8(const ScoreArgs& a, int m, int p, bool active, int& clamped) {
   const int nvb = a.np / kVarCols, nmb = a.np / 64;
   double rs = 0.0, mean = 0.0, dist = INFINITY;
@@ -370,7 +371,14 @@ __device__ __forceinline__ void small_finalize_8(const ScoreArgs& a, int m, int 
     mean += __shfl_xor_sync(0xffffffffu, mean, o);
     if (WITH_LINF) dist = fmin(dist, __shfl_xor_sync(0xffffffffu, dist, o));
   }
-  if (active && p == 0) emit_score<GENERIC>(a, m, rs, mean, dist, clamped);
+  if (GENERIC && MES && a.acq.main.kind == VZGP_ACQ_MES) {   // warp-uniform: the candidate's eight lanes share the K samples
+    double var = a.kp.sf2 - rs + a.sn2;
+    if (var < 0.0) var = 0.0;
+    const double v = mes_value_8(a.acq, mean, sqrt(var), p);
+    if (active && p == 0) emit_score<GENERIC, false>(a, m, rs, mean, dist, clamped, &v);
+    return;
+  }
+  if (active && p == 0) emit_score<GENERIC, MES>(a, m, rs, mean, dist, clamped);
 }
 
 // Host side (score.cu).  The argument block of the scoring kernels for M candidates on `h`; fn: the acquisition

@@ -34,12 +34,17 @@ it raises NotImplementedError.
 `scoring_function_factory` (e.g. `acquisitions.bayesian_scoring_function_factory(lambda d: EI(get_best_labels(d.labels)))`
 or `AcquisitionTrustRegion.default_ucb_pi`) selects UCB, LCB, EI, PI or a thresholded pair of those; the device
 scoring kernels evaluate it (`acquisitions.lower_acquisition`).  Multi-metric problems keep their scalarised UCB.
+`scoring_function_factory=acquisitions.MaxValueEntropySearch.scoring_fn_factory` scores MaxValueEntropySearch
+(acquisitions.py:293-365): after each `_update_gp` the device draws 100 Gumbel-fitted max values with seed 123 from the
+model (`vzgp_mes_fit`, csrc/mes.cu), and every scoring route evaluates MES on them (DESIGN §6k), under Eagle or
+L-BFGS-B, with `linear_coef` too.  As in the reference it raises ValueError for categorical parameters and for
+`ensemble_size > 1`; with `set_priors` or `scoring_function_is_parallel=True` it raises NotImplementedError.
 `scoring_function_is_parallel=True` with a factory returning `QEI`, `QPI` or `QUCB` suggests one set of `count` points
 (gp_bandit.py:496-499): Monte Carlo estimates over each set's joint posterior, scored by `vzgp_score_qsets`
 (csrc/score_q.cu) inside the n_parallel Eagle loop or the random strategy (`optimizers.optimize_qsets`).
 Not implemented (the reference supports them; SURVEY 8f "next"): parallel acquisitions for multi-metric models or
 with priors, other acquisition
-functions (MaxValueEntropySearch, Sample, user callables), priors for separable multi-task models; each raises NotImplementedError
+functions (Sample, user callables), priors for separable multi-task models; each raises NotImplementedError
 instead of silently doing something else.  Categorical parameters ARE supported
 end to end.  `padding_schedule` is accepted and has no numerical effect here: the kernels take
 explicit sizes (`n_valid`, Dc, Dk) instead of padded shapes + masks, which is what the reference's
@@ -176,9 +181,17 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
       raise NotImplementedError('the L-BFGS-B acquisition optimiser with parallel (q-) scoring functions is not '
                                 'implemented.')
     self._acquisition_optimizer = acquisition_optimizer_factory(self._converter)   # L-BFGS-B: ValueError if categorical
+    self._mes = False
     if self._scoring_function_factory is not None:
-      empty = acq_lib.ModelData(features=None, labels=acq_lib.PaddedArray.as_padded(np.zeros((0, self._n_metrics))))
-      acq_lib.check_supported(self._scoring_function(empty).acquisition_fn, parallel=self._parallel)
+      empty_features = (np.zeros((0, self._converter.n_continuous)), np.zeros((0, self._converter.n_categorical), np.int32))
+      empty = acq_lib.ModelData(features=empty_features,
+                                labels=acq_lib.PaddedArray.as_padded(np.zeros((0, self._n_metrics))))
+      sf = self._scoring_function(empty)
+      self._mes = isinstance(sf, acq_lib.MaxValueEntropySearch)
+      if not self._mes:
+        acq_lib.check_supported(sf.acquisition_fn, parallel=self._parallel)
+      elif self._parallel:
+        raise NotImplementedError('MaxValueEntropySearch is not a parallel (q-) scoring function.')
     # Scalarisation weights are drawn once per designer (gp_bandit.py:217-222: one weights_rng): |N(0,1)|,
     # rows normalised to unit L2 norm (acquisitions.py:585-589).
     self._scal_weights = None
@@ -209,6 +222,8 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     retrains the prior stack from scratch on what it is given."""
     if self._parallel:
       raise NotImplementedError('transfer-learning priors with parallel (q-) scoring functions are not implemented.')
+    if self._mes:
+      raise NotImplementedError('transfer-learning priors with MaxValueEntropySearch are not implemented.')
     if self._lbfgsb:
       raise NotImplementedError('transfer-learning priors with the L-BFGS-B acquisition optimiser are not implemented.')
     if self._multitask_type:
@@ -326,6 +341,10 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     sf = self._scoring_function_factory(
         data, None, self._converter.continuous_feasible_values(_MAX_NUM_FEASIBLE_VALUES_FOR_TRUST_REGION),
         self._use_trust_region)
+    if isinstance(sf, acq_lib.MaxValueEntropySearch):
+      if self._ensemble_size > 1:   # gp_bandit.py:261-268
+        raise ValueError('MaxValueEntropySearch is not supported with ensemble size greater than one.')
+      return sf
     if not isinstance(sf, acq_lib.BayesianScoringFunction):
       raise NotImplementedError(f'scoring function {type(sf).__name__} is not implemented on the device '
                                 '(use acquisitions.bayesian_scoring_function_factory)')
@@ -345,7 +364,8 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     if self._scoring_function_factory is not None:
       # gp_bandit.py:497-505: the factory sees the (warped) labels of this suggest
       data = acq_lib.ModelData(features=features, labels=acq_lib.PaddedArray.as_padded(labels))
-      acq.acq_fn = acq_lib.lower_acquisition(self._scoring_function(data).acquisition_fn)
+      sf = self._scoring_function(data)
+      acq.acq_fn = gp.MES if isinstance(sf, acq_lib.MaxValueEntropySearch) else acq_lib.lower_acquisition(sf.acquisition_fn)
     return acq
 
   @profiler.record_runtime
@@ -407,6 +427,9 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
       best = self._optimize_parallel_acquisition(dev, count, labels, (cont, cat))
     else:
       acq = self._acquisition(cont.shape[0], labels, features=(cont, cat))
+      if self._mes:
+        # the max values belong to the model just fitted (acquisitions.py:328-338: seed 123, 100 samples)
+        dev.mes_fit(float(np.max(labels[:, 0])), num_samples=100, seed=123)
       best = self._optimize_acquisition(dev, acq, count, features=(cont, cat))
     out = []
     for t in best:

@@ -161,6 +161,16 @@ class AcqFnSpec:
     return f
 
 
+@dataclasses.dataclass(frozen=True)
+class MesSpec:
+  """MaxValueEntropySearch as `Acquisition.acq_fn`: the handle scores with the max-value samples that
+  `DeviceGP.mes_fit` / `set_mes` gave it after its last fit (vzgp_mes_fit, include/vzgp.h)."""
+
+
+MES = MesSpec()
+_STALE = object()   # DeviceGP._acq_fn after a fit replaced the model its MES samples were drawn for
+
+
 @dataclasses.dataclass
 class Acquisition:
   """UCB coefficient + trust region (acquisitions.py:213-225, :691-820).  `acq_fn` (acquisitions.lower_acquisition)
@@ -172,7 +182,7 @@ class Acquisition:
   tr_dim_mask: Optional[np.ndarray] = None  # bool [Dc]
   tr_rows: int = 0          # trusted points = first tr_rows rows of the model's X (0 = all)
   tr_strict: bool = False   # dist < radius (gp_ucb_pe.py) instead of dist <= radius (acquisitions.py)
-  acq_fn: Optional[AcqFnSpec] = None
+  acq_fn: Optional[AcqFnSpec | MesSpec] = None
 
   def _c(self):
     a = _lib.Acq()
@@ -432,8 +442,30 @@ class DeviceGP:
 
   def _use_acq(self, acq) -> None:
     fn = acq.acq_fn if isinstance(acq, Acquisition) else None
+    if isinstance(fn, MesSpec):
+      # the samples depend on the fitted model, not on the spec: they are set by mes_fit / set_mes after each fit
+      if not isinstance(self._acq_fn, MesSpec):
+        raise RuntimeError('MaxValueEntropySearch scoring needs mes_fit (or set_mes) after the last fit')
+      return
     if fn != self._acq_fn:
       self.set_acquisition(fn)
+
+  def mes_fit(self, best_label: float, num_samples: int = 100, seed: int = 123) -> torch.Tensor:
+    """Draws MaxValueEntropySearch max values from the fitted model (vzgp_mes_fit) and makes MES the handle's
+    acquisition; returns the samples [num_samples] (device)."""
+    out = torch.empty((int(num_samples),), dtype=torch.float64, device=self.device)
+    self._stream.wait_stream(torch.cuda.current_stream(self.device))
+    _lib.check('vzgp_mes_fit', self._lib.vzgp_mes_fit(self._h, float(best_label), int(num_samples),
+                                                      C.c_uint64(int(seed) & (2**64 - 1)), _ptr(out)))
+    self._acq_fn = MES
+    torch.cuda.current_stream(self.device).wait_stream(self._stream)
+    return out
+
+  def set_mes(self, values) -> None:
+    """Makes MaxValueEntropySearch with the given max values [K] the handle's acquisition (vzgp_set_mes)."""
+    v = np.ascontiguousarray(np.asarray(values, np.float64).reshape(-1))
+    _lib.check('vzgp_set_mes', self._lib.vzgp_set_mes(self._h, v.ctypes.data_as(C.c_void_p), v.shape[0]))
+    self._acq_fn = MES
 
   def close(self):
     if getattr(self, '_h', None):
@@ -563,6 +595,8 @@ class DeviceGP:
     retries = _lib.check('vzgp_fit_multi', self._lib.vzgp_fit_multi(
         self._h, _ptr(xt), _ptr(zt), _ptr(yt), n, dc, dk, n if n_valid is None else n_valid, n_metrics, C.byref(p)))
     self.n_metrics = n_metrics
+    if isinstance(self._acq_fn, MesSpec):
+      self._acq_fn = _STALE   # the library now refuses to score until mes_fit / set_mes or another acquisition
     self.synchronize()  # inputs may be freed by the caller after return
     self.n, self.dc, self.dk = n, dc, dk
     # retrying_cholesky(max_iters=5) exhausted (tuned_gp_models.py:272-280): the factor holds NaN exactly
