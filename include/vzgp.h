@@ -534,7 +534,8 @@ typedef struct vzgp_eagle_config {
   double prob_same_category_without_perturbation; /* 0.98 */
   int mutate_normalization_type;  /* 0 = MEAN (default), 1 = RANDOM (eagle_strategy.py:858-885; the
                                      GP-UCB-PE default, gp_ucb_pe.py:678-692) */
-  int n_parallel;       /* 0 / 1: a fly is one point.  q > 1 (host-stepped loop only, continuous features, q*Dc <= 64):
+  int n_parallel;       /* 0 / 1: a fly is one point.  q > 1 (host-stepped loop only, continuous features, q <= 16,
+                           q*Dc <= 1024; anything else is VZGP_ERR_ARG):
                            a fly is a SET of q points [q x Dc] scored together (set acquisitions, gp_ucb_pe.py:510-594;
                            vectorized_base.py:331-377): distances and moves over all q*Dc coordinates, forces normalised by
                            Dc, Laplace perturbations normalised over the q members of each coordinate

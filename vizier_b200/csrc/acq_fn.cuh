@@ -15,6 +15,10 @@
 namespace vzgp {
 
 constexpr int kMaxDc = 64;     // continuous feature dims supported by the tile kernels
+// Set flies of the Eagle optimiser (n_parallel = q > 1): at most kMaxSetPoints points of Dc continuous features,
+// q * Dc <= kMaxFlyDim coordinates per fly (k_eagle_suggest_wide walks a fly in 64-column chunks).
+constexpr int kMaxSetPoints = 16;
+constexpr int kMaxFlyDim = 1024;
 constexpr int kMaxMesSamples = 256;   // max-value samples of MaxValueEntropySearch
 
 struct AcqTerm {

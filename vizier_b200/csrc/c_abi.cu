@@ -1144,7 +1144,8 @@ static int eagle_setup(vzgp_handle* h, const vzgp_eagle_config* cfg, const int32
                        int n_prior, EagleDev* pe_, EagleScratch* sc) {
   EagleDev& e = *pe_;
   const int q = cfg->n_parallel > 1 ? cfg->n_parallel : 1;
-  VZ_ARG(q == 1 || (h->dk == 0 && h->dc * q <= kMaxDc), "n_parallel > 1 needs continuous features only and n_parallel * Dc <= 64");
+  VZ_ARG(q == 1 || (h->dk == 0 && q <= kMaxSetPoints && h->dc * q <= kMaxFlyDim),
+         "n_parallel > 1 needs continuous features only, n_parallel <= 16 and n_parallel * Dc <= 1024");
   const int P = cfg->pool_size, B = cfg->batch_size, D = h->dc * q, Dk = h->dk;
   VZ_TRY(check_cat_sizes(h, cat_sizes, e.sizes, &e.smax));
   e.q = q;

@@ -1,5 +1,5 @@
 // Vectorised Eagle/Firefly acquisition optimiser: device-resident population state and the
-// suggest / update / trim / top-k steps (continuous + categorical features, n_parallel == 1).
+// suggest / update / trim / top-k steps (continuous + categorical features; set flies of n_parallel points).
 //
 // Replaces (reference): VectorizedEagleStrategy.init_state/_populate_pool_with_prior_trials
 // (vizier/_src/algorithms/optimizers/eagle_strategy.py:527-713), suggest/_create_features/
@@ -120,6 +120,13 @@ __global__ void __launch_bounds__(256) k_eagle_seed_priors(EagleDev e, const dou
 __global__ void __launch_bounds__(256) k_eagle_suggest(EagleDev e) {
   extern __shared__ double smem[];
   eagle_suggest_block<8>(e, blockIdx.x, smem);
+}
+
+// Set flies wider than kEagleChunk coordinates.  The grid is B / 8 CTAs and a pool of 3000 flies takes 196 KB of shared
+// memory, so one CTA per SM costs nothing and lets ptxas keep the chunk loop in registers (no spills).
+__global__ void __launch_bounds__(256, 1) k_eagle_suggest_wide(EagleDev e) {
+  extern __shared__ double smem[];
+  eagle_suggest_wide<8>(e, blockIdx.x, smem);
 }
 
 __global__ void __launch_bounds__(256) k_eagle_update(EagleDev e) {
@@ -434,7 +441,8 @@ int launch_eagle_seed_priors(vzgp_handle* h, const EagleDev& e, const double* pr
   return 0;
 }
 size_t eagle_suggest_smem(const EagleDev& e) {
-  return sizeof(double) * (size_t)8 * (e.P + e.D) + sizeof(int32_t) * 8 * (size_t)(e.Dk + 2);
+  const int dx = e.D < kEagleChunk ? e.D : kEagleChunk;
+  return sizeof(double) * (size_t)8 * (e.P + dx) + sizeof(int32_t) * 8 * (size_t)(e.Dk + 2);
 }
 size_t eagle_suggest_cta_smem(const EagleDev& e) {
   return sizeof(double) * ((size_t)e.P + e.D + 8 * (size_t)(e.D + 2) + 4 + 64) + sizeof(int32_t) * (size_t)(e.Dk + 2 + 16) + 16;
@@ -443,12 +451,16 @@ size_t eagle_update_smem(const EagleDev& e) {
   return sizeof(double) * (size_t)(e.B + e.count) + (size_t)(e.B + e.count) + 16;
 }
 int eagle_prepare(const EagleDev& e) {
-  VZ_TRY(raise_dyn_smem((const void*)k_eagle_suggest, eagle_suggest_smem(e)));
+  VZ_TRY(raise_dyn_smem(e.D > kEagleChunk ? (const void*)k_eagle_suggest_wide : (const void*)k_eagle_suggest,
+                       eagle_suggest_smem(e)));
   VZ_TRY(raise_dyn_smem((const void*)k_eagle_update, eagle_update_smem(e)));
   return 0;
 }
 int launch_eagle_suggest(vzgp_handle* h, const EagleDev& e) {
-  k_eagle_suggest<<<(e.B + 7) / 8, 256, eagle_suggest_smem(e), h->stream>>>(e);
+  if (e.D > kEagleChunk)
+    k_eagle_suggest_wide<<<(e.B + 7) / 8, 256, eagle_suggest_smem(e), h->stream>>>(e);
+  else
+    k_eagle_suggest<<<(e.B + 7) / 8, 256, eagle_suggest_smem(e), h->stream>>>(e);
   VZ_CHECK_LAUNCH();
   h->launches++;
   return 0;

@@ -218,6 +218,147 @@ __device__ __forceinline__ void eagle_suggest_block(const EagleDev& e, int vbloc
 }
 
 // ---------------------------------------------------------------------------
+// suggest for set flies wider than kEagleChunk coordinates (q * Dc <= kMaxFlyDim, continuous features only): one warp
+// per fly as in eagle_suggest_block, with the fly walked in chunks of kEagleChunk columns so that shared memory holds
+// one chunk of each fly's own features whatever D is.  Every column gets the sums eagle_suggest_block would give it:
+// s_f[j] carries fly j's squared distance from chunk to chunk (the one fma chain over d = 0 .. D-1 of fly_distance),
+// and each chunk's columns take the same j-order partial sums, ssum and eagle_perturbation at the global d.
+// Flies of at most kEagleChunk coordinates stay on eagle_suggest_block: the chunk loop costs it a few per cent at
+// P = 3000 (DESIGN.md 6e).  Dynamic smem: NWARPS * (P + kEagleChunk) doubles.
+// ---------------------------------------------------------------------------
+constexpr int kEagleChunk = 64;
+template <int NWARPS>
+__device__ __forceinline__ void eagle_suggest_wide(const EagleDev& e, int vblock, double* smem) {
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const int P = e.P, B = e.B, D = e.D;
+  const int t = *e.iter;
+  const int nb = P / B;
+  const int start = (t % nb) * B;
+  const int b = vblock * NWARPS + warp;
+  if (b >= B) return;
+  const int i = start + b;
+  const double* xi = e.pool + (size_t)i * D;
+  double* s_f = smem + (size_t)warp * P;
+  double* s_x = smem + (size_t)NWARPS * P + warp * kEagleChunk;
+  double* out = e.batch + (size_t)b * D;
+  if (t < nb) {  // still initialising: return the pool features (projected)
+    for (int d = lane; d < D; d += 32) out[d] = fmin(fmax(xi[d], 0.0), 1.0);
+    return;
+  }
+  const double ri = e.rewards[i];
+  const double cexp = -e.cfg.visibility / (double)e.norm_dim * 10.0;
+  int npull = 0, npush = 0;
+  for (int c0 = 0; c0 < D; c0 += kEagleChunk) {
+    const int w = D - c0 < kEagleChunk ? D - c0 : kEagleChunk;
+    const bool last = c0 + kEagleChunk >= D;
+    __syncwarp();
+    for (int d = lane; d < w; d += 32) s_x[d] = xi[c0 + d];
+    __syncwarp();
+    for (int j = lane; j < P; j += 32) {
+      const double* pj = e.pool + (size_t)j * D + c0;
+      double d2 = c0 > 0 ? s_f[j] : 0.0;
+      for (int d = 0; d < w; ++d) {
+        const double df = s_x[d] - pj[d];
+        d2 = fma(df, df, d2);
+      }
+      if (!last) {
+        s_f[j] = d2;
+        continue;
+      }
+      const double rj = e.rewards[j];
+      const double dir = rj - ri;
+      const double sd = (dir >= 0.0) ? e.cfg.gravity : -e.cfg.negative_gravity;
+      const double f = sd * exp(cexp * d2) * (isfinite(rj) ? 1.0 : 0.0);
+      s_f[j] = f;
+      npull += (f > 0.0);
+      npush += (f < 0.0);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    npull += __shfl_xor_sync(0xffffffffu, npull, o);
+    npush += __shfl_xor_sync(0xffffffffu, npush, o);
+  }
+  __syncwarp();
+  if (e.cfg.mutate_normalization_type == 1) {
+    // RANDOM normalisation (see eagle_suggest_block)
+    double s1 = 0.0, s2 = 0.0;
+    for (int j = lane; j < P; j += 32) {
+      const double pos = s_f[j] > 0.0 ? 1.0 : 0.0;
+      s1 += philox_uniform(e.seed, kStreamPullRand, (uint32_t)t, (uint64_t)b * P + j) * pos;
+      s2 += philox_uniform(e.seed, kStreamPushRand, (uint32_t)t, (uint64_t)b * P + j) * pos;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+      s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    for (int j = lane; j < P; j += 32) {
+      const double f = s_f[j];
+      const double pos = f > 0.0 ? 1.0 : 0.0;
+      const double w1 = s1 > 0.0 ? philox_uniform(e.seed, kStreamPullRand, (uint32_t)t, (uint64_t)b * P + j) * pos / s1 : 0.0;
+      const double w2 = s2 > 0.0 ? philox_uniform(e.seed, kStreamPushRand, (uint32_t)t, (uint64_t)b * P + j) * pos / s2 : 0.0;
+      s_f[j] = e.cfg.normalization_scale * fmax(f, 0.0) * w1 + e.cfg.normalization_scale * fmin(f, 0.0) * w2;
+    }
+  } else {
+    const double wpull = npull > 0 ? e.cfg.normalization_scale / (double)npull : 0.0;
+    const double wpush = npush > 0 ? e.cfg.normalization_scale / (double)npush : 0.0;
+    // convert the forces to the normalised scale in place
+    for (int j = lane; j < P; j += 32) {
+      const double f = s_f[j];
+      s_f[j] = f > 0.0 ? f * wpull : (f < 0.0 ? f * wpush : 0.0);
+    }
+  }
+  __syncwarp();
+  // ---- continuous features, kEagleChunk columns per pass: lane handles columns c0 + lane and c0 + lane + 32 ----
+  const double pert = e.pert[i];
+  for (int c0 = 0; c0 < D; c0 += kEagleChunk) {
+    double acc0, acc1, ssum;
+    const int d0 = c0 + lane, d1 = c0 + lane + 32;
+    {
+      double a0[4] = {0.0, 0.0, 0.0, 0.0}, a1[4] = {0.0, 0.0, 0.0, 0.0}, ss[4] = {0.0, 0.0, 0.0, 0.0};
+      const bool wide = D - c0 > 32;
+      int j = 0;
+      for (; j + 4 <= P; j += 4) {
+        double sc[4], p0[4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          sc[r] = s_f[j + r];
+          p0[r] = d0 < D ? e.pool[(size_t)(j + r) * D + d0] : 0.0;
+        }
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          ss[r] += sc[r];
+          a0[r] = fma(sc[r], p0[r], a0[r]);
+        }
+        if (wide) {
+#pragma unroll
+          for (int r = 0; r < 4; ++r)
+            if (d1 < D) a1[r] = fma(sc[r], e.pool[(size_t)(j + r) * D + d1], a1[r]);
+        }
+      }
+      for (; j < P; ++j) {
+        const double sc = s_f[j];
+        ss[0] += sc;
+        if (d0 < D) a0[0] = fma(sc, e.pool[(size_t)j * D + d0], a0[0]);
+        if (d1 < D) a1[0] = fma(sc, e.pool[(size_t)j * D + d1], a1[0]);
+      }
+      acc0 = (a0[0] + a0[1]) + (a0[2] + a0[3]);
+      acc1 = (a1[0] + a1[1]) + (a1[2] + a1[3]);
+      ssum = (ss[0] + ss[1]) + (ss[2] + ss[3]);
+    }
+    if (d0 < D) {
+      const double v = xi[d0] + (acc0 - xi[d0] * ssum) + eagle_perturbation(e, t, b, d0, pert);
+      out[d0] = fmin(fmax(v, 0.0), 1.0);
+    }
+    if (d1 < D) {
+      const double v = xi[d1] + (acc1 - xi[d1] * ssum) + eagle_perturbation(e, t, b, d1, pert);
+      out[d1] = fmin(fmax(v, 0.0), 1.0);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------
 // suggest, one CTA (NT threads) per batch fly: the same arithmetic as eagle_suggest_block with the
 // loops over the pool spread over the CTA (the one-warp-per-fly form is a ~2000-instruction latency
 // chain; in the cooperative grid kernel there are more CTAs than flies).  Sums over the pool are

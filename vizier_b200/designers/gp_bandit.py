@@ -41,7 +41,8 @@ L-BFGS-B, with `linear_coef` too.  As in the reference it raises ValueError for 
 `ensemble_size > 1`; with `set_priors` or `scoring_function_is_parallel=True` it raises NotImplementedError.
 `scoring_function_is_parallel=True` with a factory returning `QEI`, `QPI` or `QUCB` suggests one set of `count` points
 (gp_bandit.py:496-499): Monte Carlo estimates over each set's joint posterior, scored by `vzgp_score_qsets`
-(csrc/score_q.cu) inside the n_parallel Eagle loop or the random strategy (`optimizers.optimize_qsets`).
+(csrc/score_q.cu) inside the n_parallel Eagle loop (continuous features, `count` <= 16 and `count` * Dc <= 1024) or
+the random strategy (`optimizers.optimize_qsets`).
 Not implemented (the reference supports them; SURVEY 8f "next"): parallel acquisitions for multi-metric models or
 with priors, other acquisition
 functions (Sample, user callables), priors for separable multi-task models; each raises NotImplementedError

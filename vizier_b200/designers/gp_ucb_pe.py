@@ -19,7 +19,7 @@ Everything numeric runs in libvzgp (two handles, or two ensembles, on one stream
 like `VizierGPBandit`.  `prior_acquisition` (a callable on NumPy features) is added to both acquisitions through the
 host-stepped Eagle loop (`gp.SteppedEagle`); `optimize_set_acquisition_for_exploration=True` optimises the rest of a
 batch as ONE set for the set-PE acquisition (`vzgp_score_set_pe`, the optimiser's n_parallel form; continuous search
-spaces with count * Dc <= 64); `mixes_linear_kernel=True` uses the Matern + linear kernel with a constant mean
+spaces with count <= 16 and count * Dc <= 1024); `mixes_linear_kernel=True` uses the Matern + linear kernel with a constant mean
 (`linear_coef = 1`, libvzgp's general scoring path).
 
 Multi-metric studies (up to 8 metrics, gp_ucb_pe.py:344-381, :434-492, :701-722, :917-942) use one default output

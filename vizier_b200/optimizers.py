@@ -23,6 +23,11 @@ import numpy as np
 
 from vizier_b200 import _lib, ard, gp
 
+MAX_SET_POINTS = 16      # points of one set fly (n_parallel)
+MAX_FLY_DIM = 1024       # coordinates of one set fly: n_parallel * Dc
+_SET_LIMITS = (f'set acquisitions need the Eagle strategy, continuous features, n_parallel <= {MAX_SET_POINTS} and '
+               f'n_parallel * Dc <= {MAX_FLY_DIM}')
+
 
 @dataclasses.dataclass(frozen=True)
 class EagleStrategyConfig:
@@ -144,8 +149,7 @@ class VectorizedOptimizer:
     import torch
     q, d = int(n_parallel), self.n_continuous
     if isinstance(self.strategy_factory, _RandomStrategyFactory):
-      raise NotImplementedError('set acquisitions need the Eagle strategy, continuous features, n_parallel * Dc <= 64 '
-                                'and n_parallel <= 16')
+      raise NotImplementedError(_SET_LIMITS)
 
     def score(xs_flat):          # [B, q * Dc] device -> [B] device
       with torch.cuda.stream(dev._stream):
@@ -170,9 +174,8 @@ class VectorizedOptimizer:
     grouped into n // q consecutive sets (vectorized_base.py:108-122).  Returns the best set [q, Dc] and its score."""
     import torch
     d = self.n_continuous
-    if self.n_categorical > 0 or q * d > 64 or q > 16:
-      raise NotImplementedError('set acquisitions need the Eagle strategy, continuous features, n_parallel * Dc <= 64 '
-                                'and n_parallel <= 16')
+    if self.n_categorical > 0 or q > MAX_SET_POINTS or q * d > MAX_FLY_DIM:
+      raise NotImplementedError(_SET_LIMITS)
     cfg = self._eagle_config()
     cfg.n_parallel = q
     lead = getattr(dev, 'members', [dev])[0]     # an ensemble's optimiser state lives on its first member
@@ -197,7 +200,7 @@ class VectorizedOptimizer:
     """`acquisition_optimizer(scoring_fn.score, ..., count=1, n_parallel=q)` with a parallel acquisition (QEI / QPI /
     QUCB; vectorized_base.py:331-377): sets of q points scored by `score_qsets` (dev: DeviceGP or EnsembleGP) with
     one acquisition seed for the whole run, so the draws depend on a set's position in its batch
-    (vectorized_base.py:382-404, :504-520).  Eagle: continuous features, n_parallel * Dc <= 64.  Random strategy: a
+    (vectorized_base.py:382-404, :504-520).  Eagle: continuous features, n_parallel * Dc <= 1024.  Random strategy: a
     Philox pool of n_sets * q points (any features), scored at once, device top-1.  Returns the best set: features
     [q, Dc], categorical [q, Dk], rewards [q] (the set's acquisition value repeated), aux per point."""
     import torch
