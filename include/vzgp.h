@@ -166,7 +166,11 @@ int64_t vzgp_launch_count(const vzgp_handle* h);
  * kernel) are scored by the wgmma integer-split kernel, 0 = always the FP64 DMMA kernel, -1 = the process
  * default (environment VZGP_SCORE_I8, default 0).
  * "small_tiles": pools of at most this many 64-candidate tiles take the small-pool kernels (0 = never), -1 = the
- * process default (environment VZGP_SMALL_TILES, default 8). */
+ * process default (environment VZGP_SMALL_TILES, default 8).
+ * "eagle_perturbation": ContinuousFeaturePerturbationType of every Eagle loop later started on the handle that owns
+ * it (vzgp_eagle_run* and vzgp_eagle_begin; eagle_strategy.py:101-108, :917-935): 0 = ADDITIVE (default), the new
+ * feature is moved + p; 1 = MULTIPLICATIVE, moved * exp(p).  p is the fly's continuous perturbation, single points
+ * and set flies alike, and the result is clipped to [0, 1] as before. */
 int vzgp_set_int(vzgp_handle* h, const char* key, int value);
 
 /* Route the last scoring call on a handle took (vzgp_get_int key "score_route"; -1 before the first one).
@@ -533,7 +537,9 @@ typedef struct vzgp_eagle_config {
   double pure_categorical_perturbation_factor;  /* 30.0 (no continuous feature) */
   double prob_same_category_without_perturbation; /* 0.98 */
   int mutate_normalization_type;  /* 0 = MEAN (default), 1 = RANDOM (eagle_strategy.py:858-885; the
-                                     GP-UCB-PE default, gp_ucb_pe.py:678-692) */
+                                     GP-UCB-PE default, gp_ucb_pe.py:678-692), 2 = UNNORMALIZED (:886-891, the raw
+                                     forces move continuous features and enter the categorical logits).  Any other
+                                     value is VZGP_ERR_ARG. */
   int n_parallel;       /* 0 / 1: a fly is one point.  q > 1 (host-stepped loop only, continuous features, q <= 16,
                            q*Dc <= 1024; anything else is VZGP_ERR_ARG):
                            a fly is a SET of q points [q x Dc] scored together (set acquisitions, gp_ucb_pe.py:510-594;
@@ -546,7 +552,7 @@ typedef struct vzgp_eagle_config {
  * (vectorized_base.py:324-542; eagle_strategy.py:527-1247) scoring against
  * the fitted model.  prior [n_prior x Dc] / prior_z [n_prior x Dk] device (may
  * be NULL/0) are the observed trials in creation order.  cat_sizes (host, [Dk])
- * = number of categories of each categorical feature (<= 64).  best_x
+ * = number of categories of each categorical feature (>= 1, no upper bound).  best_x
  * [count x Dc], best_z [count x Dk], best_score [count] are HOST outputs, best
  * first.  Randomness: Philox4x32-10 keyed by `seed`.
  * Execution: the whole loop runs on the device - one persistent single-CTA kernel (N <= 64 trials,

@@ -668,6 +668,11 @@ int vzgp_set_int(vzgp_handle* h, const char* key, int value) {
   if (std::strcmp(key, "dataflow_ctas") == 0) { VZ_ARG(value >= 0, "value >= 0"); h->df_ctas = value; return 0; }
   if (std::strcmp(key, "score_i8") == 0) { VZ_ARG(value >= -1 && value <= 1, "value in {-1, 0, 1}"); h->score_i8 = value; return 0; }
   if (std::strcmp(key, "small_tiles") == 0) { VZ_ARG(value >= -1, "value >= -1"); h->small_tiles = value; return 0; }
+  if (std::strcmp(key, "eagle_perturbation") == 0) {
+    VZ_ARG(value == 0 || value == 1, "value in {0 = ADDITIVE, 1 = MULTIPLICATIVE}");
+    h->eagle_perturbation = value;
+    return 0;
+  }
   set_error("vzgp_set_int: unknown key '%s'", key);
   return VZGP_ERR_ARG;
 }
@@ -1074,7 +1079,7 @@ static int check_cat_sizes(const vzgp_handle* h, const int32_t* cat_sizes, int* 
   if (h->dk == 0) return 0;
   VZ_ARG(cat_sizes != nullptr, "cat_sizes is required when the model has categorical features");
   for (int k = 0; k < h->dk; ++k) {
-    VZ_ARG(cat_sizes[k] >= 1 && cat_sizes[k] <= 64, "1 <= cat_sizes[k] <= 64");
+    VZ_ARG(cat_sizes[k] >= 1, "cat_sizes[k] >= 1");
     sizes[k] = cat_sizes[k];
     if (sizes[k] > *smax) *smax = sizes[k];
   }
@@ -1180,6 +1185,7 @@ static int eagle_setup(vzgp_handle* h, const vzgp_eagle_config* cfg, const int32
   e.best_z = ip; ip += (size_t)count * Dk;
   e.tmp_z = ip; ip += (size_t)count * Dk;
   e.P = P; e.B = B; e.D = D; e.Dk = Dk; e.count = count; e.cfg = *cfg; e.seed = seed;
+  e.pert_mult = h->eagle_perturbation;
   return eagle_prepare(e);
 }
 static int eagle_check_config(const vzgp_handle* h, const vzgp_eagle_config* cfg, int count) {
@@ -1189,6 +1195,8 @@ static int eagle_check_config(const vzgp_handle* h, const vzgp_eagle_config* cfg
   VZ_ARG(cfg->batch_size <= 8192, "batch_size <= 8192");
   VZ_ARG(count >= 1 && count <= kMaxTopk, "count");
   VZ_ARG(cfg->max_evaluations >= 1, "max_evaluations");
+  VZ_ARG(cfg->mutate_normalization_type >= 0 && cfg->mutate_normalization_type <= 2,
+         "mutate_normalization_type in {0 = MEAN, 1 = RANDOM, 2 = UNNORMALIZED}");
   (void)h;
   return 0;
 }

@@ -197,6 +197,9 @@ struct vzgp_handle {
   // Form of the last Eagle loop on this handle (vzgp_eagle_route); -1 before the first.  A cooperative launch that was
   // refused records the graph form that ran instead.  Tests read it through vzgp_get_int.
   int eagle_route = -1;
+  // ContinuousFeaturePerturbationType of the Eagle loops started on this handle (vzgp_set_int "eagle_perturbation"):
+  // 0 = ADDITIVE, 1 = MULTIPLICATIVE.  Copied into EagleDev when a loop starts.
+  int eagle_perturbation = 0;
 
   // Acquisition function set by vzgp_set_acquisition (c_abi.cu); without one the calls score UCB with their
   // vzgp_acq.ucb_coefficient.  Read at every call: no launch state is built from it.

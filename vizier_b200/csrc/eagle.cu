@@ -445,7 +445,7 @@ size_t eagle_suggest_smem(const EagleDev& e) {
   return sizeof(double) * (size_t)8 * (e.P + dx) + sizeof(int32_t) * 8 * (size_t)(e.Dk + 2);
 }
 size_t eagle_suggest_cta_smem(const EagleDev& e) {
-  return sizeof(double) * ((size_t)e.P + e.D + 8 * (size_t)(e.D + 2) + 4 + 64) + sizeof(int32_t) * (size_t)(e.Dk + 2 + 16) + 16;
+  return sizeof(double) * ((size_t)e.P + e.D + 8 * (size_t)(e.D + 2) + 4) + sizeof(int32_t) * (size_t)(e.Dk + 2 + 16) + 16;
 }
 size_t eagle_update_smem(const EagleDev& e) {
   return sizeof(double) * (size_t)(e.B + e.count) + (size_t)(e.B + e.count) + 16;

@@ -40,6 +40,11 @@ __device__ __forceinline__ double eagle_perturbation(const EagleDev& e, int t, i
   }
   return big > 0.0 ? mine / big * pert : 0.0;
 }
+// The new continuous feature from the moved one (eagle_strategy.py:917-935): ADDITIVE moved + p, MULTIPLICATIVE
+// moved * exp(p).  The caller clips the result to [0, 1].
+__device__ __forceinline__ double eagle_perturb(const EagleDev& e, double moved, double p) {
+  return e.pert_mult ? moved * exp(p) : moved + p;
+}
 __device__ __forceinline__ int uniform_category(double u, int size) {
   const int c = (int)(u * (double)size);
   return c < size - 1 ? c : size - 1;
@@ -126,7 +131,7 @@ __device__ __forceinline__ void eagle_suggest_block(const EagleDev& e, int vbloc
       const double w2 = s2 > 0.0 ? philox_uniform(e.seed, kStreamPushRand, (uint32_t)t, (uint64_t)b * P + j) * pos / s2 : 0.0;
       s_f[j] = e.cfg.normalization_scale * fmax(f, 0.0) * w1 + e.cfg.normalization_scale * fmin(f, 0.0) * w2;
     }
-  } else {
+  } else if (e.cfg.mutate_normalization_type == 0) {   // MEAN; UNNORMALIZED (2, :886-891) keeps the raw forces
     const double wpull = npull > 0 ? e.cfg.normalization_scale / (double)npull : 0.0;
     const double wpush = npush > 0 ? e.cfg.normalization_scale / (double)npush : 0.0;
     // convert the forces to the normalised scale in place
@@ -174,14 +179,15 @@ __device__ __forceinline__ void eagle_suggest_block(const EagleDev& e, int vbloc
   }
   const double pert = e.pert[i];
   if (d0 < D) {
-    const double v = s_x[d0] + (acc0 - s_x[d0] * ssum) + eagle_perturbation(e, t, b, d0, pert);
+    const double v = eagle_perturb(e, s_x[d0] + (acc0 - s_x[d0] * ssum), eagle_perturbation(e, t, b, d0, pert));
     out[d0] = fmin(fmax(v, 0.0), 1.0);
   }
   if (d1 < D) {
-    const double v = s_x[d1] + (acc1 - s_x[d1] * ssum) + eagle_perturbation(e, t, b, d1, pert);
+    const double v = eagle_perturb(e, s_x[d1] + (acc1 - s_x[d1] * ssum), eagle_perturbation(e, t, b, d1, pert));
     out[d1] = fmin(fmax(v, 0.0), 1.0);
   }
-  // ---- categorical features (eagle_strategy.py:936-1011): lane = category (and lane+32) ----
+  // ---- categorical features (eagle_strategy.py:936-1011): lane takes categories lane, lane + 32, ... (any size);
+  // each lane keeps its best category, the lowest index winning ties, and the warp reduces them the same way ----
   const double factor = D > 0 ? e.cfg.categorical_perturbation_factor : e.cfg.pure_categorical_perturbation_factor;
   const double log_same = Dk > 0 ? log(e.cfg.prob_same_category_without_perturbation) : 0.0;
   for (int k = 0; k < Dk; ++k) {
@@ -193,19 +199,15 @@ __device__ __forceinline__ void eagle_suggest_block(const EagleDev& e, int vbloc
     const double log_diff = log((1.0 - e.cfg.prob_same_category_without_perturbation) / ((double)size - 1.0));
     double best_v = -INFINITY;
     int best_c = INT_MAX;
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      const int c = lane + 32 * half;
-      if (c < size) {
-        double lg = 0.0;
-        for (int j = 0; j < P; ++j) lg += (e.pool_z[(size_t)j * Dk + k] == c) ? s_f[j] : 0.0;
-        lg += log_diff;
-        if (c == s_z[k]) lg += -ssum + log_same - log_diff;
-        const uint64_t el = ((uint64_t)b * Dk + k) * e.smax + c;
-        lg += laplace_from_uniform(philox_uniform(e.seed, kStreamCatLaplace, (uint32_t)t, el)) * factor * pert;
-        lg += gumbel_from_uniform(philox_uniform(e.seed, kStreamCatGumbel, (uint32_t)t, el));
-        if (lg > best_v || (lg == best_v && c < best_c)) { best_v = lg; best_c = c; }
-      }
+    for (int c = lane; c < size; c += 32) {
+      double lg = 0.0;
+      for (int j = 0; j < P; ++j) lg += (e.pool_z[(size_t)j * Dk + k] == c) ? s_f[j] : 0.0;
+      lg += log_diff;
+      if (c == s_z[k]) lg += -ssum + log_same - log_diff;
+      const uint64_t el = ((uint64_t)b * Dk + k) * e.smax + c;
+      lg += laplace_from_uniform(philox_uniform(e.seed, kStreamCatLaplace, (uint32_t)t, el)) * factor * pert;
+      lg += gumbel_from_uniform(philox_uniform(e.seed, kStreamCatGumbel, (uint32_t)t, el));
+      if (lg > best_v || (lg == best_v && c < best_c)) { best_v = lg; best_c = c; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -300,7 +302,7 @@ __device__ __forceinline__ void eagle_suggest_wide(const EagleDev& e, int vblock
       const double w2 = s2 > 0.0 ? philox_uniform(e.seed, kStreamPushRand, (uint32_t)t, (uint64_t)b * P + j) * pos / s2 : 0.0;
       s_f[j] = e.cfg.normalization_scale * fmax(f, 0.0) * w1 + e.cfg.normalization_scale * fmin(f, 0.0) * w2;
     }
-  } else {
+  } else if (e.cfg.mutate_normalization_type == 0) {   // MEAN; UNNORMALIZED (2, :886-891) keeps the raw forces
     const double wpull = npull > 0 ? e.cfg.normalization_scale / (double)npull : 0.0;
     const double wpush = npush > 0 ? e.cfg.normalization_scale / (double)npush : 0.0;
     // convert the forces to the normalised scale in place
@@ -348,11 +350,11 @@ __device__ __forceinline__ void eagle_suggest_wide(const EagleDev& e, int vblock
       ssum = (ss[0] + ss[1]) + (ss[2] + ss[3]);
     }
     if (d0 < D) {
-      const double v = xi[d0] + (acc0 - xi[d0] * ssum) + eagle_perturbation(e, t, b, d0, pert);
+      const double v = eagle_perturb(e, xi[d0] + (acc0 - xi[d0] * ssum), eagle_perturbation(e, t, b, d0, pert));
       out[d0] = fmin(fmax(v, 0.0), 1.0);
     }
     if (d1 < D) {
-      const double v = xi[d1] + (acc1 - xi[d1] * ssum) + eagle_perturbation(e, t, b, d1, pert);
+      const double v = eagle_perturb(e, xi[d1] + (acc1 - xi[d1] * ssum), eagle_perturbation(e, t, b, d1, pert));
       out[d1] = fmin(fmax(v, 0.0), 1.0);
     }
   }
@@ -376,8 +378,7 @@ __device__ __forceinline__ void eagle_suggest_cta(const EagleDev& e, int b, doub
   double* s_x = s_f + P;                       // [D]
   double* s_part = s_x + D;                    // [NW][D + 2]  per-warp partial sums
   double* s_bc = s_part + NW * (D + 2);        // [4] broadcast scalars
-  double* s_lg = s_bc + 4;                     // [64] categorical logits
-  int32_t* s_z = reinterpret_cast<int32_t*>(s_lg + 64);   // [Dk]
+  int32_t* s_z = reinterpret_cast<int32_t*>(s_bc + 4);    // [Dk]
   int* s_cnt = s_z + Dk + (Dk & 1);            // [2 * NW]
   for (int d = tid; d < D; d += NT) s_x[d] = e.pool[(size_t)i * D + d];
   for (int d = tid; d < Dk; d += NT) s_z[d] = e.pool_z[(size_t)i * Dk + d];
@@ -437,7 +438,7 @@ __device__ __forceinline__ void eagle_suggest_cta(const EagleDev& e, int b, doub
       const double w2 = s2 > 0.0 ? philox_uniform(e.seed, kStreamPushRand, (uint32_t)t, (uint64_t)b * P + j) * pos / s2 : 0.0;
       s_f[j] = e.cfg.normalization_scale * fmax(f, 0.0) * w1 + e.cfg.normalization_scale * fmin(f, 0.0) * w2;
     }
-  } else {
+  } else if (e.cfg.mutate_normalization_type == 0) {   // MEAN; UNNORMALIZED (2, :886-891) keeps the raw forces
     const double wpull = npull > 0 ? e.cfg.normalization_scale / (double)npull : 0.0;
     const double wpush = npush > 0 ? e.cfg.normalization_scale / (double)npush : 0.0;
     for (int j = tid; j < P; j += NT) {
@@ -469,10 +470,12 @@ __device__ __forceinline__ void eagle_suggest_cta(const EagleDev& e, int b, doub
     double acc = 0.0;
     for (int w = 0; w < NW; ++w) acc += s_part[w * (D + 2) + d];
     const double u = philox_uniform(e.seed, kStreamPerturbSign, (uint32_t)t, (uint64_t)b * D + d);
-    const double v = s_x[d] + (acc - s_x[d] * ssum) + (u >= 0.5 ? pert : -pert);
+    const double v = eagle_perturb(e, s_x[d] + (acc - s_x[d] * ssum), u >= 0.5 ? pert : -pert);
     out[d] = fmin(fmax(v, 0.0), 1.0);
   }
-  // ---- categorical features: warp w takes categories w, w + NW, ...; lanes sum over the pool ----
+  // ---- categorical features: warp w takes categories w, w + NW, ... (any size); lanes sum over the pool.  Each warp
+  // keeps its best category and thread 0 takes the best of the warps', the lowest index winning ties.  s_part and
+  // s_cnt, free once the continuous features are written, carry the warps' winners. ----
   if (Dk > 0) {
     const double factor = D > 0 ? e.cfg.categorical_perturbation_factor : e.cfg.pure_categorical_perturbation_factor;
     const double log_same = log(e.cfg.prob_same_category_without_perturbation);
@@ -484,6 +487,8 @@ __device__ __forceinline__ void eagle_suggest_cta(const EagleDev& e, int b, doub
         continue;
       }
       const double log_diff = log((1.0 - e.cfg.prob_same_category_without_perturbation) / ((double)size - 1.0));
+      double best_v = -INFINITY;
+      int best_c = INT_MAX;
       for (int c = warp; c < size; c += NW) {
         double lg = 0.0;
         for (int j = lane; j < P; j += 32) lg += (e.pool_z[(size_t)j * Dk + k] == c) ? s_f[j] : 0.0;
@@ -495,16 +500,17 @@ __device__ __forceinline__ void eagle_suggest_cta(const EagleDev& e, int b, doub
           const uint64_t el = ((uint64_t)b * Dk + k) * e.smax + c;
           lg += laplace_from_uniform(philox_uniform(e.seed, kStreamCatLaplace, (uint32_t)t, el)) * factor * pert;
           lg += gumbel_from_uniform(philox_uniform(e.seed, kStreamCatGumbel, (uint32_t)t, el));
-          s_lg[c] = lg;
+          if (lg > best_v) { best_v = lg; best_c = c; }   // ascending c: the first of equal logits stays
         }
       }
+      if (lane == 0) { s_part[warp] = best_v; s_cnt[warp] = best_c; }
       __syncthreads();
       if (tid == 0) {
-        double best_v = -INFINITY;
-        int best_c = 0;
-        for (int c = 0; c < size; ++c)
-          if (s_lg[c] > best_v) { best_v = s_lg[c]; best_c = c; }
-        outz[k] = best_c;
+        double bv = -INFINITY;
+        int bc = INT_MAX;
+        for (int w = 0; w < NW; ++w)
+          if (s_part[w] > bv || (s_part[w] == bv && s_cnt[w] < bc)) { bv = s_part[w]; bc = s_cnt[w]; }
+        outz[k] = bc;
       }
     }
   }

@@ -205,6 +205,7 @@ struct EagleDev {
   int P, B, D, Dk, smax, count;
   int norm_dim;   // feature dimensions of ONE point (Dc + Dk of the model): normalises the force exponent
   int q;          // points per fly (n_parallel); D = q * Dc
+  int pert_mult;  // ContinuousFeaturePerturbationType: 0 ADDITIVE (moved + p), 1 MULTIPLICATIVE (moved * exp(p))
   int sizes[kMaxDk];
   vzgp_eagle_config cfg;
   uint64_t seed;

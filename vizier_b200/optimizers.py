@@ -16,6 +16,7 @@ evaluated on the device (`vzgp_score_grad`), one batched call per round.
 from __future__ import annotations
 
 import dataclasses
+import enum
 import math
 from typing import Callable, Dict, Optional, Union
 
@@ -27,6 +28,19 @@ MAX_SET_POINTS = 16      # points of one set fly (n_parallel)
 MAX_FLY_DIM = 1024       # coordinates of one set fly: n_parallel * Dc
 _SET_LIMITS = (f'set acquisitions need the Eagle strategy, continuous features, n_parallel <= {MAX_SET_POINTS} and '
                f'n_parallel * Dc <= {MAX_FLY_DIM}')
+
+
+class MutateNormalizationType(enum.IntEnum):
+  """How the forces on a fly are normalised (eagle_strategy.py:92-98, :847-896)."""
+  MEAN = 0          # pulls and pushes each divided by the number of flies exerting them
+  RANDOM = 1        # random convex weights over the pulling flies
+  UNNORMALIZED = 2  # the raw forces
+
+
+class ContinuousFeaturePerturbationType(enum.IntEnum):
+  """How the perturbation enters a moved continuous feature (eagle_strategy.py:101-108, :917-935)."""
+  ADDITIVE = 0        # moved + perturbation
+  MULTIPLICATIVE = 1  # moved * exp(perturbation)
 
 
 @dataclasses.dataclass(frozen=True)
@@ -45,7 +59,14 @@ class EagleStrategyConfig:
   max_pool_size: int = 100
   normalization_scale: float = 0.5
   prior_trials_pool_pct: float = 0.96
-  mutate_normalization_type: int = 0   # 0 = MEAN (default), 1 = RANDOM (MutateNormalizationType)
+  mutate_normalization_type: int = MutateNormalizationType.MEAN
+  continuous_feature_perturbation_type: int = ContinuousFeaturePerturbationType.ADDITIVE
+
+  def __post_init__(self):
+    # ValueError for a value the enums do not name, as the reference raises when it builds the features (:892-896,
+    # :931-935); plain integers stay accepted.
+    MutateNormalizationType(self.mutate_normalization_type)
+    ContinuousFeaturePerturbationType(self.continuous_feature_perturbation_type)
 
 
 @dataclasses.dataclass(frozen=True)
@@ -101,6 +122,11 @@ class VectorizedOptimizer:
                             c.categorical_perturbation_factor, c.pure_categorical_perturbation_factor,
                             c.prob_same_category_without_perturbation, c.mutate_normalization_type)
 
+  def _set_perturbation(self, owner) -> None:
+    """The perturbation type is a setting of the handle that owns the Eagle loop (vzgp_set_int "eagle_perturbation"):
+    set before every run so that no earlier optimiser's choice carries over."""
+    owner.set_int('eagle_perturbation', int(self.strategy_factory.eagle_config.continuous_feature_perturbation_type))
+
   def _stepped_eagle(self, dev, acq, count, prior_features, prior_categorical, seed, other, prior_acquisition):
     """Eagle with the batch scored here: device acquisition + the caller's `prior_acquisition(continuous [m, Dc],
     categorical [m, Dk]) -> [m]` evaluated on the host (gp_ucb_pe.py:376-379, :487-490).  One D2H + H2D round trip
@@ -123,6 +149,7 @@ class VectorizedOptimizer:
         return out['score'] + torch.as_tensor(vals, dtype=torch.float64, device=dev.device)
 
     n_prior = 0 if prior_features is None else len(prior_features)
+    self._set_perturbation(dev._lead() if hasattr(dev, '_lead') else dev)
     se = gp.SteppedEagle(dev, self._eagle_config(), count, seed, n_prior, list(self.categorical_sizes))
     if n_prior > 0:
       pt = dev._dev(prior_features, torch.float64)
@@ -180,6 +207,7 @@ class VectorizedOptimizer:
     cfg.n_parallel = q
     lead = getattr(dev, 'members', [dev])[0]     # an ensemble's optimiser state lives on its first member
     n_sets = 0 if prior_features is None else len(prior_features) // q
+    self._set_perturbation(lead)
     se = gp.SteppedEagle(lead, cfg, 1, seed, n_sets)
     if n_sets > 0:
       ps = np.ascontiguousarray(np.asarray(prior_features, np.float64)[: n_sets * q].reshape(n_sets, q * d))
@@ -290,6 +318,7 @@ class VectorizedOptimizer:
       bx, bz, bs, _ = dev.random_search(m, acq, count, seed, cat_sizes=sizes)
     else:
       cfg = self._eagle_config()
+      self._set_perturbation(dev._lead() if hasattr(dev, '_lead') else dev)
       bx, bz, bs = dev.eagle_run(cfg, acq, count, seed, prior=prior_features, prior_z=prior_categorical,
                                  cat_sizes=sizes, other=other)
     if is_pe:
