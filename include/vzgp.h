@@ -25,6 +25,10 @@
  *    not.
  *  - Categorical features (int32, Hamming term of the kernel) are accepted by
  *    every entry point through (Z, Dk); pass NULL / 0 when absent.
+ *    0 <= Dk <= 1024 (VZGP_ERR_ARG beyond), 0 <= Dc <= 64.  Models with Dk > 32
+ *    stage their categorical features 32 at a time and are scored on
+ *    VZGP_ROUTE_GENERAL; their Eagle loops run as the replayed graph.
+ *    vzgp_score_qsets takes Dk <= 32.
  */
 #ifndef VZGP_H_
 #define VZGP_H_
@@ -181,7 +185,8 @@ typedef enum vzgp_score_route {
   VZGP_ROUTE_SPLIT = 1,    /* 2 * tiles <= SMs: k_score, score_nsplit CTAs per tile, then k_score_finalize */
   VZGP_ROUTE_CLUSTER = 2,  /* every other pool: k_score in 2-CTA clusters */
   VZGP_ROUTE_I8 = 3,       /* "score_i8" on and eligible: k_score_i8 */
-  VZGP_ROUTE_GENERAL = 4   /* linear_coef models: explicit K* and W, k_general_finalize; every vzgp_score_qsets call */
+  VZGP_ROUTE_GENERAL = 4   /* linear_coef models and Dk > 32: explicit K* and W, k_general_finalize; every
+                              vzgp_score_qsets call */
 } vzgp_score_route;
 
 /* Route the last NLL + gradient evaluation on a handle took (vzgp_get_int key "nll_route"; -1 before the first).
@@ -732,7 +737,7 @@ int vzgp_random_search(vzgp_handle* h, int64_t M, int64_t index_base, const vzgp
  * uses (stream STREAM_RANDOM_POOL), for parity tests and the benchmark. */
 int vzgp_random_pool(vzgp_handle* h, int64_t M, int Dc, int64_t index_base, uint64_t seed,
                      double* X);
-/* Categorical counterpart: Z [M x Dk] int32 device, uniform over [0, cat_sizes[k]). */
+/* Categorical counterpart: Z [M x Dk] int32 device, uniform over [0, cat_sizes[k]), 1 <= Dk <= 1024. */
 int vzgp_random_pool_cat(vzgp_handle* h, int64_t M, int Dk, const int32_t* cat_sizes,
                          int64_t index_base, uint64_t seed, int32_t* Z);
 

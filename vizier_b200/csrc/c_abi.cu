@@ -41,13 +41,17 @@ constexpr size_t kOffClamp = 0;      // int
 constexpr size_t kOffFlag = 8;       // int
 constexpr size_t kOffLogdet = 64;    // double[3]: M sum log L_ii, quadratic form / 2, sum alpha
 constexpr size_t kOffGrad = 5120;    // double[<= 2 kMaxDc + kMaxDk + 8] (the free 3 KiB below kOffPartial)
-constexpr int kMaxGrad = 2 * kMaxDc + kMaxDk + 8;
+constexpr int kMaxGrad = 2 * kMaxDc + kMaxDkWide + 8;
 constexpr size_t kOffTopIdx = 1024;  // long long[256]
 constexpr size_t kOffTopVal = 3072;  // double[256]
 constexpr size_t kOffPartial = 8192; // ArgMax[<=2048] = 32 KiB
 constexpr size_t kOffRows = 40960;   // winner rows of the fused top-k calls (24 KiB)
 constexpr size_t kRowsBytes = kSmallBytes - kOffRows;
 constexpr int kMaxTopk = 256;
+// The gradient sums of models with Dk > kMaxDk (4 + kMaxGrad doubles) follow the 64 KiB layout.
+constexpr size_t kOffGradWide = kSmallBytes;
+constexpr size_t kSmallAlloc = kOffGradWide + sizeof(double) * (4 + kMaxGrad);
+static size_t grad_off(int dk) { return dk > kMaxDk ? kOffGradWide : kOffGrad; }
 
 struct Guard {
   int prev = -1;
@@ -181,7 +185,7 @@ static int fit_common(vzgp_handle* h, const double* X, const int32_t* Z, const d
   VZ_ARG(Z != nullptr || dk == 0, "Z");
   VZ_ARG(y != nullptr, "y");
   KernelParams kp;
-  VZ_TRY(fill_kernel_params(p, dc, dk, &kp));
+  VZ_TRY(fill_kernel_params(p, dc, dk, &kp, &h->wk, h->stream));
   const int np = round_up(N, kBlk);
   VZ_TRY(ensure_model_buffers(h, np, dc, dk, n_metrics));
   h->fitted = false; h->i8_ready = false; h->model_gen++;
@@ -228,7 +232,7 @@ static int nll_sequence(vzgp_handle* h, const double* X, const int32_t* Z, const
   h->nll_factor_route = h->factor_route;
   VZ_TRY(solve_alphas(h, y, N, n_valid, np, n_metrics, 0.0, df));
   double* out2 = reinterpret_cast<double*>(h->small.as<char>() + kOffLogdet);
-  double* gout = reinterpret_cast<double*>(h->small.as<char>() + kOffGrad);
+  double* gout = reinterpret_cast<double*>(h->small.as<char>() + grad_off(dk));
   VZ_TRY(launch_logdet_quad(h, h->L.as<double>(), np, N, n_valid, h->ypad.as<double>() + np, out2, 4 * np, n_metrics));
   if (!df) VZ_TRY(launch_lauum(h, h->Linv.as<double>(), np, h->Kinv.as<double>(), np, np));
   VZ_TRY(launch_nll_grad_tiles(h, h->X.as<double>(), h->Z.as<int32_t>(), np, n_valid, kp, h->Kinv.as<double>(), np,
@@ -250,7 +254,7 @@ static int nll_graph_eval(vzgp_handle* h, const double* X, const int32_t* Z, con
   static const bool enabled = [] { const char* e = getenv("VZGP_NLL_GRAPH"); return !(e && e[0] == '0'); }();
   if (!enabled) return 1;
   KernelParams kp;
-  VZ_TRY(fill_kernel_params(p, dc, dk, &kp));
+  VZ_TRY(fill_kernel_params(p, dc, dk, &kp, &h->wk, h->stream));
   double sn2 = p->observation_noise_variance;
   const int np = round_up(N, kBlk), nq = dc + dk + 2;
   auto bufs = [&](const void** o) {
@@ -289,7 +293,7 @@ static int nll_graph_eval(vzgp_handle* h, const double* X, const int32_t* Z, con
     cudaGraphGetNodes(graph, nullptr, &nn);
     std::vector<cudaGraphNode_t> nodes(nn);
     cudaGraphGetNodes(graph, nodes.data(), &nn);
-    const void* want[3] = {kernel_matrix_func(), transpose_scale_func(), nll_grad_tiles_func()};
+    const void* want[3] = {kernel_matrix_func(dk > kMaxDk), transpose_scale_func(), nll_grad_tiles_func(dk > kMaxDk)};
     cudaGraphNode_t found[3] = {nullptr, nullptr, nullptr};
     for (size_t i = 0; i < nn; ++i) {
       cudaGraphNodeType ty;
@@ -327,7 +331,7 @@ static int nll_graph_eval(vzgp_handle* h, const double* X, const int32_t* Z, con
   h->launches += h->nll_launches;
   int bad = 0;
   VZ_CUDA(cudaMemcpyAsync(host2, h->small.as<char>() + kOffLogdet, sizeof(double) * 2, cudaMemcpyDeviceToHost, h->stream));
-  VZ_CUDA(cudaMemcpyAsync(hostg, h->small.as<char>() + kOffGrad, sizeof(double) * nq, cudaMemcpyDeviceToHost, h->stream));
+  VZ_CUDA(cudaMemcpyAsync(hostg, h->small.as<char>() + grad_off(dk), sizeof(double) * nq, cudaMemcpyDeviceToHost, h->stream));
   VZ_CUDA(cudaMemcpyAsync(&bad, h->small.as<char>() + kOffFlag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   VZ_CUDA(cudaStreamSynchronize(h->stream));
   h->nll_route = VZGP_NLL_GRAPH; h->factor_route = h->nll_factor_route;
@@ -385,7 +389,7 @@ static int nll_eager_raw(vzgp_handle* h, const double* X, const int32_t* Z, cons
   const int np = h->np, nq = Dc + Dk + 2 + (lin ? Dc + 2 : 0);
   VZ_TRY(h->Kinv.reserve(sizeof(double) * (size_t)np * np * kLauumSplit));   // partial planes of K_y^-1
   double* out2 = reinterpret_cast<double*>(h->small.as<char>() + kOffLogdet);
-  double* gout = reinterpret_cast<double*>(h->small.as<char>() + kOffGrad);
+  double* gout = reinterpret_cast<double*>(h->small.as<char>() + grad_off(Dk));
   double* w = h->ypad.as<double>() + np;
   VZ_TRY(launch_logdet_quad(h, h->L.as<double>(), np, N, n_valid, w, out2, 4 * np, n_metrics, h->alpha.as<double>()));
   VZ_TRY(launch_lauum(h, h->Linv.as<double>(), np, h->Kinv.as<double>(), np, np));
@@ -617,9 +621,9 @@ int vzgp_create(int device, void* stream, vzgp_handle** out) {
   }
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) h->sm_count = prop.multiProcessorCount;
-  int s = h->small.reserve(kSmallBytes);
+  int s = h->small.reserve(kSmallAlloc);
   if (s < 0) { delete h; return s; }
-  cudaMemsetAsync(h->small.ptr, 0, kSmallBytes, h->stream);
+  cudaMemsetAsync(h->small.ptr, 0, kSmallAlloc, h->stream);
   *out = h;
   return 0;
 }
@@ -633,7 +637,7 @@ int vzgp_destroy(vzgp_handle* h) {
   for (DevBuf* b : {&h->X, &h->Z, &h->L, &h->Linv, &h->alpha, &h->ypad, &h->Kws, &h->Tws, &h->Kinv, &h->XT,
                     &h->scratch, &h->small, &h->xs_dev, &h->out_dev, &h->eagle, &h->pe_tmp, &h->pe_multi_tmp,
                     &h->LinvT, &h->df_tasks[0], &h->df_tasks[1], &h->df_flags, &h->df_S, &h->scal, &h->gen,
-                    &h->i8_planes, &h->i8_scale, &h->i8_kdig, &h->sep_y})
+                    &h->i8_planes, &h->i8_scale, &h->i8_kdig, &h->sep_y, &h->wk, &h->wk_scratch, &h->cat_sizes})
     b->release();
   eagle_step_free(h);
   if (h->pinned) cudaFreeHost(h->pinned);
@@ -755,7 +759,7 @@ int vzgp_kernel_matrix(vzgp_handle* h, const double* X, const int32_t* Z, int N,
   VZ_ARG(n_valid >= 0 && n_valid <= N, "n_valid");
   Guard g(h->device);
   KernelParams kp;
-  VZ_TRY(fill_kernel_params(p, Dc, Dk, &kp));
+  VZ_TRY(fill_kernel_params(p, Dc, Dk, &kp, &h->wk_scratch, h->stream));
   return launch_kernel_matrix(h, X, Z, N, n_valid, kp, diag_add, K, ldk);
 }
 
@@ -766,7 +770,7 @@ int vzgp_cross_kernel(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M
   VZ_ARG(M >= 1 && N >= 1 && ldks >= N, "M, N, ldks");
   Guard g(h->device);
   KernelParams kp;
-  VZ_TRY(fill_kernel_params(p, Dc, Dk, &kp));
+  VZ_TRY(fill_kernel_params(p, Dc, Dk, &kp, &h->wk_scratch, h->stream));
   return launch_cross_kernel(h, Xs, Zs, M, X, Z, N, N, kp, Ks, ldks);
 }
 
@@ -902,7 +906,7 @@ int vzgp_nll_grad_multi(vzgp_handle* h, const double* X, const int32_t* Z, const
   static const bool small_ok = [] { const char* e = getenv("VZGP_NLL_SMALL"); return !(e && e[0] == '0'); }();
   const bool lin = p->linear_coef != 0.0;
   VZ_ARG(!lin || n_metrics == 1, "linear_coef with several metrics is not implemented");
-  if (N <= kBlk && small_ok && n_metrics == 1 && !lin) {
+  if (N <= kBlk && small_ok && n_metrics == 1 && !lin && nll_small_smem_bytes(Dc, Dk) <= kMaxDynSmem) {
     // Small studies: the whole evaluation is one single-CTA kernel (nll_small.cu).  The handle's
     // fitted model is not touched (ARD callers refit with the chosen parameters afterwards).
     VZ_ARG(N >= 1 && n_valid >= 1 && n_valid <= N, "1 <= n_valid <= N");
@@ -910,9 +914,9 @@ int vzgp_nll_grad_multi(vzgp_handle* h, const double* X, const int32_t* Z, const
     VZ_ARG(Z != nullptr || Dk == 0, "Z");
     VZ_ARG(y != nullptr, "y");
     KernelParams kp;
-    VZ_TRY(fill_kernel_params(p, Dc, Dk, &kp));
+    VZ_TRY(fill_kernel_params(p, Dc, Dk, &kp, &h->wk_scratch, h->stream));
     const int nq = Dc + Dk + 2;
-    double* dout = reinterpret_cast<double*>(h->small.as<char>() + kOffGrad);   // 4 + nq doubles
+    double* dout = reinterpret_cast<double*>(h->small.as<char>() + grad_off(Dk));   // 4 + nq doubles
     VZ_TRY(launch_nll_grad_small(h, X, Z, y, N, n_valid, kp, p->observation_noise_variance, 1e-4, 5, dout));
     double host[4 + kMaxGrad];
     VZ_CUDA(cudaMemcpyAsync(host, dout, sizeof(double) * (4 + nq), cudaMemcpyDeviceToHost, h->stream));
@@ -1073,9 +1077,10 @@ int vzgp_random_pool(vzgp_handle* h, int64_t M, int Dc, int64_t index_base, uint
   return launch_random_fill(h, X, M * Dc, index_base * Dc, seed, 3u, 0u);
 }
 
+// sizes: [kMaxDkWide].
 static int check_cat_sizes(const vzgp_handle* h, const int32_t* cat_sizes, int* sizes, int* smax) {
   *smax = 0;
-  for (int k = 0; k < kMaxDk; ++k) sizes[k] = 1;
+  for (int k = 0; k < kMaxDkWide; ++k) sizes[k] = 1;
   if (h->dk == 0) return 0;
   VZ_ARG(cat_sizes != nullptr, "cat_sizes is required when the model has categorical features");
   for (int k = 0; k < h->dk; ++k) {
@@ -1089,9 +1094,9 @@ static int check_cat_sizes(const vzgp_handle* h, const int32_t* cat_sizes, int* 
 int vzgp_random_pool_cat(vzgp_handle* h, int64_t M, int Dk, const int32_t* cat_sizes, int64_t index_base,
                          uint64_t seed, int32_t* Z) {
   VZ_ARG(h && Z && cat_sizes, "handle / Z / cat_sizes");
-  VZ_ARG(M >= 0 && Dk >= 1 && Dk <= kMaxDk, "M, Dk");
+  VZ_ARG(M >= 0 && Dk >= 1 && Dk <= kMaxDkWide, "M, Dk (1 <= Dk <= 1024)");
   Guard g(h->device);
-  int sizes[kMaxDk];
+  int sizes[kMaxDkWide];
   for (int k = 0; k < Dk; ++k) {
     VZ_ARG(cat_sizes[k] >= 1, "cat_sizes[k] >= 1");
     sizes[k] = cat_sizes[k];
@@ -1110,7 +1115,7 @@ int vzgp_random_search(vzgp_handle* h, int64_t M, int64_t index_base, const vzgp
   VZ_ARG(best_z != nullptr || h->dk == 0, "best_z");
   Guard g(h->device);
   const int dc = h->dc, dk = h->dk;
-  int sizes[kMaxDk], smax;
+  int sizes[kMaxDkWide], smax;
   VZ_TRY(check_cat_sizes(h, cat_sizes, sizes, &smax));
   const size_t xb = sizeof(double) * (size_t)M * (dc > 0 ? dc : 1);
   VZ_TRY(h->xs_dev.reserve(xb + sizeof(int32_t) * (size_t)M * (dk > 0 ? dk : 1) + 64));
@@ -1152,14 +1157,17 @@ static int eagle_setup(vzgp_handle* h, const vzgp_eagle_config* cfg, const int32
   VZ_ARG(q == 1 || (h->dk == 0 && q <= kMaxSetPoints && h->dc * q <= kMaxFlyDim),
          "n_parallel > 1 needs continuous features only, n_parallel <= 16 and n_parallel * Dc <= 1024");
   const int P = cfg->pool_size, B = cfg->batch_size, D = h->dc * q, Dk = h->dk;
-  VZ_TRY(check_cat_sizes(h, cat_sizes, e.sizes, &e.smax));
+  int sizes[kMaxDkWide];
+  VZ_TRY(check_cat_sizes(h, cat_sizes, sizes, &e.smax));
+  for (int k = 0; k < kMaxDk; ++k) e.sizes[k] = sizes[k];
+  const size_t nw = Dk > kMaxDk ? (size_t)Dk : 0;   // device category counts of a wide model
   e.q = q;
   e.norm_dim = h->dc + h->dk;
   // carve the eagle buffer: doubles | long longs | ints
   const size_t np1 = (size_t)(n_prior > 0 ? n_prior : 1);
   const size_t nd = (size_t)P * D + 2 * (size_t)P + 8 + (size_t)B * D + B + 2 * ((size_t)count * D + count) + np1 + P;
   const size_t nl = 2 * (size_t)count;
-  const size_t ni = 16 + np1 + (size_t)P * Dk + (size_t)B * Dk + 2 * (size_t)count * Dk;
+  const size_t ni = 16 + np1 + (size_t)P * Dk + (size_t)B * Dk + 2 * (size_t)count * Dk + nw;
   VZ_TRY(h->eagle.reserve(nd * sizeof(double) + nl * sizeof(long long) + ni * sizeof(int32_t) + 64));
   double* p = h->eagle.as<double>();
   e.pool = p; p += (size_t)P * D;
@@ -1184,8 +1192,15 @@ static int eagle_setup(vzgp_handle* h, const vzgp_eagle_config* cfg, const int32
   e.batch_z = ip; ip += (size_t)B * Dk;
   e.best_z = ip; ip += (size_t)count * Dk;
   e.tmp_z = ip; ip += (size_t)count * Dk;
+  e.sizes_wide = nullptr;
+  if (nw > 0) {
+    VZ_CUDA(cudaMemcpyAsync(ip, sizes, sizeof(int) * nw, cudaMemcpyHostToDevice, h->stream));
+    VZ_CUDA(cudaStreamSynchronize(h->stream));   // `sizes` is on this stack
+    e.sizes_wide = ip; ip += nw;
+  }
   e.P = P; e.B = B; e.D = D; e.Dk = Dk; e.count = count; e.cfg = *cfg; e.seed = seed;
   e.pert_mult = h->eagle_perturbation;
+  VZ_ARG(eagle_suggest_smem(e) <= kMaxDynSmem, "pool_size and Dk: the suggest step needs more than 227 KiB of shared memory");
   return eagle_prepare(e);
 }
 static int eagle_check_config(const vzgp_handle* h, const vzgp_eagle_config* cfg, int count) {
@@ -1771,8 +1786,6 @@ static int nll_batch_eval(vzgp_handle* const* hs, int R, const double* X, const 
   const size_t res_bytes = sizeof(double) * (2 + nq) + sizeof(int) * 2;
   if (!lead->batch) lead->batch = new BatchGraph();
   BatchGraph* b = static_cast<BatchGraph*>(lead->batch);
-  KernelParams kps[kMaxBatch];
-  for (int r = 0; r < R; ++r) VZ_TRY(fill_kernel_params(&ps[r], Dc, Dk, &kps[r]));
   // ---- is the captured graph still valid? ----
   bool hit = b->exec && b->key_ptr[0] == X && b->key_ptr[1] == Z && b->key_dims[0] == N &&
              b->key_dims[1] == Dc && b->key_dims[2] == Dk && b->key_dims[3] == n_valid && b->key_dims[4] == n_metrics &&
@@ -1783,6 +1796,11 @@ static int nll_batch_eval(vzgp_handle* const* hs, int R, const double* X, const 
     hit = b->hs[r] == hs[r] && b->key_y[r] == Ys[r] && hs[r]->df_nb[1] == np / 64;
     for (int q = 0; hit && q < kNllBufs; ++q) hit = cur[q] == b->bufs[r][q];
   }
+  // A capture records every branch, so every branch needs its parameters then; a replay updates the active ones only,
+  // and a handle's wide length scales (hs[r]->wk) change together with its kernel nodes and hs[r]->kp.
+  KernelParams kps[kMaxBatch];
+  for (int r = 0; r < R; ++r)
+    if (!hit || !active || active[r]) VZ_TRY(fill_kernel_params(&ps[r], Dc, Dk, &kps[r], &hs[r]->wk, hs[r]->stream));
   if (!hit) {
     batch_drop(b);
     if (!b->fork) {
@@ -1815,7 +1833,7 @@ static int nll_batch_eval(vzgp_handle* const* hs, int R, const double* X, const 
       if (st < 0) break;
       char* pin = static_cast<char*>(h->pinned);
       cudaMemcpyAsync(pin, h->small.as<char>() + kOffLogdet, sizeof(double) * 2, cudaMemcpyDeviceToHost, h->stream);
-      cudaMemcpyAsync(pin + 16, h->small.as<char>() + kOffGrad, sizeof(double) * nq, cudaMemcpyDeviceToHost, h->stream);
+      cudaMemcpyAsync(pin + 16, h->small.as<char>() + grad_off(Dk), sizeof(double) * nq, cudaMemcpyDeviceToHost, h->stream);
       cudaMemcpyAsync(pin + 16 + sizeof(double) * nq, h->small.as<char>() + kOffFlag, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
       if (r > 0) { cudaEventRecord(b->join[r], h->stream); cudaStreamWaitEvent(lead->stream, b->join[r], 0); }
     }
@@ -1835,7 +1853,7 @@ static int nll_batch_eval(vzgp_handle* const* hs, int R, const double* X, const 
     cudaGraphGetNodes(graph, nullptr, &nn);
     std::vector<cudaGraphNode_t> nodes(nn);
     cudaGraphGetNodes(graph, nodes.data(), &nn);
-    const void* want[3] = {kernel_matrix_func(), transpose_scale_func(), nll_grad_tiles_func()};
+    const void* want[3] = {kernel_matrix_func(Dk > kMaxDk), transpose_scale_func(), nll_grad_tiles_func(Dk > kMaxDk)};
     const int id_arg[3] = {6, 4, 5};       // output / workspace pointer that tells the R branches apart
     for (int r = 0; r < R; ++r) for (int q = 0; q < 3; ++q) b->nodes[r][q] = nullptr;
     for (size_t i = 0; i < nn; ++i) {
@@ -2174,7 +2192,7 @@ int vzgp_nll_grad_separable_batch(vzgp_handle* const* hs, int R, int M, const do
       VZ_CUDA(cudaMemcpyAsync(packed + (size_t)j * np, hs[r * M + j]->alpha.ptr, sizeof(double) * np,
                               cudaMemcpyDeviceToDevice, lead->stream));
     KernelParams kp;
-    VZ_TRY(fill_kernel_params(&ps[r], Dc, Dk, &kp));
+    VZ_TRY(fill_kernel_params(&ps[r], Dc, Dk, &kp, &hr->wk_scratch, lead->stream));
     kp.sf2 = 1.0;
     VZ_TRY(launch_task_gram(lead, hr->X.as<double>(), hr->Z.as<int32_t>(), np, n_valid, kp, packed, M, ka, gd));
     VZ_CUDA(cudaMemcpyAsync(&gram[(size_t)r * MM], gd, sizeof(double) * M * M, cudaMemcpyDeviceToHost, lead->stream));

@@ -15,8 +15,11 @@
 namespace vzgp {
 
 constexpr int kBlk = 64;       // padding / factorisation block size
-constexpr int kMaxDk = 32;     // categorical feature dims
+constexpr int kMaxDk = 32;     // categorical feature dims held in KernelParams; wider models take the tiled kernels
+constexpr int kMaxDkWide = 1024;   // categorical feature dims of any model
+constexpr int kCatTile = 32;       // categorical features the tiled (wide) kernels stage in shared memory at a time
 constexpr int kMaxMetrics = 8; // metrics of the independent multi-task GP (one factor, several alpha)
+constexpr size_t kMaxDynSmem = 227 * 1024;   // dynamic shared memory of one sm_90 CTA
 constexpr int kNllBufs = 15;   // handle buffers a captured NLL graph points into
 
 void set_error(const char* fmt, ...);
@@ -95,7 +98,8 @@ struct KernelParams {
   double sf2;
   double inv_ls2_c[kMaxDc];
   double inv_ls_c[kMaxDc];   // sqrt(inv_ls2_c): the reference's FeatureScaled divides by the length scale
-  double inv_ls2_k[kMaxDk];
+  double inv_ls2_k[kMaxDk];      // dk <= kMaxDk
+  const double* inv_ls2_k_wide;  // dk > kMaxDk: device array [dk] owned by a handle (fill_kernel_params); else null
   // linear_coef variant: k += lin_a * sum_d (x_d inv_ls_c[d] - lin_b)(x'_d inv_ls_c[d] - lin_b)
   int use_linear;
   double lin_a, lin_b;
@@ -132,6 +136,11 @@ struct vzgp_handle {
   vzgp::DevBuf LinvT;  // [np x np] L^-T (upper), produced by the dataflow factorisation (dataflow.cu)
   vzgp::DevBuf alpha;  // [n_metrics][np]
   vzgp::DevBuf ypad;   // [n_metrics][4][np]: y, w = Linv y, r, tmp
+  // Models with more than kMaxDk categorical features: the inverse categorical length scales [kMaxDkWide] that kp
+  // points to (allocated once, so captured graphs keep one address), and the same for the calls that must not
+  // overwrite the fitted model's (stand-alone kernel matrices, the N <= 64 NLL kernel, the separable task Gram).
+  // cat_sizes: the category counts of the random candidate pools (launch_random_fill_cat).
+  vzgp::DevBuf wk, wk_scratch, cat_sizes;
 
   // Workspaces.
   vzgp::DevBuf Kws;     // [np x np] kernel matrix / temporaries

@@ -28,7 +28,7 @@ __global__ void k_eagle_init(EagleDev e) {
   const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = tid; i < total; i += nth) e.pool[i] = philox_uniform(e.seed, kStreamInitPool, 0, (uint64_t)i);
   for (int64_t i = tid; i < (int64_t)e.P * e.Dk; i += nth)
-    e.pool_z[i] = uniform_category(philox_uniform(e.seed, kStreamInitCat, 0, (uint64_t)i), e.sizes[i % e.Dk]);
+    e.pool_z[i] = uniform_category(philox_uniform(e.seed, kStreamInitCat, 0, (uint64_t)i), cat_size(e, (int)(i % e.Dk)));
   for (int64_t i = tid; i < e.P; i += nth) {
     e.rewards[i] = -INFINITY;
     e.pert[i] = e.cfg.perturbation;
@@ -408,13 +408,17 @@ __global__ void __launch_bounds__(kPThreads) k_eagle_persistent64(const EagleDev
 }
 
 // Z[m, k] = uniform category of feature k for candidate index_base+m (RandomVectorizedStrategy).
+// WIDE (dk > kMaxDk): the sizes come from the device array sizes_wide.
 struct CatSizes { int v[kMaxDk]; };
+template <bool WIDE>
 __global__ void k_random_pool_cat(int32_t* __restrict__ Z, int64_t total, int dk, CatSizes sizes,
-                                  int64_t elem_base, uint64_t seed, uint32_t stream) {
+                                  const int* __restrict__ sizes_wide, int64_t elem_base, uint64_t seed, uint32_t stream) {
   int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (; e < total; e += stride)
-    Z[e] = uniform_category(philox_uniform(seed, stream, 0, (uint64_t)(elem_base + e)), sizes.v[(elem_base + e) % dk]);
+  for (; e < total; e += stride) {
+    const int k = (int)((elem_base + e) % dk);
+    Z[e] = uniform_category(philox_uniform(seed, stream, 0, (uint64_t)(elem_base + e)), WIDE ? sizes_wide[k] : sizes.v[k]);
+  }
 }
 
 __global__ void k_gather_rows_i32(const int32_t* __restrict__ Z, int dk, const long long* __restrict__ idx,
@@ -477,6 +481,7 @@ static size_t eagle_persistent_state_bytes(const EagleDev& e) {
 }
 
 bool eagle_persistent_eligible(const vzgp_handle* h, const vzgp_handle* hB, const EagleDev& e) {
+  if (e.Dk > kMaxDk) return false;   // dk x kPXLD slabs in shared memory
   static const bool enabled = [] { const char* v = getenv("VZGP_EAGLE_PERSISTENT"); return !(v && v[0] == '0'); }();
   const bool linear = h->kp.use_linear || (hB != nullptr && hB->kp.use_linear);   // in-kernel scoring knows Matern only
   return enabled && !linear && h->np == 64 && (hB == nullptr || hB->np == 64) && e.B <= 64 &&
@@ -516,7 +521,7 @@ int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e
   const size_t sm = sizeof(double) * (scratch + (size_t)(nm + 1) * 64 * kPLD + (size_t)(nm + 1) * h->dc * kPXLD +
                                       (size_t)nm * 64 + 128 + 128 + 64 + 256) +
                     sizeof(int32_t) * ((size_t)(nm + 1) * h->dk * kPXLD + 2) + eagle_persistent_state_bytes(e);
-  if (sm > 227 * 1024) { set_error("persistent eagle kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
+  if (sm > kMaxDynSmem) { set_error("persistent eagle kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
   if (q.pe_mode < 0 && !acq_fn_is_ucb(q.fn)) {
     VZ_TRY(raise_dyn_smem((const void*)k_eagle_persistent64<true>, sm));
     k_eagle_persistent64<true><<<1, kPThreads, sm, h->stream>>>(e, m, mb, q, steps, scratch, h->small.as<int>());
@@ -535,9 +540,16 @@ int launch_random_fill_cat(vzgp_handle* h, int32_t* Z, int64_t M, int dk, const 
   if (total <= 0) return 0;
   CatSizes cs;
   for (int k = 0; k < kMaxDk; ++k) cs.v[k] = k < dk ? sizes[k] : 1;
+  const bool wide = dk > kMaxDk;
+  if (wide) {
+    VZ_TRY(h->cat_sizes.reserve(sizeof(int) * kMaxDkWide));
+    VZ_CUDA(cudaMemcpyAsync(h->cat_sizes.ptr, sizes, sizeof(int) * dk, cudaMemcpyHostToDevice, h->stream));
+    VZ_CUDA(cudaStreamSynchronize(h->stream));   // `sizes` may be a caller's stack array
+  }
   int64_t blocks = (total + 255) / 256;
   if (blocks > (int64_t)h->sm_count * 16) blocks = (int64_t)h->sm_count * 16;
-  k_random_pool_cat<<<(unsigned)blocks, 256, 0, h->stream>>>(Z, total, dk, cs, index_base * dk, seed, stream);
+  (wide ? k_random_pool_cat<true> : k_random_pool_cat<false>)<<<(unsigned)blocks, 256, 0, h->stream>>>(
+      Z, total, dk, cs, h->cat_sizes.as<int>(), index_base * dk, seed, stream);
   VZ_CHECK_LAUNCH();
   h->launches++;
   return 0;

@@ -45,6 +45,8 @@ __device__ __forceinline__ double eagle_perturbation(const EagleDev& e, int t, i
 __device__ __forceinline__ double eagle_perturb(const EagleDev& e, double moved, double p) {
   return e.pert_mult ? moved * exp(p) : moved + p;
 }
+// Number of categories of feature k.
+__device__ __forceinline__ int cat_size(const EagleDev& e, int k) { return e.Dk > kMaxDk ? e.sizes_wide[k] : e.sizes[k]; }
 __device__ __forceinline__ int uniform_category(double u, int size) {
   const int c = (int)(u * (double)size);
   return c < size - 1 ? c : size - 1;
@@ -191,7 +193,7 @@ __device__ __forceinline__ void eagle_suggest_block(const EagleDev& e, int vbloc
   const double factor = D > 0 ? e.cfg.categorical_perturbation_factor : e.cfg.pure_categorical_perturbation_factor;
   const double log_same = Dk > 0 ? log(e.cfg.prob_same_category_without_perturbation) : 0.0;
   for (int k = 0; k < Dk; ++k) {
-    const int size = e.sizes[k];
+    const int size = cat_size(e, k);
     if (size <= 1) {
       if (lane == 0) outz[k] = 0;
       continue;
@@ -480,7 +482,7 @@ __device__ __forceinline__ void eagle_suggest_cta(const EagleDev& e, int b, doub
     const double factor = D > 0 ? e.cfg.categorical_perturbation_factor : e.cfg.pure_categorical_perturbation_factor;
     const double log_same = log(e.cfg.prob_same_category_without_perturbation);
     for (int k = 0; k < Dk; ++k) {
-      const int size = e.sizes[k];
+      const int size = cat_size(e, k);
       __syncthreads();
       if (size <= 1) {
         if (tid == 0) outz[k] = 0;
@@ -616,7 +618,7 @@ __device__ __forceinline__ void eagle_update_block(const EagleDev& e, double* sm
           e.pool[(size_t)i * D + d] = philox_uniform(e.seed, kStreamTrim, (uint32_t)t, (uint64_t)b * D + d);
         for (int d = 0; d < Dk; ++d)
           e.pool_z[(size_t)i * Dk + d] = uniform_category(
-              philox_uniform(e.seed, kStreamTrimCat, (uint32_t)t, (uint64_t)b * Dk + d), e.sizes[d]);
+              philox_uniform(e.seed, kStreamTrimCat, (uint32_t)t, (uint64_t)b * Dk + d), cat_size(e, d));
         pert = e.cfg.perturbation;
         nr = -INFINITY;
       } else if (improve) {

@@ -141,6 +141,7 @@ __global__ void __launch_bounds__(kSmallThreads) k_eagle_grid(const __grid_const
 }
 
 bool eagle_grid_eligible(const vzgp_handle* h, const vzgp_handle* hB, const EagleDev& e) {
+  if (e.Dk > kMaxDk) return false;   // dk x kPXLD slabs in shared memory
   static const bool enabled = [] { const char* v = getenv("VZGP_EAGLE_GRID"); return !(v && v[0] == '0'); }();
   int coop = 0;
   if (cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, h->device) != cudaSuccess) coop = 0;
@@ -183,7 +184,7 @@ int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const 
   if (s_u > sm) sm = s_u;
   if (s_c > sm) sm = s_c;
   if (s_v > sm) sm = s_v;
-  if (sm > 227 * 1024) { set_error("eagle grid kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
+  if (sm > kMaxDynSmem) { set_error("eagle grid kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
   const void* kfn = (!pe && !acq_fn_is_ucb(G.a.acq)) ? (const void*)k_eagle_grid<true> : (const void*)k_eagle_grid<false>;
   VZ_TRY(raise_dyn_smem(kfn, sm));
   int occ = 0;
@@ -346,7 +347,7 @@ int launch_eagle_grid_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* h
   if (s_u > sm) sm = s_u;
   if (s_c > sm) sm = s_c;
   if (s_v > sm) sm = s_v;
-  if (sm > 227 * 1024) { set_error("eagle grid kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
+  if (sm > kMaxDynSmem) { set_error("eagle grid kernel needs %zu bytes of shared memory", sm); return VZGP_ERR_UNSUPPORTED; }
   const void* kfn = (const void*)k_eagle_grid_pe_ensemble;
   VZ_TRY(raise_dyn_smem(kfn, sm));
   int occ = 0;

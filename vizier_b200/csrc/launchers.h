@@ -8,7 +8,10 @@
 
 namespace vzgp {
 
-int fill_kernel_params(const vzgp_params* p, int dc, int dk, KernelParams* kp);
+// Dk > kMaxDk: the inverse categorical length scales go to `wide` (a handle buffer, copied on `stream` before this
+// returns) and kp->inv_ls2_k_wide points there.
+int fill_kernel_params(const vzgp_params* p, int dc, int dk, KernelParams* kp, DevBuf* wide = nullptr,
+                       cudaStream_t stream = nullptr);
 int launch_kernel_matrix(vzgp_handle* h, const double* X, const int32_t* Z, int n, int n_valid,
                          const KernelParams& kp, double diag_add, double* K, int ldk);
 int launch_cross_kernel(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const double* X,
@@ -29,10 +32,11 @@ template <class... A> struct KernelArgs<void (*)(A...)> {
   static constexpr int count = (int)sizeof...(A);
   template <int I> using arg = typename std::tuple_element<I, std::tuple<A...>>::type;
 };
-// Host-side entry addresses of the three kernels whose arguments carry the hyper-parameters (graph node lookup).
-const void* kernel_matrix_func();
+// Host-side entry addresses of the three kernels whose arguments carry the hyper-parameters (graph node lookup);
+// `wide`: the form for Dk > kMaxDk.
+const void* kernel_matrix_func(bool wide);
 const void* transpose_scale_func();
-const void* nll_grad_tiles_func();
+const void* nll_grad_tiles_func(bool wide);
 constexpr int kLauumSplit = 4;   // K_y^-1 is produced as this many partial planes [z][np][ldk] (linalg.cu)
 int lauum_plane_rows(int np);
 int launch_sum_planes(vzgp_handle* h, double* Kinv, int np, int kc);
@@ -167,6 +171,7 @@ int launch_topk_device(vzgp_handle* h, const double* score, int64_t M, int count
 int launch_gather_rows(vzgp_handle* h, const double* X, int dc, const long long* idx, int count,
                        int64_t M, double* out);
 
+size_t nll_small_smem_bytes(int dc, int dk);
 int launch_nll_grad_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int n_valid,
                           const KernelParams& kp, double sn2, double jitter0, int max_iters, double* out);
 // The acquisition and its gradient in the continuous features (score_grad.cu): hs[0..E), E = 1 for one model, scored
@@ -206,7 +211,8 @@ struct EagleDev {
   int norm_dim;   // feature dimensions of ONE point (Dc + Dk of the model): normalises the force exponent
   int q;          // points per fly (n_parallel); D = q * Dc
   int pert_mult;  // ContinuousFeaturePerturbationType: 0 ADDITIVE (moved + p), 1 MULTIPLICATIVE (moved * exp(p))
-  int sizes[kMaxDk];
+  int sizes[kMaxDk];       // Dk <= kMaxDk
+  const int* sizes_wide;   // Dk > kMaxDk: device [Dk] in the handle's eagle buffer; read them through cat_size
   vzgp_eagle_config cfg;
   uint64_t seed;
 };
@@ -245,6 +251,7 @@ size_t eagle_suggest_cta_smem(const EagleDev& e);
 int launch_eagle_init(vzgp_handle* h, const EagleDev& e);
 int launch_eagle_seed_priors(vzgp_handle* h, const EagleDev& e, const double* prior, const int32_t* prior_z,
                              const double* prior_r, int n, int* ord, double* chosen_r);
+// sizes: host [dk]; dk > kMaxDk copies them to h->cat_sizes.
 int launch_random_fill_cat(vzgp_handle* h, int32_t* Z, int64_t M, int dk, const int* sizes, int64_t index_base,
                            uint64_t seed, uint32_t stream);
 int launch_gather_rows_i32(vzgp_handle* h, const int32_t* Z, int dk, const long long* idx, int count, int64_t M,

@@ -15,7 +15,9 @@ using G64 = GemmCfg<64, 64, 16, 4, 4>;  // 256 threads, 4x4 register tile
 // Kernel matrices
 // ---------------------------------------------------------------------------
 // K[i,j] = k(X_i, X_j) + diag_add*[i==j]; rows/cols >= n_valid -> identity.  One CTA per
-// lower-triangular 64x64 tile; the mirrored tile is written too.
+// lower-triangular 64x64 tile; the mirrored tile is written too.  WIDE (Dk > kMaxDk): the categorical features are
+// staged kCatTile at a time (tiles.cuh, for_cat_tiles).
+template <bool WIDE>
 __global__ void __launch_bounds__(256) k_kernel_matrix(const double* __restrict__ X,
                                                        const int32_t* __restrict__ Z, int n,
                                                        int n_valid, KernelParams kp,
@@ -28,17 +30,21 @@ __global__ void __launch_bounds__(256) k_kernel_matrix(const double* __restrict_
   double* sa = smem;
   double* sb = sa + kp.dc * LD;
   int32_t* za = reinterpret_cast<int32_t*>(sb + kp.dc * LD);
-  int32_t* zb = za + kp.dk * LD;
+  int32_t* zb = za + (WIDE ? kCatTile : kp.dk) * LD;
   stage_rows_T(X, n, kp.dc, bi * 64, 64, sa, LD);
   stage_rows_T(X, n, kp.dc, bj * 64, 64, sb, LD);
-  if (kp.dk > 0) {
+  if (!WIDE && kp.dk > 0) {
     stage_rows_T_i32(Z, n, kp.dk, bi * 64, 64, za, LD);
     stage_rows_T_i32(Z, n, kp.dk, bj * 64, 64, zb, LD);
   }
   __syncthreads();
   const int ty = threadIdx.x / 16, tx = threadIdx.x % 16;
   double d2[4][4], unused[4][4];
-  tile_d2<G64, 4, 4, false>(sa, LD, sb, LD, za, LD, zb, LD, kp, nullptr, ty, tx, d2, unused);
+  tile_d2<G64, 4, 4, false, !WIDE>(sa, LD, sb, LD, za, LD, zb, LD, kp, nullptr, ty, tx, d2, unused);
+  if (WIDE)
+    for_cat_tiles(Z, n, bi * 64, 64, Z, n, bj * 64, 64, kp.dk, za, LD, zb, LD, [&](int k0, int kt) {
+      tile_hamming<G64, 4, 4>(za, LD, zb, LD, kp.inv_ls2_k_wide + k0, kt, ty, tx, d2);
+    });
   if (kp.use_linear) tile_lin<G64, 4, 4>(sa, LD, sb, LD, kp, ty, tx, unused);   // `unused` now holds the linear term
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -59,8 +65,9 @@ __global__ void __launch_bounds__(256) k_kernel_matrix(const double* __restrict_
     }
 }
 
-// Ks[m, j] = k(Xs_m, X_j) for m < M, j < n; columns j >= n_valid are written as 0.
+// Ks[m, j] = k(Xs_m, X_j) for m < M, j < n; columns j >= n_valid are written as 0.  WIDE as in k_kernel_matrix.
 using G128x64 = GemmCfg<128, 64, 16, 8, 4>;
+template <bool WIDE>
 __global__ void __launch_bounds__(256) k_cross_kernel(const double* __restrict__ Xs,
                                                       const int32_t* __restrict__ Zs, int M,
                                                       const double* __restrict__ X,
@@ -72,19 +79,23 @@ __global__ void __launch_bounds__(256) k_cross_kernel(const double* __restrict__
   double* sa = smem;
   double* sb = sa + kp.dc * LDA;
   int32_t* za = reinterpret_cast<int32_t*>(sb + kp.dc * LDB);
-  int32_t* zb = za + kp.dk * LDA;
+  int32_t* zb = za + (WIDE ? kCatTile : kp.dk) * LDA;
   const int m0 = blockIdx.y * 128, j0 = blockIdx.x * 64;
   stage_rows_T(Xs, M, kp.dc, m0, 128, sa, LDA);
   stage_rows_T(X, n, kp.dc, j0, 64, sb, LDB);
-  if (kp.dk > 0) {
+  if (!WIDE && kp.dk > 0) {
     stage_rows_T_i32(Zs, M, kp.dk, m0, 128, za, LDA);
     stage_rows_T_i32(Z, n, kp.dk, j0, 64, zb, LDB);
   }
   __syncthreads();
   const int ty = threadIdx.x / 16, tx = threadIdx.x % 16;
   double d2[8][4], unused[8][4];
-  tile_d2<G128x64, 8, 4, false>(sa, LDA, sb, LDB, za, LDA, zb, LDB, kp, nullptr, ty, tx, d2,
-                                unused);
+  tile_d2<G128x64, 8, 4, false, !WIDE>(sa, LDA, sb, LDB, za, LDA, zb, LDB, kp, nullptr, ty, tx, d2,
+                                       unused);
+  if (WIDE)
+    for_cat_tiles(Zs, M, m0, 128, Z, n, j0, 64, kp.dk, za, LDA, zb, LDB, [&](int k0, int kt) {
+      tile_hamming<G128x64, 8, 4>(za, LDA, zb, LDB, kp.inv_ls2_k_wide + k0, kt, ty, tx, d2);
+    });
   if (kp.use_linear) tile_lin<G128x64, 8, 4>(sa, LDA, sb, LDB, kp, ty, tx, unused);
 #pragma unroll
   for (int i = 0; i < 8; ++i)
@@ -466,10 +477,11 @@ static size_t kernel_smem_bytes(int dc, int dk, int rows_a, int rows_b) {
   return sizeof(double) * dc * (rows_a + 2 + rows_b + 2) + sizeof(int32_t) * dk * (rows_a + 2 + rows_b + 2);
 }
 
-int fill_kernel_params(const vzgp_params* p, int dc, int dk, KernelParams* kp) {
+int fill_kernel_params(const vzgp_params* p, int dc, int dk, KernelParams* kp, DevBuf* wide, cudaStream_t stream) {
   VZ_ARG(p != nullptr, "params");
   VZ_ARG(dc >= 0 && dc <= kMaxDc, "Dc out of range [0,64]");
-  VZ_ARG(dk >= 0 && dk <= kMaxDk, "Dk out of range [0,32]");
+  VZ_ARG(dk >= 0 && dk <= kMaxDkWide, "Dk out of range [0,1024]");
+  VZ_ARG(dk <= kMaxDk || wide != nullptr, "Dk > 32 needs a handle buffer for the categorical length scales");
   VZ_ARG(dc + dk > 0, "no features");
   VZ_ARG(dc == 0 || p->continuous_length_scale_squared != nullptr, "continuous length scales");
   VZ_ARG(dk == 0 || p->categorical_length_scale_squared != nullptr, "categorical length scales");
@@ -481,7 +493,18 @@ int fill_kernel_params(const vzgp_params* p, int dc, int dk, KernelParams* kp) {
     kp->inv_ls_c[d] = d < dc ? 1.0 / std::sqrt(p->continuous_length_scale_squared[d]) : 0.0;
   }
   for (int d = 0; d < kMaxDk; ++d)
-    kp->inv_ls2_k[d] = d < dk ? 1.0 / p->categorical_length_scale_squared[d] : 0.0;
+    kp->inv_ls2_k[d] = (d < dk && dk <= kMaxDk) ? 1.0 / p->categorical_length_scale_squared[d] : 0.0;
+  kp->inv_ls2_k_wide = nullptr;
+  if (dk > kMaxDk) {
+    // One allocation of the largest size: the buffer's address is baked into captured graphs.  The copy completes
+    // before this returns, so the caller may launch on any stream (the batched NLL graph forks from another one).
+    std::vector<double> w(dk);
+    for (int d = 0; d < dk; ++d) w[d] = 1.0 / p->categorical_length_scale_squared[d];
+    VZ_TRY(wide->reserve(sizeof(double) * kMaxDkWide));
+    VZ_CUDA(cudaMemcpyAsync(wide->ptr, w.data(), sizeof(double) * dk, cudaMemcpyHostToDevice, stream));
+    VZ_CUDA(cudaStreamSynchronize(stream));
+    kp->inv_ls2_k_wide = wide->as<double>();
+  }
   kp->use_linear = p->linear_coef != 0.0 ? 1 : 0;
   kp->lin_a = kp->use_linear ? (p->linear_coef * p->linear_slope_amplitude) * (p->linear_coef * p->linear_slope_amplitude) : 0.0;
   kp->lin_b = kp->use_linear ? p->linear_coef * p->linear_shift : 0.0;
@@ -489,22 +512,26 @@ int fill_kernel_params(const vzgp_params* p, int dc, int dk, KernelParams* kp) {
 }
 
 // The captured NLL graph re-parameterises these kernels by argument position (c_abi.cu): pin the positions.
-static_assert(KernelArgs<decltype(&k_kernel_matrix)>::count == kKernelMatrixArgs &&
-              std::is_same<KernelArgs<decltype(&k_kernel_matrix)>::arg<kKernelMatrixKpArg>, KernelParams>::value &&
-              std::is_same<KernelArgs<decltype(&k_kernel_matrix)>::arg<kKernelMatrixDiagArg>, double>::value,
+static_assert(KernelArgs<decltype(&k_kernel_matrix<false>)>::count == kKernelMatrixArgs &&
+              std::is_same<KernelArgs<decltype(&k_kernel_matrix<false>)>::arg<kKernelMatrixKpArg>, KernelParams>::value &&
+              std::is_same<KernelArgs<decltype(&k_kernel_matrix<false>)>::arg<kKernelMatrixDiagArg>, double>::value,
               "k_kernel_matrix signature changed: update kKernelMatrix*Arg in launchers.h");
 static_assert(KernelArgs<decltype(&k_transpose_scale)>::count == kTransposeScaleArgs &&
               std::is_same<KernelArgs<decltype(&k_transpose_scale)>::arg<kTransposeScaleKpArg>, KernelParams>::value,
               "k_transpose_scale signature changed: update kTransposeScale*Arg in launchers.h");
-const void* kernel_matrix_func() { return reinterpret_cast<const void*>(&k_kernel_matrix); }
+const void* kernel_matrix_func(bool wide) {
+  return wide ? reinterpret_cast<const void*>(&k_kernel_matrix<true>) : reinterpret_cast<const void*>(&k_kernel_matrix<false>);
+}
 const void* transpose_scale_func() { return reinterpret_cast<const void*>(&k_transpose_scale); }
 
 int launch_kernel_matrix(vzgp_handle* h, const double* X, const int32_t* Z, int n, int n_valid,
                          const KernelParams& kp, double diag_add, double* K, int ldk) {
   int nb = (n + 63) / 64;
-  size_t sm = kernel_smem_bytes(kp.dc, kp.dk, 64, 64);
-  VZ_TRY(raise_dyn_smem((const void*)k_kernel_matrix, sm));
-  k_kernel_matrix<<<dim3(nb, nb), 256, sm, h->stream>>>(X, Z, n, n_valid, kp, diag_add, K, ldk);
+  const bool wide = kp.dk > kMaxDk;
+  size_t sm = kernel_smem_bytes(kp.dc, wide ? kCatTile : kp.dk, 64, 64);
+  const auto kfn = wide ? k_kernel_matrix<true> : k_kernel_matrix<false>;
+  VZ_TRY(raise_dyn_smem((const void*)kfn, sm));
+  kfn<<<dim3(nb, nb), 256, sm, h->stream>>>(X, Z, n, n_valid, kp, diag_add, K, ldk);
   VZ_CHECK_LAUNCH();
   h->launches++;
   return 0;
@@ -513,10 +540,12 @@ int launch_kernel_matrix(vzgp_handle* h, const double* X, const int32_t* Z, int 
 int launch_cross_kernel(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, const double* X,
                         const int32_t* Z, int n, int n_valid, const KernelParams& kp, double* Ks,
                         int ldks) {
-  size_t sm = kernel_smem_bytes(kp.dc, kp.dk, 128, 64);
-  VZ_TRY(raise_dyn_smem((const void*)k_cross_kernel, sm));
+  const bool wide = kp.dk > kMaxDk;
+  size_t sm = kernel_smem_bytes(kp.dc, wide ? kCatTile : kp.dk, 128, 64);
+  const auto kfn = wide ? k_cross_kernel<true> : k_cross_kernel<false>;
+  VZ_TRY(raise_dyn_smem((const void*)kfn, sm));
   dim3 grid((n + 63) / 64, (M + 127) / 128);
-  k_cross_kernel<<<grid, 256, sm, h->stream>>>(Xs, Zs, M, X, Z, n, n_valid, kp, Ks, ldks);
+  kfn<<<grid, 256, sm, h->stream>>>(Xs, Zs, M, X, Z, n, n_valid, kp, Ks, ldks);
   VZ_CHECK_LAUNCH();
   h->launches++;
   return 0;

@@ -19,6 +19,8 @@ namespace vzgp {
 
 using G64 = GemmCfg<64, 64, 16, 4, 4>;
 
+// WIDE (Dk > kMaxDk): the categorical features of both sides are staged kCatTile at a time per trial block (tiles.cuh).
+template <bool WIDE>
 __global__ void __launch_bounds__(256) k_mean_multi(const double* __restrict__ Xs, const int32_t* __restrict__ Zs,
                                                     int M, const double* __restrict__ X, const int32_t* __restrict__ Z,
                                                     int np, int n_valid, KernelParams kp,
@@ -31,11 +33,11 @@ __global__ void __launch_bounds__(256) k_mean_multi(const double* __restrict__ X
   double* sb = sa + dc * LD;               // [dc][LD] trials
   double* sal = sb + dc * LD;              // [n_metrics][64] alpha chunk
   int32_t* za = reinterpret_cast<int32_t*>(sal + kMaxMetrics * 64);
-  int32_t* zb = za + dk * LD;
+  int32_t* zb = za + (WIDE ? kCatTile : dk) * LD;
   const int m0 = blockIdx.x * 64;
   const int tid = threadIdx.x, ty = tid / 16, tx = tid % 16;
   stage_rows_T(Xs, M, dc, m0, 64, sa, LD);
-  if (dk > 0) stage_rows_T_i32(Zs, M, dk, m0, 64, za, LD);
+  if (!WIDE && dk > 0) stage_rows_T_i32(Zs, M, dk, m0, 64, za, LD);
   double acc[4][kMaxMetrics];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -44,14 +46,18 @@ __global__ void __launch_bounds__(256) k_mean_multi(const double* __restrict__ X
   for (int j0 = 0; j0 < n_valid; j0 += 64) {
     __syncthreads();
     stage_rows_T(X, np, dc, j0, 64, sb, LD);
-    if (dk > 0) stage_rows_T_i32(Z, np, dk, j0, 64, zb, LD);
+    if (!WIDE && dk > 0) stage_rows_T_i32(Z, np, dk, j0, 64, zb, LD);
     for (int e = tid; e < n_metrics * 64; e += 256) {
       const int m = e >> 6, c = e & 63;
       sal[m * 64 + c] = (j0 + c < n_valid) ? alpha[(size_t)m * np + j0 + c] : 0.0;
     }
     __syncthreads();
     double d2[4][4], unused[4][4];
-    tile_d2<G64, 4, 4, false>(sa, LD, sb, LD, za, LD, zb, LD, kp, nullptr, ty, tx, d2, unused);
+    tile_d2<G64, 4, 4, false, !WIDE>(sa, LD, sb, LD, za, LD, zb, LD, kp, nullptr, ty, tx, d2, unused);
+    if (WIDE)
+      for_cat_tiles(Zs, M, m0, 64, Z, np, j0, 64, dk, za, LD, zb, LD, [&](int k0, int kt) {
+        tile_hamming<G64, 4, 4>(za, LD, zb, LD, kp.inv_ls2_k_wide + k0, kt, ty, tx, d2);
+      });
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
@@ -197,11 +203,19 @@ int prepare_scalarization(vzgp_handle* h, const vzgp_scalarization* sc, int n_me
   return 0;
 }
 
+// The k_mean_multi form for kp and its dynamic shared memory.
+static auto mean_multi_kernel(const KernelParams& kp, size_t* sm) {
+  const bool wide = kp.dk > kMaxDk;
+  *sm = sizeof(double) * (2 * kp.dc * 66 + kMaxMetrics * 64) + sizeof(int32_t) * 2 * (wide ? kCatTile : kp.dk) * 66;
+  return wide ? k_mean_multi<true> : k_mean_multi<false>;
+}
+
 // mu [n_metrics][M] of the M candidates on the model fitted on `h` (k_mean_multi; not counted in h->launches).
 static int launch_mean_multi(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, double* mu) {
-  const size_t sm = sizeof(double) * (2 * h->dc * 66 + kMaxMetrics * 64) + sizeof(int32_t) * 2 * h->dk * 66;
-  VZ_TRY(raise_dyn_smem((const void*)k_mean_multi, sm));
-  k_mean_multi<<<(M + 63) / 64, 256, sm, h->stream>>>(Xs, Zs, M, h->X.as<double>(), h->Z.as<int32_t>(), h->np, h->n_valid,
+  size_t sm;
+  const auto kfn = mean_multi_kernel(h->kp, &sm);
+  VZ_TRY(raise_dyn_smem((const void*)kfn, sm));
+  kfn<<<(M + 63) / 64, 256, sm, h->stream>>>(Xs, Zs, M, h->X.as<double>(), h->Z.as<int32_t>(), h->np, h->n_valid,
                                                       h->kp, h->alpha.as<double>(), h->n_metrics, mu, M);
   VZ_CHECK_LAUNCH();
   return 0;
@@ -491,9 +505,10 @@ __global__ void __launch_bounds__(256) k_task_gram(const double* __restrict__ al
 // gradient of the task covariance): K A by k_mean_multi with the trials as candidates, then k_task_gram.
 int launch_task_gram(vzgp_handle* h, const double* X, const int32_t* Z, int np, int n_valid, const KernelParams& kp,
                      const double* alphas, int n_tasks, double* ka, double* gram) {
-  const size_t sm = sizeof(double) * (2 * kp.dc * 66 + kMaxMetrics * 64) + sizeof(int32_t) * 2 * kp.dk * 66;
-  VZ_TRY(raise_dyn_smem((const void*)k_mean_multi, sm));
-  k_mean_multi<<<(n_valid + 63) / 64, 256, sm, h->stream>>>(X, Z, n_valid, X, Z, np, n_valid, kp, alphas, n_tasks, ka,
+  size_t sm;
+  const auto kfn = mean_multi_kernel(kp, &sm);
+  VZ_TRY(raise_dyn_smem((const void*)kfn, sm));
+  kfn<<<(n_valid + 63) / 64, 256, sm, h->stream>>>(X, Z, n_valid, X, Z, np, n_valid, kp, alphas, n_tasks, ka,
                                                             np);
   k_task_gram<<<dim3(n_tasks, n_tasks), 256, 0, h->stream>>>(alphas, ka, np, n_valid, gram);
   VZ_CHECK_LAUNCH();

@@ -16,7 +16,9 @@ using G64 = GemmCfg<64, 64, 16, 4, 4>;
 // partial[tile][0..dk) = sum G*E*neq_k, [dk..dk+dc) = sum G*E*diff_d^2, [dk+dc] = trace part of G,
 // [dk+dc+1] = sum G*K_matern; with the linear_coef model (kp.use_linear) three more groups follow:
 // [dk+dc+2 .. +dc) = sum G (x_id u_jd + x_jd u_id), then sum G sum_d u_id u_jd, then sum G sum_d (u_id + u_jd),
-// u_id = x_id / l_d - coef*shift  (the pieces of dK_lin/d ls2_d, d/d slope, d/d shift).
+// u_id = x_id / l_d - coef*shift  (the pieces of dK_lin/d ls2_d, d/d slope, d/d shift).  WIDE (Dk > kMaxDk): the
+// categorical features are staged kCatTile at a time (tiles.cuh), once for d2 and once for their gradient sums.
+template <bool WIDE>
 __global__ void __launch_bounds__(256) k_nll_grad_tiles(const double* __restrict__ X,
                                                         const int32_t* __restrict__ Z, int np,
                                                         int n_valid, KernelParams kp,
@@ -33,17 +35,21 @@ __global__ void __launch_bounds__(256) k_nll_grad_tiles(const double* __restrict
   double* sb = sa + dc * LD;
   double* s_part = sb + dc * LD;                                   // [8 warps][np_out]
   int32_t* za = reinterpret_cast<int32_t*>(s_part + 8 * np_out);
-  int32_t* zb = za + dk * LD;
+  int32_t* zb = za + (WIDE ? kCatTile : dk) * LD;
   stage_rows_T(X, np, dc, bi * 64, 64, sa, LD);
   stage_rows_T(X, np, dc, bj * 64, 64, sb, LD);
-  if (dk > 0) {
+  if (!WIDE && dk > 0) {
     stage_rows_T_i32(Z, np, dk, bi * 64, 64, za, LD);
     stage_rows_T_i32(Z, np, dk, bj * 64, 64, zb, LD);
   }
   __syncthreads();
   const int tid = threadIdx.x, ty = tid / 16, tx = tid % 16, warp = tid / 32, lane = tid % 32;
   double d2[4][4], unused[4][4];
-  tile_d2<G64, 4, 4, false>(sa, LD, sb, LD, za, LD, zb, LD, kp, nullptr, ty, tx, d2, unused);
+  tile_d2<G64, 4, 4, false, !WIDE>(sa, LD, sb, LD, za, LD, zb, LD, kp, nullptr, ty, tx, d2, unused);
+  if (WIDE)
+    for_cat_tiles(Z, np, bi * 64, 64, Z, np, bj * 64, 64, dk, za, LD, zb, LD, [&](int k0, int kt) {
+      tile_hamming<G64, 4, 4>(za, LD, zb, LD, kp.inv_ls2_k_wide + k0, kt, ty, tx, d2);
+    });
   double ge[4][4], gg[4][4];
   double sum_gk = 0.0, sum_tr = 0.0;
   const double wgt = (bi == bj) ? 1.0 : 2.0;
@@ -72,16 +78,20 @@ __global__ void __launch_bounds__(256) k_nll_grad_tiles(const double* __restrict
     for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
     if (lane == 0) s_part[warp * np_out + slot] = v;
   };
-  for (int k = 0; k < dk; ++k) {
-    double t = 0.0;
+  auto cat_sums = [&](int k0, int kt) {
+    for (int k = 0; k < kt; ++k) {
+      double t = 0.0;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int av = za[k * LD + G64::row_of(ty, i)];
+      for (int i = 0; i < 4; ++i) {
+        const int av = za[k * LD + G64::row_of(ty, i)];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) t += (av != zb[k * LD + G64::col_of(tx, j)]) ? ge[i][j] : 0.0;
+        for (int j = 0; j < 4; ++j) t += (av != zb[k * LD + G64::col_of(tx, j)]) ? ge[i][j] : 0.0;
+      }
+      warp_store(t, k0 + k);
     }
-    warp_store(t, k);
-  }
+  };
+  if (WIDE) for_cat_tiles(Z, np, bi * 64, 64, Z, np, bj * 64, 64, dk, za, LD, zb, LD, cat_sums);
+  else cat_sums(0, dk);
   for (int d = 0; d < dc; ++d) {
     double t = 0.0;
 #pragma unroll
@@ -123,12 +133,14 @@ __global__ void __launch_bounds__(256) k_nll_grad_tiles(const double* __restrict
   __syncthreads();
   // tile index in row-major lower-triangular enumeration
   const int tile = bi * (bi + 1) / 2 + bj;
-  if (tid < np_out) {
+  auto slot_sum = [&](int q) {
     double s = 0.0;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) s += s_part[w * np_out + tid];
-    partial[(size_t)tile * np_out + tid] = s;
-  }
+    for (int w = 0; w < 8; ++w) s += s_part[w * np_out + q];
+    partial[(size_t)tile * np_out + q] = s;
+  };
+  if (WIDE) for (int q = tid; q < np_out; q += 256) slot_sum(q);   // np_out > 256 only here
+  else if (tid < np_out) slot_sum(tid);
 }
 
 // out[q] = sum over tiles (fixed order) of partial[tile][q].
@@ -142,18 +154,22 @@ __global__ void k_reduce_partials(const double* __restrict__ partial, int ntiles
   if (threadIdx.x == 0) out[q] = s;
 }
 
-static_assert(KernelArgs<decltype(&k_nll_grad_tiles)>::count == kNllGradTilesArgs &&
-              std::is_same<KernelArgs<decltype(&k_nll_grad_tiles)>::arg<kNllGradTilesKpArg>, KernelParams>::value,
+static_assert(KernelArgs<decltype(&k_nll_grad_tiles<false>)>::count == kNllGradTilesArgs &&
+              std::is_same<KernelArgs<decltype(&k_nll_grad_tiles<false>)>::arg<kNllGradTilesKpArg>, KernelParams>::value,
               "k_nll_grad_tiles signature changed: update kNllGradTiles*Arg in launchers.h");
-const void* nll_grad_tiles_func() { return reinterpret_cast<const void*>(&k_nll_grad_tiles); }
+const void* nll_grad_tiles_func(bool wide) {
+  return wide ? reinterpret_cast<const void*>(&k_nll_grad_tiles<true>) : reinterpret_cast<const void*>(&k_nll_grad_tiles<false>);
+}
 
 int launch_nll_grad_tiles(vzgp_handle* h, const double* X, const int32_t* Z, int np, int n_valid,
                           const KernelParams& kp, const double* Kinv, int ldk, const double* alpha,
                           double* partial, double* out, int plane_rows, int n_metrics) {
   const int nb = np / 64, nq = kp.dc + kp.dk + 2 + (kp.use_linear ? kp.dc + 2 : 0), ntiles = nb * (nb + 1) / 2;
-  size_t sm = sizeof(double) * (kp.dc * 2 * 66 + 8 * nq) + sizeof(int32_t) * kp.dk * 2 * 66;
-  VZ_TRY(raise_dyn_smem((const void*)k_nll_grad_tiles, sm));
-  k_nll_grad_tiles<<<dim3(nb, nb), 256, sm, h->stream>>>(X, Z, np, n_valid, kp, Kinv, ldk, plane_rows > 0 ? plane_rows : lauum_plane_rows(np), alpha,
+  const bool wide = kp.dk > kMaxDk;
+  size_t sm = sizeof(double) * (kp.dc * 2 * 66 + 8 * nq) + sizeof(int32_t) * (wide ? kCatTile : kp.dk) * 2 * 66;
+  const auto kfn = wide ? k_nll_grad_tiles<true> : k_nll_grad_tiles<false>;
+  VZ_TRY(raise_dyn_smem((const void*)kfn, sm));
+  kfn<<<dim3(nb, nb), 256, sm, h->stream>>>(X, Z, np, n_valid, kp, Kinv, ldk, plane_rows > 0 ? plane_rows : lauum_plane_rows(np), alpha,
                                                          partial, nb, n_metrics, np);
   VZ_CHECK_LAUNCH();
   k_reduce_partials<<<nq, 256, 0, h->stream>>>(partial, ntiles, nq, out);

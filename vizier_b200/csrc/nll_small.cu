@@ -11,6 +11,7 @@
 #include "launchers.h"
 #include "device.cuh"
 #include "potf2.cuh"
+#include "tiles.cuh"
 
 namespace vzgp {
 
@@ -27,7 +28,11 @@ __device__ __forceinline__ double warp_sum(double v) {
 // out: [0] = sum_i log L_ii (i < N), [1] = 0.5 * |L^-1 y|^2, [2] = shift used, [3] = retries
 //      (max_iters + 1 = never succeeded), [4 .. 4 + nq) = raw gradient sums in the order
 //      categorical (G E neq_k), continuous (G E diff_d^2), trace(G), sum(G K).
-__global__ void __launch_bounds__(256) k_nll_grad_small(const double* __restrict__ X, const int32_t* __restrict__ Z,
+// WIDE (Dk > kMaxDk): the categorical features are staged kCatTile at a time (tiles.cuh), and d2 takes the Hamming
+// term tile by tile in ascending feature order, the order of the one-pass sum.  Without a minimum of one CTA per SM
+// ptxas holds the wide form to 64 registers and spills.
+template <bool WIDE>
+__global__ void __launch_bounds__(256, WIDE ? 1 : 0) k_nll_grad_small(const double* __restrict__ X, const int32_t* __restrict__ Z,
                                                         const double* __restrict__ y, int N, int n_valid,
                                                         KernelParams kp, double sn2, double jitter0, int max_iters,
                                                         double* __restrict__ out) {
@@ -46,7 +51,7 @@ __global__ void __launch_bounds__(256) k_nll_grad_small(const double* __restrict
   double* tv = rv + 64;              // [64]
   double* rd = tv + 64;              // [64]
   double* s_part = rd + 64;          // [8][nq]
-  int32_t* zt = reinterpret_cast<int32_t*>(s_part + 8 * nq);   // [dk][66]
+  int32_t* zt = reinterpret_cast<int32_t*>(s_part + 8 * nq);   // [dk][66]  (WIDE: [kCatTile][66])
   __shared__ int s_bad;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
@@ -54,7 +59,7 @@ __global__ void __launch_bounds__(256) k_nll_grad_small(const double* __restrict
     const int i = e / dc, d = e - i * dc;
     xt[d * kLD + i] = i < N ? X[(size_t)i * dc + d] : 0.0;
   }
-  for (int e = tid; e < 64 * dk; e += 256) {
+  for (int e = tid; !WIDE && e < 64 * dk; e += 256) {
     const int i = e / dk, k = e - i * dk;
     zt[k * kLD + i] = i < N ? Z[(size_t)i * dk + k] : -1;
   }
@@ -68,12 +73,31 @@ __global__ void __launch_bounds__(256) k_nll_grad_small(const double* __restrict
       const double df = xt[d * kLD + i] - xt[d * kLD + j];
       s = fma(df * df, kp.inv_ls2_c[d], s);
     }
-    for (int k = 0; k < dk; ++k) s += (zt[k * kLD + i] != zt[k * kLD + j]) ? kp.inv_ls2_k[k] : 0.0;
+    if (!WIDE)
+      for (int k = 0; k < dk; ++k) s += (zt[k * kLD + i] != zt[k * kLD + j]) ? kp.inv_ls2_k[k] : 0.0;
     d2m[i * kLD + j] = s;
+    if (WIDE) continue;
     double v;
     if (i >= n_valid || j >= n_valid) v = (i == j) ? 1.0 : 0.0;
     else { v = matern52(s, kp.sf2); if (i == j) v += sn2; }
     ky[i * kLD + j] = v;
+  }
+  if (WIDE) {
+    for_cat_tiles(Z, N, 0, 64, nullptr, 0, 0, 0, dk, zt, kLD, nullptr, 0, [&](int k0, int kt) {
+      for (int e = tid; e < 64 * 64; e += 256) {
+        const int i = e >> 6, j = e & 63;
+        double s = d2m[i * kLD + j];
+        for (int k = 0; k < kt; ++k) s += (zt[k * kLD + i] != zt[k * kLD + j]) ? __ldg(kp.inv_ls2_k_wide + k0 + k) : 0.0;
+        d2m[i * kLD + j] = s;
+      }
+    });
+    for (int e = tid; e < 64 * 64; e += 256) {
+      const int i = e >> 6, j = e & 63;
+      double v;
+      if (i >= n_valid || j >= n_valid) v = (i == j) ? 1.0 : 0.0;
+      else { v = matern52(d2m[i * kLD + j], kp.sf2); if (i == j) v += sn2; }
+      ky[i * kLD + j] = v;
+    }
   }
   __syncthreads();
   // ---- Cholesky with retry ----
@@ -165,15 +189,19 @@ __global__ void __launch_bounds__(256) k_nll_grad_small(const double* __restrict
     v = warp_sum(v);
     if (lane == 0) s_part[warp * nq + slot] = v;
   };
-  for (int k = 0; k < dk; ++k) {
-    double s = 0.0;
+  auto cat_sums = [&](int k0, int kt) {
+    for (int k = 0; k < kt; ++k) {
+      double s = 0.0;
 #pragma unroll
-    for (int u = 0; u < 16; ++u) {
-      const int e = tid + 256 * u, i = e >> 6, j = e & 63;
-      s += (zt[k * kLD + i] != zt[k * kLD + j]) ? ge[u] : 0.0;
+      for (int u = 0; u < 16; ++u) {
+        const int e = tid + 256 * u, i = e >> 6, j = e & 63;
+        s += (zt[k * kLD + i] != zt[k * kLD + j]) ? ge[u] : 0.0;
+      }
+      warp_store(s, k0 + k);
     }
-    warp_store(s, k);
-  }
+  };
+  if (WIDE) for_cat_tiles(Z, N, 0, 64, nullptr, 0, 0, 0, dk, zt, kLD, nullptr, 0, cat_sums);
+  else cat_sums(0, dk);
   for (int d = 0; d < dc; ++d) {
     double s = 0.0;
 #pragma unroll
@@ -187,24 +215,28 @@ __global__ void __launch_bounds__(256) k_nll_grad_small(const double* __restrict
   warp_store(sum_tr, dk + dc);
   warp_store(sum_gk, dk + dc + 1);
   __syncthreads();
-  if (tid < nq) {
+  auto slot_sum = [&](int q) {
     double s = 0.0;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) s += s_part[w * nq + tid];
-    out[4 + tid] = s;
-  }
+    for (int w = 0; w < 8; ++w) s += s_part[w * nq + q];
+    out[4 + q] = s;
+  };
+  if (WIDE) for (int q = tid; q < nq; q += 256) slot_sum(q);   // nq > 256 only here
+  else if (tid < nq) slot_sum(tid);
 }
 
 size_t nll_small_smem_bytes(int dc, int dk) {
   const int nq = dc + dk + 2;
-  return sizeof(double) * (4 * 64 * kLD + 32 * 34 + (size_t)dc * kLD + 6 * 64 + 8 * nq) + sizeof(int32_t) * (size_t)dk * kLD;
+  const int zk = dk > kMaxDk ? kCatTile : dk;
+  return sizeof(double) * (4 * 64 * kLD + 32 * 34 + (size_t)dc * kLD + 6 * 64 + 8 * nq) + sizeof(int32_t) * (size_t)zk * kLD;
 }
 
 int launch_nll_grad_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int n_valid,
                           const KernelParams& kp, double sn2, double jitter0, int max_iters, double* out) {
   const size_t sm = nll_small_smem_bytes(kp.dc, kp.dk);
-  VZ_TRY(raise_dyn_smem((const void*)k_nll_grad_small, sm));
-  k_nll_grad_small<<<1, 256, sm, h->stream>>>(X, Z, y, N, n_valid, kp, sn2, jitter0, max_iters, out);
+  const auto kfn = kp.dk > kMaxDk ? k_nll_grad_small<true> : k_nll_grad_small<false>;
+  VZ_TRY(raise_dyn_smem((const void*)kfn, sm));
+  kfn<<<1, 256, sm, h->stream>>>(X, Z, y, N, n_valid, kp, sn2, jitter0, max_iters, out);
   VZ_CHECK_LAUNCH();
   h->launches++;
   return 0;

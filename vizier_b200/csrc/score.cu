@@ -861,7 +861,8 @@ int launch_score(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M, con
                  double* score, double* mu, double* sigma, double* linf, const AcqFn* fn) {
   if (M <= 0) return 0;
   auto record = [&](int route, int nsplit, int grid) { h->score_route = route; h->score_nsplit = nsplit; h->score_grid = grid; };
-  if (h->kp.use_linear) {
+  // The linear_coef kernel and models past kMaxDk categorical features are scored by the general route only.
+  if (h->kp.use_linear || h->dk > kMaxDk) {
     record(VZGP_ROUTE_GENERAL, 0, 0);
     return launch_score_general(h, Xs, Zs, M, acq, fn, score, mu, sigma, linf);
   }

@@ -33,7 +33,8 @@ __device__ __forceinline__ void stage_rows_T_i32(const int32_t* __restrict__ Z, 
 // stage_rows_T.  The difference is formed before scaling so that it is exact for
 // inputs in [0,1] (DESIGN.md, "accuracy of d2").  If WITH_LINF, also tracks
 // linf[i][j] = max_{d in mask} |a_i[d]-b_j[d]| (trust region, acquisitions.py:779-820).
-template <typename Cfg, int TTM, int TTN, bool WITH_LINF>
+// CAT = false leaves out the categorical term (models past kMaxDk add it with tile_hamming, tile by tile).
+template <typename Cfg, int TTM, int TTN, bool WITH_LINF, bool CAT = true>
 __device__ __forceinline__ void tile_d2(const double* sa, int lda, const double* sb, int ldb,
                                         const int32_t* za, int ldza, const int32_t* zb, int ldzb,
                                         const KernelParams& kp, const uint8_t* tr_mask_smem,
@@ -69,6 +70,7 @@ __device__ __forceinline__ void tile_d2(const double* sa, int lda, const double*
         if (WITH_LINF && in_tr) linf[i][j] = fmax(linf[i][j], fabs(diff));
       }
   }
+  if (!CAT) return;
   for (int k = 0; k < kp.dk; ++k) {
     const double w = kp.inv_ls2_k[k];
 #pragma unroll
@@ -79,6 +81,55 @@ __device__ __forceinline__ void tile_d2(const double* sa, int lda, const double*
         int bv = zb[k * ldzb + Cfg::col_of(tx, j)];
         d2[i][j] += (av != bv) ? w : 0.0;
       }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------
+// Models with more than kMaxDk categorical features.  Their inverse length scales are a device array
+// (kp.inv_ls2_k_wide), and the kernels stage the features kCatTile at a time, so shared memory does not grow with
+// Dk.  The Hamming term is summed tile by tile in ascending feature order, the order of tile_d2's categorical loop.
+// ---------------------------------------------------------------------------
+// s[k * lds + r] = Z[row0 + r][k0 + k] for k < kt, r < rows (Z is [nrows x dk]); rows >= nrows read -1.
+__device__ __forceinline__ void stage_cat_tile_T(const int32_t* __restrict__ Z, int nrows, int dk, int k0, int kt,
+                                                 int row0, int rows, int32_t* s, int lds) {
+  const int total = rows * kt;
+  for (int e = threadIdx.x; e < total; e += blockDim.x) {
+    const int r = e / kt, k = e - r * kt;
+    const int gr = row0 + r;
+    s[k * lds + r] = gr < nrows ? __ldg(Z + (size_t)gr * dk + k0 + k) : -1;
+  }
+}
+
+// Calls f(k0, kt) once per tile of categorical features [k0, k0 + kt), after rows [rowa, rowa + rows_a) of Za and
+// [rowb, rowb + rows_b) of Zb are staged into za / zb ([kCatTile][ld]).  Every thread of the block calls it; it
+// begins with a barrier (the previous tile's readers) and leaves the last tile staged.
+template <class F>
+__device__ __forceinline__ void for_cat_tiles(const int32_t* __restrict__ Za, int na, int rowa, int rows_a,
+                                              const int32_t* __restrict__ Zb, int nb, int rowb, int rows_b, int dk,
+                                              int32_t* za, int ldza, int32_t* zb, int ldzb, F f) {
+  for (int k0 = 0; k0 < dk; k0 += kCatTile) {
+    const int kt = dk - k0 < kCatTile ? dk - k0 : kCatTile;
+    __syncthreads();
+    stage_cat_tile_T(Za, na, dk, k0, kt, rowa, rows_a, za, ldza);
+    if (Zb) stage_cat_tile_T(Zb, nb, dk, k0, kt, rowb, rows_b, zb, ldzb);
+    __syncthreads();
+    f(k0, kt);
+  }
+}
+
+// d2[i][j] += sum_{k < kt} w[k] [a_i[k] != b_j[k]] over one staged tile, w = the tile's inverse length scales.
+template <typename Cfg, int TTM, int TTN>
+__device__ __forceinline__ void tile_hamming(const int32_t* za, int ldza, const int32_t* zb, int ldzb,
+                                             const double* __restrict__ w, int kt, int ty, int tx,
+                                             double (&d2)[TTM][TTN]) {
+  for (int k = 0; k < kt; ++k) {
+    const double wk = __ldg(w + k);
+#pragma unroll
+    for (int i = 0; i < TTM; ++i) {
+      const int av = za[k * ldza + Cfg::row_of(ty, i)];
+#pragma unroll
+      for (int j = 0; j < TTN; ++j) d2[i][j] += (av != zb[k * ldzb + Cfg::col_of(tx, j)]) ? wk : 0.0;
     }
   }
 }
