@@ -741,6 +741,25 @@ int vzgp_random_pool(vzgp_handle* h, int64_t M, int Dc, int64_t index_base, uint
 int vzgp_random_pool_cat(vzgp_handle* h, int64_t M, int Dk, const int32_t* cat_sizes,
                          int64_t index_base, uint64_t seed, int32_t* Z);
 
+/* Pareto frontiers of multi-objective studies (xla_pareto.py; every metric maximised).  Row a dominates row p when
+ * all(p <= a), and - strictly - also any(a > p); a row with a NaN coordinate neither dominates nor is dominated.  All
+ * buffers are device memory, rows of m contiguous doubles, 1 <= m <= 64, at most 2^30 rows per set; the handle needs no
+ * fitted model.  The calls are asynchronous on the handle's stream; n = 0 (or v = 0) does nothing.
+ *
+ * optimal[i] = 1 when no row of `against` dominates row i of `points` (strict: strictly), else 0; n_against = 0 makes
+ * every row optimal.  The self-frontier is points == against with strict = 1. */
+int vzgp_pareto_optimal_against(vzgp_handle* h, const double* points, int n, const double* against, int n_against,
+                                int m, int strict, uint8_t* optimal);
+/* rank[i] = the number of rows of `points` that strictly dominate row i (xla_pareto.pareto_rank). */
+int vzgp_pareto_rank(vzgp_handle* h, const double* points, int n, int m, int32_t* rank);
+/* out[i] = mean over the v rows u of `vectors` of (max_{j <= i} min_k points[j][k] / u[k])^m: the randomized
+ * cumulative hypervolume from the origin (hypervolume.py _cum_hypervolume_origin, unnormalised).  NaN propagates
+ * through the min and the running max as in NumPy.  The summation order is fixed: repeated calls are bit-identical.
+ * The partial sums live in the handle (at most 256 MiB: fewer, wider CTAs at large n); VZGP_ERR_ARG when even the
+ * widest CTAs would need more: n > 2^25 / ceil(v / 14 208) at m = 2, n > 2^25 / ceil(v / 6272) at m = 64. */
+int vzgp_cum_hypervolume_origin(vzgp_handle* h, const double* points, int n, int m, const double* vectors, int v,
+                                double* out);
+
 #ifdef __cplusplus
 }
 #endif

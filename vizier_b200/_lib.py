@@ -271,6 +271,9 @@ SIGNATURES = {
     'vzgp_random_search': (_i, [_vp, _i64, _i64, _pA, _pi32, _i, _u64, _pd, _pi32, _pd, _pi64]),
     'vzgp_random_pool': (_i, [_vp, _i64, _i, _i64, _u64, _vp]),
     'vzgp_random_pool_cat': (_i, [_vp, _i64, _i, _pi32, _i64, _u64, _vp]),
+    'vzgp_pareto_optimal_against': (_i, [_vp, _vp, _i, _vp, _i, _i, _i, _vp]),
+    'vzgp_pareto_rank': (_i, [_vp, _vp, _i, _i, _vp]),
+    'vzgp_cum_hypervolume_origin': (_i, [_vp, _vp, _i, _i, _vp, _i, _vp]),
 }
 
 _lock = threading.Lock()

@@ -637,7 +637,8 @@ int vzgp_destroy(vzgp_handle* h) {
   for (DevBuf* b : {&h->X, &h->Z, &h->L, &h->Linv, &h->alpha, &h->ypad, &h->Kws, &h->Tws, &h->Kinv, &h->XT,
                     &h->scratch, &h->small, &h->xs_dev, &h->out_dev, &h->eagle, &h->pe_tmp, &h->pe_multi_tmp,
                     &h->LinvT, &h->df_tasks[0], &h->df_tasks[1], &h->df_flags, &h->df_S, &h->scal, &h->gen,
-                    &h->i8_planes, &h->i8_scale, &h->i8_kdig, &h->sep_y, &h->wk, &h->wk_scratch, &h->cat_sizes})
+                    &h->i8_planes, &h->i8_scale, &h->i8_kdig, &h->sep_y, &h->wk, &h->wk_scratch, &h->cat_sizes,
+                    &h->pareto})
     b->release();
   eagle_step_free(h);
   if (h->pinned) cudaFreeHost(h->pinned);
@@ -1102,6 +1103,38 @@ int vzgp_random_pool_cat(vzgp_handle* h, int64_t M, int Dk, const int32_t* cat_s
     sizes[k] = cat_sizes[k];
   }
   return launch_random_fill_cat(h, Z, M, Dk, sizes, index_base, seed, 8u);
+}
+
+int vzgp_pareto_optimal_against(vzgp_handle* h, const double* points, int n, const double* against, int n_against,
+                                int m, int strict, uint8_t* optimal) {
+  VZ_ARG(h, "handle");
+  VZ_ARG(n >= 0 && n_against >= 0 && n <= kMaxParetoRows && n_against <= kMaxParetoRows, "0 <= n, n_against <= 2^30");
+  VZ_ARG(m >= 1 && m <= kMaxParetoMetrics, "1 <= m <= 64");
+  if (n == 0) return 0;
+  VZ_ARG(points && optimal && (n_against == 0 || against), "points / against / optimal");
+  Guard g(h->device);
+  return launch_pareto_dominance(h, points, n, against, n_against, m, strict ? 1 : 0, optimal, nullptr);
+}
+
+int vzgp_pareto_rank(vzgp_handle* h, const double* points, int n, int m, int32_t* rank) {
+  VZ_ARG(h, "handle");
+  VZ_ARG(n >= 0 && n <= kMaxParetoRows, "0 <= n <= 2^30");
+  VZ_ARG(m >= 1 && m <= kMaxParetoMetrics, "1 <= m <= 64");
+  if (n == 0) return 0;
+  VZ_ARG(points && rank, "points / rank");
+  Guard g(h->device);
+  return launch_pareto_dominance(h, points, n, points, n, m, 1, nullptr, rank);
+}
+
+int vzgp_cum_hypervolume_origin(vzgp_handle* h, const double* points, int n, int m, const double* vectors, int v,
+                                double* out) {
+  VZ_ARG(h, "handle");
+  VZ_ARG(n >= 0 && v >= 0 && n <= kMaxParetoRows && v <= kMaxParetoRows, "0 <= n, v <= 2^30");
+  VZ_ARG(m >= 1 && m <= kMaxParetoMetrics, "1 <= m <= 64");
+  if (n == 0 || v == 0) return 0;
+  VZ_ARG(points && vectors && out, "points / vectors / out");
+  Guard g(h->device);
+  return launch_cum_hypervolume(h, points, n, m, vectors, v, out);
 }
 
 int vzgp_random_search(vzgp_handle* h, int64_t M, int64_t index_base, const vzgp_acq* acq,

@@ -220,4 +220,7 @@ struct vzgp_handle {
   // change of the fitted model bumps model_gen, and samples with mes_gen != model_gen are stale.
   vzgp::DevBuf mes, mes_tmp;
   int64_t model_gen = 0, mes_gen = -1;
+
+  // Cumulative hypervolume (pareto.cu): per-CTA partial sums [CTAs][n] of the last call.
+  vzgp::DevBuf pareto;
 };

@@ -254,6 +254,15 @@ int launch_eagle_seed_priors(vzgp_handle* h, const EagleDev& e, const double* pr
 // sizes: host [dk]; dk > kMaxDk copies them to h->cat_sizes.
 int launch_random_fill_cat(vzgp_handle* h, int32_t* Z, int64_t M, int dk, const int* sizes, int64_t index_base,
                            uint64_t seed, uint32_t stream);
+// Pareto dominance and the cumulative hypervolume from the origin (pareto.cu), 1 <= m <= kMaxParetoMetrics.
+// rank != nullptr: rank[i] = the number of rows of `against` that strictly dominate row i; otherwise optimal[i] = 1 when
+// no row of `against` dominates row i (strictly or not).
+constexpr int kMaxParetoMetrics = 64;
+// Row counts (n, n_against, v) stay below 2^30, so that row indices plus a CTA's or a slab's extent fit an int.
+constexpr int kMaxParetoRows = 1 << 30;
+int launch_pareto_dominance(vzgp_handle* h, const double* pts, int n, const double* against, int n_against, int m,
+                            int strict, uint8_t* optimal, int* rank);
+int launch_cum_hypervolume(vzgp_handle* h, const double* pts, int n, int m, const double* vec, int v, double* out);
 int launch_gather_rows_i32(vzgp_handle* h, const int32_t* Z, int dk, const long long* idx, int count, int64_t M,
                            int32_t* out);
 int eagle_prepare(const EagleDev& e);
