@@ -202,6 +202,7 @@ def _ptxas(src, tmp):
     ('eagle.cu', '_ZN4vzgp20k_eagle_suggest_wideENS_8EagleDevE'),
     ('eagle_grid.cu', '_ZN4vzgp12k_eagle_gridILb0EEEvNS_8GridArgsE'),
     ('eagle_grid.cu', '_ZN4vzgp12k_eagle_gridILb1EEEvNS_8GridArgsE'),
+    ('eagle_grid.cu', '_ZN4vzgp24k_eagle_grid_pe_ensembleENS_11GridEnsArgsE'),
 ])
 def test_suggest_kernels_have_no_spills_and_no_stack_frame(tmp_path, src, name):
   log = _ptxas(src, tmp_path)

@@ -203,6 +203,24 @@ def _fused_oracle(c: Fused):
   return (wc, wz, wr), rep, thr, best
 
 
+def test_pe_pair_on_one_handle_takes_the_graph_form():
+  """GP-UCB-PE with one handle as both models: the cooperative kernel keeps a workspace per member handle, so a shared
+  handle must take the replayed graph."""
+  c = next(f for f in FUSED if f.name == 'cooperative-pe1')
+  _lib, gp = _mods()
+  x, y, _, mask, _, prior_c, _ = _fused_problem(c)
+  _, pg = _params(c.d, c.dk)
+  dev = gp.DeviceGP(0)
+  try:
+    dev.fit(x[:c.n], y, pg)
+    acq = gp.UcbPeAcquisition(mode=1, threshold=float(np.max(y)), trust_radius=c.radius, tr_dim_mask=mask, tr_rows=c.n)
+    _, _, br = dev.eagle_run(_config(CHEAP_TRIM, c.pool, c.batch, c.steps), acq, COUNT, 5, other=dev, prior=prior_c)
+    assert dev.get_int('eagle_route') == GRAPH
+    assert np.all(np.isfinite(br))
+  finally:
+    dev.close()
+
+
 @pytest.mark.parametrize('c', FUSED, ids=lambda c: c.name)
 def test_fused_forms_with_trust_region_and_trimming(c):
   _lib, gp = _mods()

@@ -3,8 +3,9 @@
 1. `vzgp_score_pe` against `vzgp_score_pe_ensemble` for E = 1..5 on the same 100 000-candidate pool at N = 1000
    trials, D = 20 (PE mode, strict trust radius 0.3): CUDA events around whole calls, the variants run alternately,
    median of `--reps`.
-2. The default Eagle loop (75 000 evaluations, batches of 25) at E = 3 and N = 1000 in the cooperative form and in
-   the replayed-graph form (VZGP_EAGLE_GRID=0 is read once per process, so that form runs in a child process).
+2. The default Eagle loop (75 000 evaluations, batches of 25) at N = 1000 in the cooperative form at E = 1 (a pair of
+   models) and E = 3, and at E = 3 in the replayed-graph form (VZGP_EAGLE_GRID=0 is read once per process, so that
+   form runs in a child process).
 3. One `suggest(1)` of VizierGPUCBPEBandit at 1000 completed trials with ensemble_size 1 and 3 (ARD + Eagle).
 
 Prints one JSON line with the card name and power limit read in the same run.  Usage:
@@ -83,13 +84,13 @@ def _score(reps):
           for k, v in times.items()}
 
 
-def _eagle(reps):
-  """Median wall time of the default Eagle loop at E = 3 in whichever form this process takes."""
+def _eagle(reps, e=3):
+  """Median wall time of the default Eagle loop at E members in whichever form this process takes."""
   from vizier_b200 import optimizers as vb
   from vizier_b200 import gp
   from vizier_b200.designers import gp_ucb_pe
   rng = np.random.default_rng(3)
-  x, a, b = _ensembles(3, rng)
+  x, a, b = _ensembles(e, rng)
   opt = vb.VectorizedOptimizer(vb.VectorizedEagleStrategyFactory(eagle_config=gp_ucb_pe.default_eagle_config), D, 0,
                                25, 75_000, ())
   cfg = opt._eagle_config()   # pylint: disable=protected-access
@@ -136,6 +137,7 @@ def main():
     return
   res = {'card': _card(), 'setup': f'N={N}, D={D}, {M} candidates, PE mode, strict trust radius 0.3'}
   res['score'] = _score(args.reps)
+  res['eagle_e1_cooperative'] = _eagle(args.reps, 1)
   res['eagle_e3_cooperative'] = _eagle(args.reps)
   env = dict(os.environ, VZGP_EAGLE_GRID='0')
   proc = subprocess.run([sys.executable, os.path.abspath(__file__), '--eagle-only', '--reps', str(args.reps)], env=env,

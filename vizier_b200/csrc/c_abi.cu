@@ -1341,15 +1341,13 @@ static int eagle_run_impl(const Model& m, const vzgp_eagle_config* cfg, const do
     VZ_TRY(launch_eagle_persistent64(h, hB, e, m.acq, m.pe, steps, m.fn()));
     h->eagle_route = VZGP_EAGLE_PERSISTENT;
     done = true;
-  } else if (m.single_form() && eagle_grid_eligible(h, hB, e)) {
-    // mid-size study: one cooperative launch, phases separated by grid barriers.  If the cooperative
-    // launch is refused (nothing has run then) the launch-per-phase loop below takes over.
-    done = launch_eagle_grid(h, hB, e, m.acq, m.pe, steps, m.fn()) == 0;
-    if (done) h->eagle_route = VZGP_EAGLE_COOPERATIVE;
-    else cudaGetLastError();
-  } else if (m.kind == Model::kPe && eagle_grid_pe_ensemble_eligible(m.hs, m.hBs, m.E, e)) {
-    // the same cooperative loop over the 2E member models (2 <= E; E = 1 took the single-model forms above)
-    done = launch_eagle_grid_pe_ensemble(m.hs, m.hBs, m.E, e, m.pe, steps) == 0;
+  } else if (m.kind == Model::kSingle ? eagle_grid_eligible(h, e)
+                                      : m.kind == Model::kPe && eagle_grid_pe_ensemble_eligible(m.hs, m.hBs, m.E, e)) {
+    // mid-size study: one cooperative launch, phases separated by grid barriers; GP-UCB-PE scores its E >= 1
+    // members per model.  If the cooperative launch is refused (nothing has run then) the launch-per-phase loop
+    // below takes over.
+    done = (m.kind == Model::kSingle ? launch_eagle_grid(h, e, m.acq, steps, m.fn())
+                                     : launch_eagle_grid_pe_ensemble(m.hs, m.hBs, m.E, e, m.pe, steps)) == 0;
     if (done) h->eagle_route = VZGP_EAGLE_COOPERATIVE;
     else cudaGetLastError();
   }

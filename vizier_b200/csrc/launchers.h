@@ -238,10 +238,9 @@ bool eagle_persistent_eligible(const vzgp_handle* h, const vzgp_handle* hB, cons
 int launch_eagle_persistent64(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const vzgp_acq* acq,
                               const vzgp_pe_params* pe, int steps, const AcqFn* fn = nullptr);
 // Multi-CTA persistent Eagle loop (eagle_grid.cu): cooperative launch, batch <= 512 candidates.
-bool eagle_grid_eligible(const vzgp_handle* h, const vzgp_handle* hB, const EagleDev& e);
-int launch_eagle_grid(vzgp_handle* h, vzgp_handle* hB, const EagleDev& e, const vzgp_acq* acq,
-                      const vzgp_pe_params* pe, int steps, const AcqFn* fn = nullptr);
-// Its GP-UCB-PE ensemble form: the E members of A (hAs) and of B (hBs), E <= kMaxGridPeEnsemble (eagle_grid.cu).
+bool eagle_grid_eligible(const vzgp_handle* h, const EagleDev& e);
+int launch_eagle_grid(vzgp_handle* h, const EagleDev& e, const vzgp_acq* acq, int steps, const AcqFn* fn = nullptr);
+// Its GP-UCB-PE form: the E members of A (hAs) and of B (hBs), 1 <= E <= kMaxGridPeEnsemble (eagle_grid.cu).
 bool eagle_grid_pe_ensemble_eligible(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const EagleDev& e);
 int launch_eagle_grid_pe_ensemble(vzgp_handle* const* hAs, vzgp_handle* const* hBs, int E, const EagleDev& e,
                                   const vzgp_pe_params* pe, int steps);
