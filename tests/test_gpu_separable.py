@@ -225,6 +225,27 @@ def test_separable_joint_posterior_matches_oracle(add_noise):
   np.testing.assert_allclose(cov.cpu().numpy(), so.to_metric_major(wc, 9, 3), atol=1e-10, rtol=0)
 
 
+@pytest.mark.parametrize('nq', [63, 65, 129])
+def test_separable_joint_posterior_across_query_tiles(nq):
+  """The per-eigen-task posteriors cross the 64-row query tiles of k_cov_update and k_gemm_nt_tri before they are
+  recombined into the [M n, M n] covariance."""
+  from vizier_b200 import gp
+  from vizier_b200 import task_kernels as tk
+  rng, x, y, z, ls2, lk = _setup(150, 4, 2, 2, nq)
+  pg = gp.GPHyperParams(0.9, ls2, 5e-3, lk, multitask_type=tk.NORMAL, task_params=np.array([0.8, 0.3, 1.1]))
+  po = go.GPParams(0.9, ls2, 5e-3, lk)
+  sep = gp.SeparableGP(0, 2)
+  sep.fit(x, y, pg, z=z)
+  xs = rng.uniform(size=(nq, 4))
+  zs = rng.integers(0, 3, size=(nq, 2)).astype(np.int32)
+  xs[:3], zs[:3] = x[:3], z[:3]
+  xs[-1], zs[-1] = xs[nq // 2], zs[nq // 2]
+  mean, cov = sep.posterior(xs, zs)
+  wm, wc = so.posterior(po, pg.task_covariance(), x, y, xs, z, zs)
+  np.testing.assert_allclose(mean.cpu().numpy(), wm.T, atol=1e-10, rtol=0)
+  np.testing.assert_allclose(cov.cpu().numpy(), so.to_metric_major(wc, nq, 2), atol=1e-10, rtol=0)
+
+
 @pytest.mark.parametrize('multitask_type', ['SEPARABLE_NORMAL_TASK_KERNEL_PRIOR', 'SEPARABLE_LKJ_TASK_KERNEL_PRIOR',
                                             'SEPARABLE_DIAG_TASK_KERNEL_PRIOR'])
 def test_multi_metrics_separable_designer(multitask_type):

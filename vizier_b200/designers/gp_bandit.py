@@ -171,7 +171,11 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     self._scoring_function_factory = scoring_function_factory if self._n_metrics == 1 else None
     self._ucb_coefficient = ucb_coefficient
     self._metadata_ns = 'oss_gp_bandit'
+    # one warper per metric, each fitted on its own metric's labels: metric 0 keeps the configured warper, the others
+    # warp with fresh copies of it (the warpers are stateful, and a user warper may be given)
     self._output_warper = output_warper or output_warpers.create_default_warper()
+    self._output_warpers = [self._output_warper] + [copy.deepcopy(self._output_warper)
+                                                    for _ in range(self._n_metrics - 1)]
     self._rng = np.random.default_rng(_seed_from(rng))
     self._converter = converters.TrialToModelInputConverter.from_problem(problem)
     self._lbfgsb = isinstance(acquisition_optimizer_factory, vb.LBFGSBOptimizerFactory)
@@ -301,7 +305,7 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     return out
 
   def _warp_labels(self, labels: np.ndarray) -> np.ndarray:
-    return np.concatenate([self._output_warper.warp(labels[:, i:i + 1]) for i in range(labels.shape[1])], axis=-1)
+    return np.concatenate([w.warp(labels[:, i:i + 1]) for i, w in enumerate(self._output_warpers)], axis=-1)
 
   @profiler.record_runtime
   def _trials_to_data(self, trials):
@@ -474,10 +478,10 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     chol, _, _ = self._ard_dev.cholesky_retry(cov, jitter=1e-10, max_iters=8)
     mean, chol = mean.cpu().numpy(), chol.cpu().numpy()
     out = np.empty((num_samples, mean.shape[1], self._n_metrics))
-    for m in range(self._n_metrics):
+    for m, warper in enumerate(self._output_warpers):
       z = g.standard_normal((num_samples, mean.shape[1]))
       warped = mean[m][None, :] + z @ chol.T
-      out[:, :, m] = self._output_warper.unwarp(warped.reshape(-1, 1)).reshape(num_samples, -1)
+      out[:, :, m] = warper.unwarp(warped.reshape(-1, 1)).reshape(num_samples, -1)
     return out
 
   def _sample_stack_multi(self, stack, xs, zq, g, num_samples: int) -> np.ndarray:
@@ -485,9 +489,9 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     150-152) with the stddev shared by the metrics.  Returns unwarped samples [num_samples, num_trials, num_metrics]."""
     mean, sd = stack.predict(xs, zq)                            # [n, M], [n]
     res = np.empty((num_samples, mean.shape[0], self._n_metrics))
-    for m in range(self._n_metrics):
+    for m, warper in enumerate(self._output_warpers):
       warped = mean[:, m][None, :] + g.standard_normal((num_samples, mean.shape[0])) * sd[None, :]
-      res[:, :, m] = self._output_warper.unwarp(warped.reshape(-1, 1)).reshape(num_samples, -1)
+      res[:, :, m] = warper.unwarp(warped.reshape(-1, 1)).reshape(num_samples, -1)
     return res
 
   @profiler.record_runtime
@@ -506,6 +510,6 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
     z = g.standard_normal((num_samples, m * n))
     warped = (mean.reshape(-1)[None, :] + z @ chol.T).reshape(num_samples, m, n)
     out = np.empty((num_samples, n, m))
-    for t in range(m):
-      out[:, :, t] = self._output_warper.unwarp(warped[:, t, :].reshape(-1, 1)).reshape(num_samples, n)
+    for t, warper in enumerate(self._output_warpers):
+      out[:, :, t] = warper.unwarp(warped[:, t, :].reshape(-1, 1)).reshape(num_samples, n)
     return out
