@@ -79,6 +79,16 @@ def spd_with_lambda_min(n, lam_min, seed=0):
   return 0.5 * (a + a.T)
 
 
+def require_device_bytes(need: int) -> None:
+  """Skips the calling test, naming the bytes, unless `need` bytes of device memory are free on cuda:0 (the large
+  studies share the GPU with whatever else runs there)."""
+  import pytest
+  import torch
+  free, total = torch.cuda.mem_get_info(0)
+  if need > free:
+    pytest.skip(f'needs {need / 2**30:.2f} GiB of device memory, {free / 2**30:.2f} GiB of {total / 2**30:.2f} free')
+
+
 # lambda_min of vzgp_cholesky_retry fixtures -> retries: each sits a factor >= 3 inside its ladder interval
 # (shift k-1 + lambda_min < 0 < shift k + lambda_min, with margins of at least 3x on both sides)
 LADDER_LAMBDA = {0: 1e-2, 1: -3e-5, 2: -3e-4, 3: -3e-3, 4: -3e-2, 5: -0.3, 6: -3.0}

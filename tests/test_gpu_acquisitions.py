@@ -118,10 +118,12 @@ def test_single_model_routes(route, n, d, dk, tr):
   dev.close()
 
 
-@pytest.mark.parametrize('tr', [True, False], ids=['tr', 'no-tr'])
-def test_general_route_linear_model(tr):
+# N = 4097: two kGeneralChunk (4096) candidate chunks, each K* and W of 4096 x np = 4160
+@pytest.mark.parametrize('tr,n,m', [(True, 90, 777), (False, 90, 777), (True, 4097, 4096 + 69)],
+                         ids=['tr', 'no-tr', 'tr-N4097'])
+def test_general_route_linear_model(tr, n, m):
   _lib, acq, gp = _mods()
-  n, d = 90, 4
+  d = 4
   x, y, _ = _problem(n, d, 8)
   ls2 = 0.5 * (1 + np.arange(d) / d)
   po = go.GPParams(0.8, ls2, 2e-3, None, go.LinearParams(0.1, 0.9, 0.3, -0.4))
@@ -129,7 +131,7 @@ def test_general_route_linear_model(tr):
   pred = go.precompute_predictive(po, x, y)
   dev = gp.DeviceGP(0)
   dev.fit(x, y, pg)
-  xs = np.random.default_rng(9).uniform(size=(777, d))
+  xs = np.random.default_rng(9).uniform(size=(m, d))
   mu, sd = go.predict(pred, xs)
   dist = go.min_linf_distance(xs, x, np.ones(d, bool), pred.row_valid)
   for kind, fn in _acq_fns(y).items():

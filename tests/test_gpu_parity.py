@@ -288,13 +288,15 @@ def test_random_search_matches_oracle(dev):
   np.testing.assert_allclose(bs, ws, atol=TOL)
 
 
-# The last two rows are BASELINE C3's shape (P = B = 1000 fireflies, N = 1000 trials, D = 20) and a
+# The fourth and fifth rows are BASELINE C3's shape (P = B = 1000 fireflies, N = 1000 trials, D = 20) and a
 # batch-600 case: batches above 512 take the replayed CUDA-graph form of the loop (c_abi.cu,
-# eagle_run_impl over the Model descriptor) with k_eagle_suggest / k_eagle_update at 1000 flies and the large-pool k_score.  The form each row
+# eagle_run_impl over the Model descriptor) with k_eagle_suggest / k_eagle_update at 1000 flies and the large-pool k_score.
+# The last row scores inside the cooperative kernel against np = 3008 trials.  The form each row
 # takes is asserted.  At every size here the trust radius is above 0.5 (the region is off) and no fly is visited often
 # enough to be trimmed: tests/test_gpu_eagle_steps.py covers the active region, trimming, ties and non-finite rewards.
 @pytest.mark.parametrize('n,d,pool,batch,steps', [(30, 4, 25, 25, 6), (60, 5, 20, 5, 14), (130, 3, 50, 25, 7),
-                                                  (1000, 20, 1000, 1000, 6), (700, 12, 1200, 600, 7)])
+                                                  (1000, 20, 1000, 1000, 6), (700, 12, 1200, 600, 7),
+                                                  (3000, 6, 50, 25, 4)])
 def test_eagle_run_matches_oracle(dev, n, d, pool, batch, steps):
   x, y, _ = _problem(n, d, 13)
   po, pg = _params(d)
@@ -792,20 +794,35 @@ def test_nll_grad_d50_multiblock(dev):
   assert abs(fd - g0 @ direction) < 1e-4 * max(1.0, abs(fd))
 
 
-def test_nll_grad_c4_full_size(dev):
-  """BASELINE C4 (N=2000, D=50, 52 hyper-parameters): loss and the whole gradient against the oracle."""
-  n, d = 2000, 50
+def _check_c4_nll(dev, n, d, dk=0, nv=None):
   rng = np.random.default_rng(72)
   x = rng.uniform(size=(n, d)); y = rng.normal(size=n)
+  z = rng.integers(0, 4, size=(n, dk)).astype(np.int32) if dk else None
   ls2 = np.exp(rng.uniform(np.log(0.3), np.log(5.0), size=d))
-  po = go.GPParams(0.9, ls2, 3e-2); pg = _gp().GPHyperParams(0.9, ls2, 3e-2)
-  want_l, want_g = go.loss_and_grad(po.to_vector(), x, y)
+  lk = np.linspace(0.6, 1.4, dk) if dk else None
+  po = go.GPParams(0.9, ls2, 3e-2, lk); pg = _gp().GPHyperParams(0.9, ls2, 3e-2, lk)
+  nv = n if nv is None else nv
+  want_l, want_g = go.loss_and_grad(po.to_vector(), x, y, z, np.arange(n) < nv)
   xt = torch.from_numpy(x).cuda(); yt = torch.from_numpy(y).cuda()
+  zt = torch.from_numpy(z).cuda() if dk else None
   for _ in range(2):   # eager capture call, then the replayed graph
-    loss, grad, retries = dev.loss_and_grad(xt, yt, pg)
+    loss, grad, retries = dev.loss_and_grad(xt, yt, pg, z=zt, n_valid=nv)
+    assert (dev.get_int('nll_route'), dev.get_int('factor_route')) == (1, 1)   # graph, dataflow
     assert retries == 0
     assert abs(loss - want_l) < 1e-9 * abs(want_l)
     np.testing.assert_allclose(grad, want_g, atol=1e-8 * np.max(np.abs(want_g)), rtol=0)
+
+
+def test_nll_grad_c4_full_size(dev):
+  """BASELINE C4 (N=2000, D=50, 52 hyper-parameters): loss and the whole gradient against the oracle."""
+  _check_c4_nll(dev, 2000, 50)
+
+
+# Past C4: nb = 65 and 94 64-blocks, so k_nll_grad_tiles reduces 2145 and 4465 tile partials (nb (nb + 1) / 2); the
+# host oracle holds ~10 N^2 doubles, which is why these stop at N = 6000.
+@pytest.mark.parametrize('n,d,dk,nv', [(4097, 20, 2, 4000), (6000, 8, 0, 6000)])
+def test_nll_grad_past_c4(dev, n, d, dk, nv):
+  _check_c4_nll(dev, n, d, dk, nv)
 
 
 def _two_models(dev, n, d, n_pending, seed, high_noise=False):

@@ -112,6 +112,7 @@ CASES = [
     (1000, 65, 60, 20, 0, 'metrics2', False),
     (65, 1000, 950, 20, 40, 'ensemble', True),
     (129, 5, 5, 20, 3, 'ensemble', False),
+    (65, 4097, 4000, 8, 2, 'gp', True),       # k_cov_update and the mean gemv against np = 4160
 ]
 
 
