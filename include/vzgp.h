@@ -294,6 +294,35 @@ int vzgp_nll_grad_batch(vzgp_handle* const* hs, int R, const double* X, const in
                         int Dc, int Dk, int n_valid, int n_metrics, const vzgp_params* ps, const uint8_t* active,
                         double* loss_out, double* grad_out, int* status_out);
 
+/* Adam configuration of vzgp_ard_adam_small (optax.adam: scale_by_adam, then scale by -learning_rate). */
+typedef struct vzgp_adam {
+  double learning_rate;
+  double b1;
+  double b2;
+  double eps;
+  double eps_root;
+  int epochs;
+} vzgp_adam;
+
+/* 1 when vzgp_ard_adam_small takes a study of N trials with Dc continuous and Dk categorical features (N <= 64 and the
+ * model's shared memory fits one CTA), else 0. */
+int vzgp_ard_adam_small_supported(int N, int Dc, int Dk);
+
+/* ARD with Adam, the reference's OptaxTrain (optax_wrappers.py:36-150), for a single-metric study without linear_coef:
+ * R restarts x adam->epochs epochs in ONE launch, one CTA per restart (csrc/ard_adam.cu).  Each restart starts from
+ * theta0[r] mapped through the inverse of SoftClip(lower[p], upper[p], hinge 1e-2) and, every epoch, evaluates the loss
+ * of vzgp_nll_grad at SoftClip(u) (with the regularisers) and its gradient in u, then takes one Adam step on u.
+ * X [N x Dc], Z [N x Dk], y [N]: device.  theta0 [R x P], lower, upper [P] (finite, lower < upper): host, in the
+ * vzgp_nll_grad gradient order (P = Dk + Dc + 2).  Outputs, host: theta_out [R x P] the parameters after the last
+ * update, loss_out [R] the loss of the last evaluation, status_out [R] the Cholesky retries of the last evaluation,
+ * loss_trace [epochs x R] (optional) every evaluation's loss.  A restart whose retries are exhausted, or whose loss or
+ * gradient is not finite, stops: NaN loss from that epoch on, theta_out the parameters of that evaluation.
+ * VZGP_ERR_ARG for sizes vzgp_ard_adam_small_supported refuses and for invalid arguments.  Synchronous. */
+int vzgp_ard_adam_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int Dc, int Dk,
+                        int n_valid, int R, const double* theta0, const double* lower, const double* upper,
+                        const vzgp_adam* adam, double* theta_out, double* loss_out, int* status_out,
+                        double* loss_trace);
+
 /* Hyper-volume scalarised UCB, the acquisition VizierGPBandit uses for multi-objective problems
  * (gp_bandit.py:214-242; acquisitions.py:571-625; scalarization.py:85-111):
  *   u_m = mu_m + ucb_coefficient * sigma            (sigma is shared by the metrics of the independent GP)

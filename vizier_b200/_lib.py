@@ -169,6 +169,17 @@ class EagleConfig(C.Structure):
       self.prob_same_category_without_perturbation = 0.98
 
 
+class Adam(C.Structure):
+  _fields_ = [
+      ('learning_rate', C.c_double),
+      ('b1', C.c_double),
+      ('b2', C.c_double),
+      ('eps', C.c_double),
+      ('eps_root', C.c_double),
+      ('epochs', C.c_int),
+  ]
+
+
 _vp = C.c_void_p
 _i = C.c_int
 _i64 = C.c_int64
@@ -206,6 +217,9 @@ SIGNATURES = {
     'vzgp_fit_multi': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _pP]),
     'vzgp_nll_grad_multi': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _pP, _pd, _pd]),
     'vzgp_nll_grad_batch': (_i, [C.POINTER(_vp), _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, C.POINTER(Params), C.POINTER(C.c_uint8), _pd, _pd, C.POINTER(_i)]),
+    'vzgp_ard_adam_small_supported': (_i, [_i, _i, _i]),
+    'vzgp_ard_adam_small': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _pd, _pd, _pd, C.POINTER(Adam), _pd, _pd,
+                                 C.POINTER(_i), _pd]),
     'vzgp_score_multi': (_i, [_vp, _vp, _vp, _i, C.POINTER(Scalarization), _vp, _vp, _vp]),
     'vzgp_eagle_run_multi': (_i, [_vp, _pE, C.POINTER(Scalarization), _vp, _vp, _i, _pi32, _i, _u64, _pd, _pi32, _pd]),
     'vzgp_fit_separable': (_i, [C.POINTER(_vp), _i, _vp, _vp, _vp, _i, _i, _i, _i, _pP, _pd]),

@@ -1,4 +1,4 @@
-"""ARD: fits the GP hyper-parameters by multi-restart L-BFGS-B on the device loss/gradient.
+"""ARD: fits the GP hyper-parameters by multi-restart L-BFGS-B (the default) or Adam on the device loss/gradient.
 
 Mirrors `gp_models._train_gp` (vizier/_src/algorithms/designers/gp/gp_models.py:169-223) with the
 default optimiser `JaxoptScipyLbfgsB(LbfgsBOptions(maxiter=50))`
@@ -11,12 +11,23 @@ default optimiser `JaxoptScipyLbfgsB(LbfgsBOptions(maxiter=50))`
 loss(theta) and its gradient come from `vzgp_nll_grad` (CUDA); SciPy only drives.
 The draws use NumPy's Generator rather than JAX threefry: seeded trajectories are reproducible
 but not bit-identical to a JAX run (SURVEY 8c).
+
+`OptaxTrain(adam(lr), epochs=T)` is the reference's second ARD optimiser (optax_wrappers.py:36-150): Adam on the
+unconstrained u of each parameter's SoftClip(low, high, hinge_softness=1e-2) bijector (unbounded parameters: the
+identity), all restarts for a fixed number of epochs; each epoch evaluates once, then updates; the `best_n` restarts
+with the lowest loss of the LAST evaluation are kept (their parameters after the last update).  Single-metric studies
+of N <= 64 trials without `linear_coef` run every epoch of every restart in ONE kernel launch (`vzgp_ard_adam_small`,
+csrc/ard_adam.cu: route 'fused'); every other study runs one device evaluation per epoch on the loss callables below
+with the SoftClip and Adam arithmetic in NumPy (route 'host').  `OptaxTrain.last_metrics` holds the loss trace
+[epochs, R], the final losses and the route of its last run.  Separable multi-task types raise NotImplementedError
+with it (their task parameters have non-box bijectors in the reference).
 """
 
 from __future__ import annotations
 
 import dataclasses
-from typing import List, Optional, Tuple
+import logging
+from typing import Any, List, Optional, Tuple
 
 import numpy as np
 import scipy.optimize as sopt
@@ -210,6 +221,202 @@ class ScipyLbfgsB:
     return [finals[i] for i in order], losses
 
 
+HINGE_SOFTNESS = 1e-2   # SoftClip(low, high, hinge_softness=1e-2) of every bounded parameter (tuned_gp_models.py)
+
+
+def _softplus(v):
+  """c log1p(exp(v / c)), c = HINGE_SOFTNESS, in the overflow-free form max(v, 0) + c log1p(exp(-|v| / c))."""
+  return np.maximum(v, 0.0) + HINGE_SOFTNESS * np.log1p(np.exp(-np.abs(v) / HINGE_SOFTNESS))
+
+
+def _softplus_inv(s):
+  """The inverse of `_softplus` for s > 0: s + c log(-expm1(-s / c))."""
+  return s + HINGE_SOFTNESS * np.log(-np.expm1(-s / HINGE_SOFTNESS))
+
+
+def _sigmoid(z):
+  with np.errstate(over='ignore'):
+    e = np.exp(np.minimum(z, 0.0))
+    return np.where(z >= 0.0, 1.0 / (1.0 + np.exp(-np.maximum(z, 0.0))), e / (1.0 + e))
+
+
+def soft_clip(u, lo, hi):
+  """theta = hi - sp(hi - lo - sp(u - lo)) and dtheta/du, elementwise; the identity where a bound is infinite.
+  The operations are those of csrc/ard_adam.cu, in the same order."""
+  u = np.asarray(u, np.float64)
+  box = np.isfinite(lo) & np.isfinite(hi)
+  lo_b, hi_b = np.where(box, lo, 0.0), np.where(box, hi, 1.0)
+  a = u - lo_b
+  w = (hi_b - lo_b) - _softplus(a)
+  th = hi_b - _softplus(w)
+  d = _sigmoid(w / HINGE_SOFTNESS) * _sigmoid(a / HINGE_SOFTNESS)
+  return np.where(box, th, u), np.where(box, d, 1.0)
+
+
+def soft_clip_inverse(theta, lo, hi):
+  """u with soft_clip(u) = theta; the arguments of sp^-1 are kept >= the smallest normal double, so a point on or past a
+  bound maps to a finite u (where the bijector is flat)."""
+  theta = np.asarray(theta, np.float64)
+  box = np.isfinite(lo) & np.isfinite(hi)
+  lo_b, hi_b = np.where(box, lo, 0.0), np.where(box, hi, 1.0)
+  tiny = np.finfo(np.float64).tiny
+  r = _softplus_inv(np.maximum(hi_b - theta, tiny))
+  u = lo_b + _softplus_inv(np.maximum((hi_b - lo_b) - r, tiny))
+  return np.where(box, u, theta)
+
+
+@dataclasses.dataclass(frozen=True)
+class adam:  # pylint: disable=invalid-name  # stands in for optax.adam (optax is not a dependency)
+  """optax.adam(learning_rate, b1, b2, eps, eps_root): scale_by_adam, then scale by -learning_rate."""
+
+  learning_rate: float
+  b1: float = 0.9
+  b2: float = 0.999
+  eps: float = 1e-8
+  eps_root: float = 0.0
+
+
+class _Evaluator:
+  """(indices, thetas) -> (losses, grads) over any of the loss-callable forms ScipyLbfgsB takes: a batched callable
+  (`n_restarts`: one call), a sequence of equivalent callables on distinct handles (the restarts split between them, one
+  host thread per handle, so their evaluations overlap on the GPU) or one callable (the restarts one after another).
+  Results do not depend on the number of handles."""
+
+  def __init__(self, loss_and_grad):
+    self._batch = loss_and_grad if hasattr(loss_and_grad, 'n_restarts') else None
+    fns = list(loss_and_grad) if isinstance(loss_and_grad, (list, tuple)) else [loss_and_grad]
+    self._fns = fns
+    self._pool = None
+    if self._batch is None and len(fns) > 1:
+      import concurrent.futures as cf
+      self._pool = cf.ThreadPoolExecutor(max_workers=len(fns))
+
+  def __call__(self, indices, thetas):
+    if self._batch is not None:
+      return self._batch(indices, thetas)
+    w = min(len(self._fns), len(thetas))
+    if self._pool is None or w <= 1:
+      out = [self._fns[0](t) for t in thetas]
+    else:
+      parts = [self._pool.submit(lambda j: [self._fns[j](t) for t in thetas[j::w]], j) for j in range(w)]
+      done = [p.result() for p in parts]
+      out = [done[k % w][k // w] for k in range(len(thetas))]
+    return [o[0] for o in out], [o[1] for o in out]
+
+  def close(self):
+    if self._pool is not None:
+      self._pool.shutdown()
+
+
+def adam_host_epochs(opt: adam, epochs: int, init_thetas: np.ndarray, lo, hi, evaluate):
+  """The host-stepped Adam loop: one `evaluate(indices, thetas)` per epoch over the restarts still running, SoftClip and
+  Adam in NumPy with the operations of csrc/ard_adam.cu.  A restart whose loss (or gradient) is not finite - the loss
+  callables return 1e300 for a non-finite loss - stops there: NaN losses from that epoch on and the parameters of that
+  evaluation.  Returns (theta [R, P], final losses [R], loss trace [epochs, R])."""
+  th0 = np.atleast_2d(np.asarray(init_thetas, np.float64))
+  r = th0.shape[0]
+  lo, hi = np.asarray(lo, np.float64), np.asarray(hi, np.float64)
+  u = soft_clip_inverse(th0, lo, hi)
+  mu, nu = np.zeros_like(u), np.zeros_like(u)
+  trace = np.full((epochs, r), np.nan)
+  alive = np.ones(r, bool)
+  stopped_at = np.zeros_like(u)
+  b1t = b2t = 1.0
+  for e in range(epochs):
+    idx = np.flatnonzero(alive)
+    if not idx.size:
+      break
+    th, dth = soft_clip(u[idx], lo, hi)
+    losses, grads = evaluate(list(idx), list(th))
+    good = np.zeros(idx.size, bool)
+    g = np.zeros((idx.size, u.shape[1]))
+    for k, i in enumerate(idx):
+      gk = np.asarray(grads[k], np.float64)
+      if np.isfinite(losses[k]) and losses[k] < 1e300 and np.all(np.isfinite(gk)):
+        good[k] = True
+        trace[e, i] = losses[k]
+        g[k] = gk
+      else:
+        alive[i] = False
+        stopped_at[i] = th[k]
+    b1t = b1t * opt.b1
+    b2t = b2t * opt.b2
+    j = idx[good]
+    gu = g[good] * dth[good]
+    mu[j] = (1.0 - opt.b1) * gu + opt.b1 * mu[j]
+    nu[j] = (1.0 - opt.b2) * (gu * gu) + opt.b2 * nu[j]
+    upd = (mu[j] / (1.0 - b1t)) / (np.sqrt(nu[j] / (1.0 - b2t) + opt.eps_root) + opt.eps)
+    u[j] = u[j] + (-opt.learning_rate) * upd
+  theta = np.where(alive[:, None], soft_clip(u, lo, hi)[0], stopped_at)
+  final = np.where(alive, trace[-1], np.nan)
+  return theta, final, trace
+
+
+@dataclasses.dataclass
+class OptaxTrain:
+  """The reference's `OptaxTrain(optimizer, *, epochs, verbose=0)` with `optimizer=adam(...)`; see the module
+  docstring.  Called like ScipyLbfgsB on loss callables it runs the host-stepped epochs; `fit` picks the fused kernel
+  where the study allows it."""
+
+  optimizer: Any
+  epochs: int = dataclasses.field(kw_only=True)
+  verbose: int = dataclasses.field(default=0, kw_only=True)
+  # of the last run: 'loss' [epochs, R], 'final_loss' [R], 'route' ('fused' or 'host'), 'status' [R] (fused: the
+  # Cholesky retries of each restart's last evaluation; host: None)
+  last_metrics: Optional[dict] = dataclasses.field(default=None, init=False, repr=False, compare=False)
+
+  def __post_init__(self):
+    if not isinstance(self.optimizer, adam):
+      raise NotImplementedError(f'OptaxTrain takes the ard.adam optimiser only, not {type(self.optimizer).__name__}.')
+    if int(self.epochs) < 1:
+      raise NotImplementedError('OptaxTrain needs epochs >= 1.')
+    self.epochs = int(self.epochs)
+    self.verbose = int(self.verbose)
+
+  def _finish(self, thetas, final, trace, route, status, best_n):
+    self.last_metrics = {'loss': trace, 'final_loss': final, 'route': route, 'status': status}
+    if self.verbose >= 1:
+      for e, row in enumerate(trace):
+        logging.info('Epoch %s: loss %s', e, row)
+    order = np.argsort(final, kind='stable')[:max(1, best_n)]
+    return [thetas[i] for i in order], final
+
+  def __call__(self, init_thetas: np.ndarray, loss_and_grad, bounds, best_n: int = 1):
+    """Host-stepped epochs on `loss_and_grad` (any form ScipyLbfgsB takes); returns (best_n thetas, final losses)."""
+    lo = np.array([b[0] for b in bounds], np.float64)
+    hi = np.array([b[1] for b in bounds], np.float64)
+    evaluate = _Evaluator(loss_and_grad)
+    try:
+      thetas, final, trace = adam_host_epochs(self.optimizer, self.epochs, init_thetas, lo, hi, evaluate)
+    finally:
+      evaluate.close()
+    return self._finish(thetas, final, trace, 'host', None, best_n)
+
+  def fit(self, dev: gp.DeviceGP, xt, yt, zt, init_thetas: np.ndarray, lo, hi, *, best_n: int = 1,
+          n_valid: Optional[int] = None, linear_coef: Optional[float] = None):
+    """ARD of one model on device tensors: the fused kernel for a single-metric study of N <= 64 trials without
+    linear_coef (when its shared memory fits one CTA), else host-stepped epochs on the batched loss callable (N > 64,
+    2-16 restarts, no linear_coef) or on up to MAX_ARD_WORKERS handles evaluating the restarts concurrently.  Returns
+    (best_n thetas, final losses)."""
+    from vizier_b200 import _lib
+    inits = np.atleast_2d(np.asarray(init_thetas, np.float64))
+    n, dc = xt.shape
+    dk = 0 if zt is None else zt.shape[1]
+    single = yt.ndim == 1 or yt.shape[1] == 1
+    opt = self.optimizer
+    if single and not linear_coef and _lib.load().vzgp_ard_adam_small_supported(n, dc, dk):
+      thetas, final, status, trace = dev.ard_adam_small(
+          xt, yt.reshape(-1), inits, lo, hi, learning_rate=opt.learning_rate, b1=opt.b1, b2=opt.b2, eps=opt.eps,
+          eps_root=opt.eps_root, epochs=self.epochs, z=zt, n_valid=n_valid)
+      return self._finish(list(thetas), final, trace, 'fused', status, best_n)
+    r = inits.shape[0]
+    if n > 64 and 1 < r <= 16 and not linear_coef:
+      fns = batch_loss_function(dev, xt, yt, zt, r, n_valid)
+    else:
+      fns = loss_functions(dev, xt, yt, zt, dc, dk, n_valid, workers=min(MAX_ARD_WORKERS, r), linear_coef=linear_coef)
+    return self(inits, fns, list(zip(lo, hi)), best_n=best_n)
+
+
 MAX_ARD_WORKERS = 8
 
 
@@ -291,16 +498,21 @@ def separable_loss_function(dev: gp.DeviceGP, xt, yt, zt, restarts: int, n_metri
 
 def train_gp(dev: gp.DeviceGP, x, y, z=None, *, rng: np.random.Generator,
              random_restarts: int = DEFAULT_RANDOM_RESTARTS, ensemble_size: int = 1,
-             optimizer: Optional[ScipyLbfgsB] = None, n_valid: Optional[int] = None,
+             optimizer=None, n_valid: Optional[int] = None,
              workers: int = MAX_ARD_WORKERS, linear_coef: Optional[float] = None,
              multitask_type=None) -> Tuple[List[gp.GPHyperParams], np.ndarray]:
   """Returns the best `ensemble_size` hyper-parameter sets and all final losses.
+
+  optimizer: ScipyLbfgsB (None: the default one) or OptaxTrain (Adam; not with a separable multitask_type).
 
   x [N,Dc] float64, z [N,Dk] int32 or None, y [N] or [N, M]: device tensors or arrays (copied once).
   multitask_type: a separable type (task_kernels.TYPES, a name or an enum member) fits the separable multi-task GP to
   y [N, M] with the restarts in lock step on `vzgp_nll_grad_separable_batch`; None / INDEPENDENT the independent one.
   """
   multitask_type = task_kernels.resolve(multitask_type)
+  if multitask_type and isinstance(optimizer, OptaxTrain):
+    raise NotImplementedError(f'OptaxTrain with the separable multi-task type {multitask_type} is not implemented '
+                              '(its task parameters have non-box bijectors).')
   import torch  # device-memory handles only
   optimizer = optimizer or ScipyLbfgsB()
   xt = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float64)).to(dev.device)
@@ -320,6 +532,13 @@ def train_gp(dev: gp.DeviceGP, x, y, z=None, *, rng: np.random.Generator,
                             multitask_type)
   lo, hi = gp.param_bounds(dc, dk, linear=bool(linear_coef))
   inits = log_uniform_init(rng, dc, dk, random_restarts, linear=bool(linear_coef))
+  if isinstance(optimizer, OptaxTrain):
+    try:
+      best, losses = optimizer.fit(dev, xt, yt, zt, inits, lo, hi, best_n=ensemble_size, n_valid=n_valid,
+                                   linear_coef=linear_coef)
+    finally:
+      dev.set_int('dataflow_ctas', 0)
+    return [gp.GPHyperParams.from_vector(t, dc, dk, linear_coef) for t in best], losses
   if BATCHED_ARD and _setulb is not None and xt.shape[0] > 64 and 1 < random_restarts <= 16 and workers > 1 and not linear_coef:
     fns = batch_loss_function(dev, xt, yt, zt, random_restarts, n_valid)
   else:

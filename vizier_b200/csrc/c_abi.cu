@@ -638,7 +638,7 @@ int vzgp_destroy(vzgp_handle* h) {
                     &h->scratch, &h->small, &h->xs_dev, &h->out_dev, &h->eagle, &h->pe_tmp, &h->pe_multi_tmp,
                     &h->LinvT, &h->df_tasks[0], &h->df_tasks[1], &h->df_flags, &h->df_S, &h->scal, &h->gen,
                     &h->i8_planes, &h->i8_scale, &h->i8_kdig, &h->sep_y, &h->wk, &h->wk_scratch, &h->cat_sizes,
-                    &h->pareto})
+                    &h->pareto, &h->ard})
     b->release();
   eagle_step_free(h);
   if (h->pinned) cudaFreeHost(h->pinned);
@@ -947,6 +947,56 @@ int vzgp_nll_grad_multi(vzgp_handle* h, const double* X, const int32_t* Z, const
   if (retries < 0) return retries;
   finish_loss(p, Dc, Dk, n_valid, n_metrics, host2[1] + host2[0], hostg, loss_out, grad_out, host2[2]);
   return retries;
+}
+
+int vzgp_ard_adam_small_supported(int N, int Dc, int Dk) {
+  return N >= 1 && N <= kBlk && Dc >= 0 && Dc <= kMaxDc && Dk >= 0 && Dk <= kMaxDkWide && Dc + Dk > 0 &&
+         ard_adam_small_smem_bytes(Dc, Dk) <= kMaxDynSmem;
+}
+
+int vzgp_ard_adam_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int Dc, int Dk,
+                        int n_valid, int R, const double* theta0, const double* lower, const double* upper,
+                        const vzgp_adam* adam, double* theta_out, double* loss_out, int* status_out,
+                        double* loss_trace) {
+  VZ_ARG(h != nullptr, "handle");
+  VZ_ARG(theta0 && lower && upper && adam && theta_out && loss_out && status_out, "host arrays / adam config");
+  VZ_ARG(vzgp_ard_adam_small_supported(N, Dc, Dk), "1 <= N <= 64 and a model whose shared memory fits one CTA");
+  VZ_ARG(n_valid >= 1 && n_valid <= N, "1 <= n_valid <= N");
+  VZ_ARG(X != nullptr || Dc == 0, "X");
+  VZ_ARG(Z != nullptr || Dk == 0, "Z");
+  VZ_ARG(y != nullptr, "y");
+  VZ_ARG(R >= 1, "R >= 1");
+  VZ_ARG(adam->epochs >= 1, "epochs >= 1");
+  VZ_ARG(std::isfinite(adam->learning_rate) && adam->b1 >= 0.0 && adam->b1 < 1.0 && adam->b2 >= 0.0 && adam->b2 < 1.0 &&
+         adam->eps >= 0.0 && adam->eps_root >= 0.0, "finite learning rate, 0 <= b1, b2 < 1, eps, eps_root >= 0");
+  const int P = Dc + Dk + 2;
+  for (int p = 0; p < P; ++p)
+    VZ_ARG(std::isfinite(lower[p]) && std::isfinite(upper[p]) && lower[p] < upper[p], "finite bounds, lower < upper");
+  Guard g(h->device);
+  const size_t np = (size_t)R * P, nt = (size_t)adam->epochs * R;
+  const size_t doubles = 2 * np + 2 * (size_t)P + R + nt;
+  // a larger buffer replaces the old one, which earlier launches on the stream may still be reading
+  if (sizeof(double) * doubles + sizeof(int) * R > h->ard.bytes && h->ard.ptr) VZ_CUDA(cudaStreamSynchronize(h->stream));
+  VZ_TRY(h->ard.reserve(sizeof(double) * doubles + sizeof(int) * R));
+  double* d_theta0 = h->ard.as<double>();
+  double* d_lo = d_theta0 + np;
+  double* d_hi = d_lo + P;
+  double* d_theta = d_hi + P;
+  double* d_loss = d_theta + np;
+  double* d_trace = d_loss + R;
+  int* d_status = reinterpret_cast<int*>(d_trace + nt);
+  VZ_CUDA(cudaMemcpyAsync(d_theta0, theta0, sizeof(double) * np, cudaMemcpyHostToDevice, h->stream));
+  VZ_CUDA(cudaMemcpyAsync(d_lo, lower, sizeof(double) * P, cudaMemcpyHostToDevice, h->stream));
+  VZ_CUDA(cudaMemcpyAsync(d_hi, upper, sizeof(double) * P, cudaMemcpyHostToDevice, h->stream));
+  VZ_TRY(launch_ard_adam_small(h, X, Z, y, N, n_valid, Dc, Dk, R, d_theta0, d_lo, d_hi, adam->learning_rate, adam->b1,
+                               adam->b2, adam->eps, adam->eps_root, adam->epochs, d_theta, d_loss, d_status,
+                               loss_trace ? d_trace : nullptr));
+  VZ_CUDA(cudaMemcpyAsync(theta_out, d_theta, sizeof(double) * np, cudaMemcpyDeviceToHost, h->stream));
+  VZ_CUDA(cudaMemcpyAsync(loss_out, d_loss, sizeof(double) * R, cudaMemcpyDeviceToHost, h->stream));
+  VZ_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * R, cudaMemcpyDeviceToHost, h->stream));
+  if (loss_trace) VZ_CUDA(cudaMemcpyAsync(loss_trace, d_trace, sizeof(double) * nt, cudaMemcpyDeviceToHost, h->stream));
+  VZ_CUDA(cudaStreamSynchronize(h->stream));
+  return 0;
 }
 
 static int check_scoring(vzgp_handle* h, const double* Xs, const int32_t* Zs, int M,

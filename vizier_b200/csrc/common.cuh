@@ -223,4 +223,8 @@ struct vzgp_handle {
 
   // Cumulative hypervolume (pareto.cu): per-CTA partial sums [CTAs][n] of the last call.
   vzgp::DevBuf pareto;
+
+  // Fused Adam ARD (ard_adam.cu): initial points, bounds, final parameters, losses, loss trace and status of the last
+  // vzgp_ard_adam_small call.
+  vzgp::DevBuf ard;
 };

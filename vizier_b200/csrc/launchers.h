@@ -172,6 +172,12 @@ int launch_gather_rows(vzgp_handle* h, const double* X, int dc, const long long*
                        int64_t M, double* out);
 
 size_t nll_small_smem_bytes(int dc, int dk);
+// Fused Adam ARD of a small study (ard_adam.cu): R restarts x `epochs` epochs in one launch of R CTAs.
+size_t ard_adam_small_smem_bytes(int dc, int dk);
+int launch_ard_adam_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int n_valid,
+                          int dc, int dk, int R, const double* theta0, const double* lower, const double* upper,
+                          double lr, double b1, double b2, double eps, double eps_root, int epochs, double* theta_out,
+                          double* loss_out, int* status_out, double* trace);
 int launch_nll_grad_small(vzgp_handle* h, const double* X, const int32_t* Z, const double* y, int N, int n_valid,
                           const KernelParams& kp, double sn2, double jitter0, int max_iters, double* out);
 // The acquisition and its gradient in the continuous features (score_grad.cu): hs[0..E), E = 1 for one model, scored

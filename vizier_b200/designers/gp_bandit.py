@@ -16,6 +16,11 @@ multi-task GP (one factor, one alpha per metric) scored by the mean over `num_sc
 hyper-volume scalarisations, without a trust region.  `multitask_type` SEPARABLE_NORMAL / LKJ / DIAG_TASK_KERNEL_PRIOR
 fits the separable multi-task GP instead (a task covariance shared by correlated metrics; `gp.SeparableGP`,
 task_kernels.py), scored, optimised and sampled the same way.
+`ard_optimizer` is `ard.ScipyLbfgsB` (the default) or `ard.OptaxTrain(ard.adam(lr), epochs=T)`, Adam in SoftClip-
+unconstrained coordinates (optax_wrappers.py:36-150): single-metric studies of up to 64 trials without `linear_coef` run
+every epoch of every restart in one kernel launch (csrc/ard_adam.cu), all others one device evaluation per epoch; it
+serves single models, ensembles, multi-metric models, `linear_coef` and every level of a `set_priors` stack, and raises
+NotImplementedError with the separable multi-task types.
 `linear_coef` adds the feature-scaled linear kernel and the constant mean of tuned_gp_models.py:203-245
 (general launch sequences: no captured graph, explicit K* for the scoring).
 `set_priors` trains a stack of residual GPs, one level per prior study plus the current study on top (gp_bandit.py:289-318;
@@ -128,7 +133,7 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
   """GP-Bandit designer; see module docstring."""
 
   def __init__(self, problem, *, acquisition_optimizer_factory: vb.VectorizedOptimizerFactory = default_acquisition_optimizer_factory,
-               ard_optimizer: Optional[ard.ScipyLbfgsB] = None, ard_random_restarts: int = ard.DEFAULT_RANDOM_RESTARTS,
+               ard_optimizer=None, ard_random_restarts: int = ard.DEFAULT_RANDOM_RESTARTS,
                num_seed_trials: int = 1, linear_coef: Optional[float] = None, scoring_function_factory=None,
                scoring_function_is_parallel: bool = False, padding_schedule=None, use_trust_region: bool = True,
                rng: Any = None, ensemble_size: Optional[int] = 1, output_warper=None, num_scalarizations: int = 1000,
@@ -157,6 +162,9 @@ class VizierGPBandit(vz.Designer, vz.Predictor):
                                 'returning QEI, QPI or QUCB.')
     if self._n_metrics > 1 and self._ensemble_size > 1:
       raise NotImplementedError('ensembles of multi-metric models are not implemented.')
+    if self._multitask_type and isinstance(ard_optimizer, ard.OptaxTrain):
+      raise NotImplementedError(f'OptaxTrain with the separable multi-task type {self._multitask_type} is not '
+                                'implemented (its task parameters have non-box bijectors).')
     del padding_schedule, multitask_type
     self._num_scalarizations = int(num_scalarizations)
     self._ref_scaling = float(ref_scaling)

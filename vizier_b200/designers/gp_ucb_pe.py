@@ -3,7 +3,10 @@
 Mirrors vizier/_src/algorithms/designers/gp_ucb_pe.py:609-1445 on the single-metric default
 configuration (`UCBPEConfig()` with `optimize_set_acquisition_for_exploration=False`):
 
-  * ARD: 4 random + 1 fixed initialisation (:828-838), L-BFGS-B maxiter=500, tol=1e-5 (:596-604);
+  * ARD: 4 random + 1 fixed initialisation (:828-838), L-BFGS-B maxiter=500, tol=1e-5 (:596-604), or, with
+    `ard_optimizer=ard.OptaxTrain(ard.adam(lr), epochs=T)`, Adam in SoftClip-unconstrained coordinates from the same
+    initial points (one kernel launch for single-metric studies of up to 64 trials without `mixes_linear_kernel`, one
+    device evaluation per epoch otherwise; ard.py);
   * model A = GP on the completed trials (mean, stddev); model B = same hyper-parameters on
     completed + pending trials (stddev_from_all; noise forced to 1e-10 when the signal-to-noise
     ratio is low, :996-1004);
@@ -157,7 +160,7 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
   """GP-UCB-PE designer; see module docstring."""
 
   def __init__(self, problem, *, acquisition_optimizer_factory: vb.VectorizedOptimizerFactory = default_acquisition_optimizer_factory,
-               ensemble_size: Optional[int] = 1, ard_optimizer: Optional[ard.ScipyLbfgsB] = None,
+               ensemble_size: Optional[int] = 1, ard_optimizer=None,
                ard_random_restarts: int = 4, use_trust_region: bool = True, num_seed_trials: int = 1,
                config: UCBPEConfig = UCBPEConfig(), rng: Any = None, clear_jax_cache: bool = False,
                padding_schedule=None, prior_acquisition=None, mixes_linear_kernel: bool = False,
@@ -302,6 +305,12 @@ class VizierGPUCBPEBandit(vz.Designer, vz.Predictor):
     lo, hi = gp.param_bounds(dc, dk, bool(lin))
     if lin:
       inits = np.clip(inits, lo, hi)     # the fixed slope 0 sits below its lower bound: L-BFGS-B starts from the projection
+    if isinstance(self._ard_optimizer, ard.OptaxTrain):
+      try:
+        best, _ = self._ard_optimizer.fit(dev_a, xt, yt, zt, inits, lo, hi, best_n=self._ensemble_size, linear_coef=lin)
+      finally:
+        dev_a.set_int('dataflow_ctas', 0)
+      return self._params_out(best, dc, dk)
 
     # all initial points advance in lock step, one CUDA-graph launch per round (ard.batch_loss_function); small
     # studies (one fused kernel per evaluation) keep one host thread per point

@@ -676,6 +676,37 @@ class DeviceGP:
 
     return f
 
+  def ard_adam_small(self, x, y, theta0, lower, upper, *, learning_rate: float, b1: float, b2: float, eps: float,
+                     eps_root: float, epochs: int, z=None, n_valid=None, trace: bool = True):
+    """ARD with Adam for a single-metric study of N <= 64 trials: every epoch of every restart in one launch
+    (`vzgp_ard_adam_small`, csrc/ard_adam.cu).  theta0 [R, P] initial points and lower, upper [P] finite bounds, in
+    to_vector order.  Returns (theta [R, P] after the last update, final losses [R], status [R] (Cholesky retries of
+    the last evaluation), loss trace [epochs, R] or None).  A restart whose evaluation failed keeps NaN losses from
+    that epoch on and the parameters of that evaluation."""
+    xt, zt = self._xz(x, z)
+    n, dc = xt.shape
+    yt = self._dev(y, torch.float64).reshape(-1)
+    if yt.shape[0] != n:
+      raise ValueError('ard_adam_small takes one metric: y [N]')
+    dk = 0 if zt is None else zt.shape[1]
+    th0 = np.ascontiguousarray(np.atleast_2d(np.asarray(theta0, np.float64)))
+    r, p = th0.shape
+    lo = np.ascontiguousarray(np.asarray(lower, np.float64).reshape(-1))
+    hi = np.ascontiguousarray(np.asarray(upper, np.float64).reshape(-1))
+    if p != dc + dk + 2 or lo.shape[0] != p or hi.shape[0] != p:
+      raise ValueError(f'theta0 [R, {dc + dk + 2}] and bounds [{dc + dk + 2}] expected')
+    cfg = _lib.Adam(float(learning_rate), float(b1), float(b2), float(eps), float(eps_root), int(epochs))
+    theta = np.zeros((r, p), np.float64)
+    losses = np.zeros(r, np.float64)
+    status = np.zeros(r, np.int32)
+    tr = np.zeros((int(epochs), r), np.float64) if trace else None
+    pd = lambda a: a.ctypes.data_as(C.POINTER(C.c_double))   # noqa: E731
+    _lib.check('vzgp_ard_adam_small', self._lib.vzgp_ard_adam_small(
+        self._h, _ptr(xt), _ptr(zt), _ptr(yt), n, dc, dk, n if n_valid is None else int(n_valid), r, pd(th0), pd(lo),
+        pd(hi), C.byref(cfg), pd(theta), pd(losses), status.ctypes.data_as(C.POINTER(C.c_int)),
+        pd(tr) if tr is not None else None))
+    return theta, losses, status, tr
+
   @staticmethod
   def make_batch_loss_fn(devs: Sequence['DeviceGP'], x, y, z=None, n_valid=None):
     """(indices, thetas) -> (losses, grads) for the restarts of one ARD fit: restart i is evaluated on
