@@ -7,9 +7,11 @@ runs the k_score<true> instance (L-inf distance); bench.py times that instance a
 Counters are summed over all CTAs and reported per tile: phase 1 (K* tile), the gate after it, phase 2
 (DMMA slab stream), the whole tile (all of math warp 0), the average math warp's wait on the full
 barriers (ring starved: operand feed too slow) and the producer's wait on the empty barriers (ring full:
-the math warps are the limit).  Phase 1 is split into the d2 loop, Matern + mu, the scratch stores (K* written
+the math warps are the limit).  Phase 1 is split into d2 (without --trust-region: the norms and the DMMA cross
+term of the centred form, timed to the last DMMA's result; with it: the difference-first loop), Matern + mu, the scratch stores (K* written
 to the shared-memory staging buffer, plus the TMA store issue) and the waits: barriers, cp.async and the TMA
-stores (math warp 0)."""
+stores (math warp 0).  Between builds whose d2 forms differ, phase 1 as a whole is the fair comparison: where the
+work of one part moves, its latency can show up in the next counter."""
 import ctypes as C
 import json
 import sys

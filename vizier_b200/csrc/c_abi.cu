@@ -68,7 +68,7 @@ struct Guard {
 
 static int ensure_model_buffers(vzgp_handle* h, int np, int dc, int dk, int n_metrics = 1) {
   VZ_TRY(h->X.reserve(sizeof(double) * (size_t)np * (dc > 0 ? dc : 1)));
-  VZ_TRY(h->XT.reserve(sizeof(double) * 2 * (size_t)np * (dc > 0 ? dc : 1)));
+  VZ_TRY(h->XT.reserve(sizeof(double) * xt_doubles(dc > 0 ? dc : 1, np)));
   VZ_TRY(h->Z.reserve(sizeof(int32_t) * (size_t)np * (dk > 0 ? dk : 1)));
   VZ_TRY(h->L.reserve(sizeof(double) * (size_t)np * np));
   VZ_TRY(h->Linv.reserve(sizeof(double) * (size_t)np * np));
@@ -195,6 +195,7 @@ static int fit_common(vzgp_handle* h, const double* X, const int32_t* Z, const d
   VZ_ARG(!kp.use_linear || n_metrics == 1, "linear_coef with several metrics is not implemented");
   if (dc > 0) VZ_TRY(launch_pad_rows(h, X, N, dc, np, h->X.as<double>()));
   if (dc > 0) VZ_TRY(launch_transpose_scale(h, h->X.as<double>(), np, dc, kp, h->XT.as<double>()));
+  VZ_TRY(launch_centre_trials(h, h->X.as<double>(), np, n_valid, dc, kp, h->XT.as<double>()));
   if (dk > 0) VZ_TRY(launch_pad_rows_i32(h, Z, N, dk, np, h->Z.as<int32_t>()));
   VZ_TRY(launch_kernel_matrix(h, h->X.as<double>(), h->Z.as<int32_t>(), np, n_valid, kp, h->sn2,
                               h->Kws.as<double>(), np));

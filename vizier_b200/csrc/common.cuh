@@ -90,6 +90,15 @@ struct DevBuf {
   T* as() const { return reinterpret_cast<T*>(ptr); }
 };
 
+// Layout of a handle's XT buffer (offsets in doubles): three [dc][np] planes of transposed trials - scaled by
+// 1/ls, unscaled, and centred then scaled (k_score's fast instance) - then the [np] squared norms of the third
+// plane and the [dc] centre it was taken about.  The writers (k_transpose_scale, k_centre_trials), the readers and
+// the allocation all take their offsets from here.
+__host__ __device__ constexpr size_t xt_plane(int p, int dc, int np) { return (size_t)p * dc * np; }
+__host__ __device__ constexpr size_t xt_norms(int dc, int np) { return xt_plane(3, dc, np); }
+__host__ __device__ constexpr size_t xt_centre(int dc, int np) { return xt_norms(dc, np) + np; }
+__host__ __device__ constexpr size_t xt_doubles(int dc, int np) { return xt_centre(dc, np) + dc; }
+
 // Kernel hyper-parameters in the form the kernels consume (device constant-ish,
 // passed by value in kernel arguments; <= 4 KB parameter space is fine).
 struct KernelParams {
@@ -129,7 +138,8 @@ struct vzgp_handle {
   double sn2 = 0.0;
   double mean_const = 0.0;   // constant prior mean (linear_coef variant), 0 otherwise
   vzgp::DevBuf X;      // [np x dc]
-  vzgp::DevBuf XT;     // [2][dc x np]: transposed trials, scaled by 1/ls (first) and unscaled (second)
+  vzgp::DevBuf XT;     // transposed trials, norms and centre: xt_plane / xt_norms / xt_centre (the third plane,
+                       // the norms and the centre are written by fits only)
   vzgp::DevBuf Z;      // [np x dk] int32
   vzgp::DevBuf L;      // [np x np]
   vzgp::DevBuf Linv;   // [np x np]

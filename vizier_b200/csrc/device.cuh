@@ -224,4 +224,11 @@ __device__ __forceinline__ void dmma_16x8x8(double& d0, double& d1, double& d2, 
                : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
 }
 
+// m16n8k4 f64 (sm_90): A 16 x 4 (a0 row g, a1 row g + 8, column t), B 4 x 8 (b0 row t, column g).
+__device__ __forceinline__ void dmma_16x8x4(double& d0, double& d1, double& d2, double& d3, double a0, double a1, double b0) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+               : "+d"(d0), "+d"(d1), "+d"(d2), "+d"(d3)
+               : "d"(a0), "d"(a1), "d"(b0));
+}
+
 }  // namespace vzgp

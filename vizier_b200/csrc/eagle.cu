@@ -490,7 +490,7 @@ bool eagle_persistent_eligible(const vzgp_handle* h, const vzgp_handle* hB, cons
 
 static SmallModel small_model_of(const vzgp_handle* h) {
   SmallModel m;
-  m.XTu = h->XT.as<double>() + (size_t)h->dc * h->np;
+  m.XTu = h->XT.as<double>() + xt_plane(1, h->dc, h->np);
   m.Z = h->Z.as<int32_t>();
   m.Linv = h->Linv.as<double>();
   m.alpha = h->alpha.as<double>();

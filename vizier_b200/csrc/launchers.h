@@ -54,6 +54,8 @@ int launch_add_scalar(vzgp_handle* h, int n, double a, double* y);
 int launch_pad_vector(vzgp_handle* h, const double* src, int n, int n_valid, int np, double* dst, double offset = 0.0);
 int launch_pad_rows(vzgp_handle* h, const double* src, int n, int d, int np, double* dst);
 int launch_transpose_scale(vzgp_handle* h, const double* X, int np, int dc, const KernelParams& kp, double* XT);
+int launch_centre_trials(vzgp_handle* h, const double* X, int np, int n_valid, int dc, const KernelParams& kp,
+                         double* XT);
 int launch_pad_rows_i32(vzgp_handle* h, const int32_t* src, int n, int d, int np, int32_t* dst);
 int launch_logdet_quad(vzgp_handle* h, const double* L, int ld, int n, int n_valid, const double* w, double* out,
                        int wstride = 0, int n_metrics = 1, const double* alpha = nullptr);

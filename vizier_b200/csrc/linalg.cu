@@ -437,8 +437,48 @@ __global__ void k_transpose_scale(const double* __restrict__ X, int np, int dc, 
   if (e >= (size_t)np * dc) return;
   int d = (int)(e / np), i = (int)(e % np);
   double v = X[(size_t)i * dc + d];
-  XT[e] = v * kp.inv_ls_c[d];
-  XT[(size_t)np * dc + e] = v;
+  XT[xt_plane(0, dc, np) + e] = v * kp.inv_ls_c[d];
+  XT[xt_plane(1, dc, np) + e] = v;
+}
+
+// XT[2][d][i] = (X[i][d] - c[d]) * inv_ls[d], nb[i] = sum_d XT[2][d][i]^2 and c[d], the midpoint of the valid
+// trials' range in dimension d (the layout of common.cuh: xt_plane(2), xt_norms, xt_centre).  k_score's fast instance forms
+// d2 = |a_c|^2 + |b_c|^2 - 2 a_c.b_c from these: centred, the norms stay near the spread of the trials, not near
+// their distance from the origin, and so does the rounding of the difference.  One block.
+__global__ void __launch_bounds__(1024) k_centre_trials(const double* __restrict__ X, int np, int n_valid, int dc,
+                                                        KernelParams kp, double* __restrict__ XT) {
+  __shared__ double s_c[kMaxDc];
+  double* xc = XT + xt_plane(2, dc, np);
+  double* nb = XT + xt_norms(dc, np);
+  double* ctr = XT + xt_centre(dc, np);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int d = warp; d < dc; d += blockDim.x >> 5) {
+    double lo = INFINITY, hi = -INFINITY;
+    for (int i = lane; i < n_valid; i += 32) {
+      const double v = X[(size_t)i * dc + d];
+      lo = fmin(lo, v);
+      hi = fmax(hi, v);
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+      hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    }
+    if (lane == 0) {
+      const double c = n_valid > 0 ? 0.5 * lo + 0.5 * hi : 0.0;
+      s_c[d] = c;
+      ctr[d] = c;
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < np; i += blockDim.x) {
+    double n = 0.0;
+    for (int d = 0; d < dc; ++d) {
+      const double b = (X[(size_t)i * dc + d] - s_c[d]) * kp.inv_ls_c[d];
+      xc[(size_t)d * np + i] = b;
+      n = fma(b, b, n);
+    }
+    nb[i] = n;
+  }
 }
 
 __global__ void k_pad_rows_i32(const int32_t* __restrict__ src, int n, int d, int np,
@@ -711,6 +751,14 @@ int launch_transpose_scale(vzgp_handle* h, const double* X, int np, int dc, cons
   size_t tot = (size_t)np * dc;
   if (tot == 0) return 0;
   k_transpose_scale<<<(unsigned)((tot + 255) / 256), 256, 0, h->stream>>>(X, np, dc, kp, XT);
+  VZ_CHECK_LAUNCH();
+  h->launches++;
+  return 0;
+}
+int launch_centre_trials(vzgp_handle* h, const double* X, int np, int n_valid, int dc, const KernelParams& kp,
+                         double* XT) {
+  if (np == 0) return 0;
+  k_centre_trials<<<1, 1024, 0, h->stream>>>(X, np, n_valid, dc, kp, XT);
   VZ_CHECK_LAUNCH();
   h->launches++;
   return 0;

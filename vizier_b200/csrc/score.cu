@@ -10,8 +10,9 @@
 //
 // One persistent CTA per SM walks 64-candidate tiles:
 //   phase 1  K* tile [64 x np] = Matern(x*, X) built 64 columns at a time from shared-memory
-//            staged rows; mu = K* alpha and the L-inf trust-region distance are reduced on the
-//            fly; each 64-column step of the tile is written to shared memory in the layout of phase 2's
+//            staged rows (without the trust-region distance, d2 = |a_c|^2 + |b_c|^2 - 2 a_c.b_c of centred
+//            features, the cross term on the DMMA pipe); mu = K* alpha and the L-inf trust-region distance
+//            are reduced on the fly; each 64-column step of the tile is written to shared memory in the layout of phase 2's
 //            TMA boxes and leaves by TMA store to a CTA-private scratch (L2 resident, never re-read by others).
 //   phase 2  W = K* . Linv^T in 64 x 128 blocks on the FP64 tensor pipe (mma.sync m16n8k8 f64: on the
 //            H100 the m8n8k4 shape issues at half the rate), operands streamed by a TMA producer warp
@@ -41,7 +42,7 @@
 
 namespace vzgp {
 
-using GP1 = GemmCfg<64, 64, 16, 4, 4>;  // phase-1 thread mapping: 256 threads, 4x4 outputs each
+using GP1 = GemmCfg<64, 64, 16, 4, 4>;  // phase-1 thread mapping of the trust-region instances: 256 threads, 4x4 outputs each
 constexpr int kThreads = 256;        // consumer threads (8 math warps)
 constexpr int kBlockThreads = 288;   // + one TMA producer warp
 static_assert(GP1::kThreads == kThreads, "phase 1 maps one d2 block to every math thread");
@@ -94,7 +95,7 @@ static_assert(stg_buffers(45) == 3 && stg_buffers(46) == 2 && stg_buffers(61) ==
 // Instrumented build only (make timing): clock64 sums over all CTAs, read by vzgp_debug_score_timing.
 // [0] tiles  [1] phase 1  [2] phase 2  [3] tile gate (barrier after phase 1)  [4] whole tile   (math warp 0)
 // [5] math warps waiting on full barriers (summed over the 8 warps)  [6] producer waiting on empty barriers
-// phase 1, math warp 0: [7] d2 loop  [8] Matern + mu  [9] scratch stores (K* written to the staging buffer, and
+// phase 1, math warp 0: [7] d2 (the fast instance: n_a + n_b, the DMMA cross term and the categorical terms)  [8] Matern + mu  [9] scratch stores (K* written to the staging buffer, and
 // thread 0's TMA store issue)  [10] barriers, cp.async waits and thread 0's waits for the TMA stores
 constexpr int kScoreCounters = 11;
 __device__ unsigned long long g_score_t[kScoreCounters];
@@ -120,8 +121,8 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   double* sk = ring;                                     // [nstg][8 boxes]  K* of a step, 1024-byte aligned
   double* sa = sk + nstg * kStgDoubles;                  // [dc][LD]     candidates (transposed)
   double* sb = sa + dc * LD;                             // [3][trial_stride]  trials [dc][LD] and alpha [64]
-  double* s_mu = ring + kStages * kStageDoubles;         // [64]
-  double* s_linf = s_mu + 64;                            // [64]
+  double* s_mu = ring + kStages * kStageDoubles;         // [4][64]  one partial mean per column quarter (one [64] with WITH_LINF)
+  double* s_linf = s_mu + 256;                           // [64]
   double* s_rowsq = s_linf + 64;                         // [4][64]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_rowsq + 256);  // [kStages] TMA bytes landed
   uint64_t* empty_bar = full_bar + kStages;                         // [kStages] all 8 math warps of every CTA in the cluster released the stage
@@ -131,7 +132,11 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int ty = tid / 16, tx = tid % 16;      // phase-1 mapping (16 x 16 threads)
-  const int wm = warp & 1, wn = warp >> 1;     // phase-2 warp grid 2 (M) x 4 (N)
+  // Warp grid 2 (M) x 4 (N) of phase 2 (and of the fast instance's phase 1).  Warp w runs on SM sub-partition
+  // w % 4, and column quarter wn of a 128-column block runs 4 jb + wn + 1 slabs (Linv is triangular).  Warps
+  // 4-7 take quarters 3, 3, 2, 2, so every sub-partition holds quarters {0, 3} or {1, 2}: 8 jb + 5 slab-units
+  // per block on each (with wn = warp / 2 it was 8 jb + 4 on two of them and 8 jb + 6 on the other two).
+  const int wm = warp & 1, wn = (warp >> 1) ^ (warp >> 2);
   const int fr = lane >> 2, fk = lane & 3;     // fragment row / k within a DMMA tile
   // Linv row (output column) that B fragment row fr stands for within its 8-row group.  An LDS.128 is
   // served 8 lanes at a time; lanes 0-7 are fragment rows 0 and 1.  With the 128-byte swizzle rows r and
@@ -164,8 +169,10 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
   const int ntiles = (a.M + kTM - 1) / kTM;
   const int nblocks = (np + kBN - 1) / kBN;
   const int nsplit = a.nsplit;
-  const double* XTs = a.XT;
-  const double* XTu = a.XT + (size_t)dc * np;
+  const double* XTu = a.XT + xt_plane(1, dc, np);   // unscaled (trust-region instances)
+  const double* XTc = a.XT + xt_plane(2, dc, np);   // centred and scaled (fast instance)
+  const double* nb_g = a.XT + xt_norms(dc, np);     // [np] their squared norms
+  const double* ctr = a.XT + xt_centre(dc, np);     // [dc] the centre
 
   // The CTAs of a cluster take adjacent work items and run the same number of rounds.  In the last
   // round a CTA can be left without a tile (work >= ntiles, nsplit == 1): it scores an all-padding tile
@@ -214,12 +221,13 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     }
     VZ_ST(const long long t_tile0 = clock64(); w_tile = 0;)
     consumer_sync();  // previous tile fully consumed by the math warps (sa, s_mu, s_rowsq, ring)
-    // candidate tile, transposed and in pair order; scaled by 1/ls like the reference's FeatureScaled kernel
+    // candidate tile, transposed and in pair order.  The fast instance stages -2 a_c, a_c = (x - centre) / ls
+    // (the trials' centre, the reference's FeatureScaled scaling), the A operand of the cross term.
     for (int e = tid; e < kTM * dc; e += kThreads) {
       const int r = e / dc, d = e - r * dc;
       const int gr = m0 + r;
       const double v = gr < a.M ? __ldg(a.Xs + (size_t)gr * dc + d) : 0.0;
-      sa[d * LD + pair_pos(r)] = WITH_LINF ? v : v * a.kp.inv_ls_c[d];
+      sa[d * LD + pair_pos(r)] = WITH_LINF ? v : -2.0 * ((v - ctr[d]) * a.kp.inv_ls_c[d]);
     }
     if (dk > 0) stage_rows_T_i32(a.Zs, a.M, dk, m0, kTM, za, LD, kThreads);
 
@@ -229,7 +237,7 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     // it fills was last read in step jb-2, which every thread left before the barrier of step jb-1.
     auto stage_trials = [&](int jb, int buf) {
       double* dst = sb + buf * trial_stride(dc);
-      const double* src = WITH_LINF ? XTu : XTs;
+      const double* src = WITH_LINF ? XTu : XTc;
       for (int c = tid; c < dc * 32; c += kThreads) {       // dc rows x 32 chunks of 16 B
         const int d = c >> 5, q = c & 31;
         cp_async16(dst + d * LD + q * 2, src + (size_t)d * np + jb * 64 + q * 2, true);
@@ -254,6 +262,12 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       const int buf = jb % kTrialBufs;
       if (jb + 1 < nj) stage_trials(jb + 1, (jb + 1) % kTrialBufs);
       cp_async_commit();
+      // |b_c|^2 of the lane's four columns (fast instance), loaded before the barrier wait
+      double2 nbv[2];
+      if constexpr (!WITH_LINF) {
+#pragma unroll
+        for (int nf = 0; nf < 2; ++nf) nbv[nf] = __ldg(reinterpret_cast<const double2*>(nb_g + jb * 64 + 16 * wn + 8 * nf + 2 * fk));
+      }
       cp_async_wait<1>();
       // With nstg >= 2 staging buffers, step jb writes the one the store of step jb-nstg reads.  That store was
       // issued at the start of step jb-nstg+1, and at most the nstg-2 stores issued after it may still be reading;
@@ -271,25 +285,27 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       VZ_ST(t_st += clock64() - tc; tc = clock64();)
       const double* sbj = sb + buf * trial_stride(dc);
       const double* alj = sbj + dc * LD;
-      double d2[4][4], lf[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { d2[i][j] = 0.0; lf[i][j] = 0.0; }
-      // Software-pipelined over d: the LDS.128 operands of dimension d + 1 (and its weight and mask) are loaded
-      // while the 32 FP64 operations of dimension d run.  The FMA sequence of every element is unchanged.
+      // kv: the sixteen kernel values of this thread (the two instances map them to the step differently).
+      double kv[4][4];
       auto ld2 = [](const double* p) { return *reinterpret_cast<const double2*>(p); };
-      double2 a0 = ld2(sa + GP1::row_of(ty, 0)), a1 = ld2(sa + GP1::row_of(ty, 2));
-      double2 b0 = ld2(sbj + GP1::col_of(tx, 0)), b1 = ld2(sbj + GP1::col_of(tx, 2));
-      double w_n = WITH_LINF ? a.kp.inv_ls2_c[0] : 0.0;
-      bool in_tr_n = WITH_LINF ? s_mask[0] != 0 : false;
-      for (int d = 0; d < dc; ++d) {
-        const int dn = d + 1 < dc ? d + 1 : d;
-        const double2 a0n = ld2(sa + dn * LD + GP1::row_of(ty, 0)), a1n = ld2(sa + dn * LD + GP1::row_of(ty, 2));
-        const double2 b0n = ld2(sbj + dn * LD + GP1::col_of(tx, 0)), b1n = ld2(sbj + dn * LD + GP1::col_of(tx, 2));
-        const double aa[4] = {a0.x, a0.y, a1.x, a1.y}, bb[4] = {b0.x, b0.y, b1.x, b1.y};
-        a0 = a0n; a1 = a1n; b0 = b0n; b1 = b1n;
-        if (WITH_LINF) {
+      if constexpr (WITH_LINF) {
+        double d2[4][4], lf[4][4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) { d2[i][j] = 0.0; lf[i][j] = 0.0; }
+        // Software-pipelined over d: the LDS.128 operands of dimension d + 1 (and its weight and mask) are loaded
+        // while the 32 FP64 operations of dimension d run.  The FMA sequence of every element is unchanged.
+        double2 a0 = ld2(sa + GP1::row_of(ty, 0)), a1 = ld2(sa + GP1::row_of(ty, 2));
+        double2 b0 = ld2(sbj + GP1::col_of(tx, 0)), b1 = ld2(sbj + GP1::col_of(tx, 2));
+        double w_n = a.kp.inv_ls2_c[0];
+        bool in_tr_n = s_mask[0] != 0;
+        for (int d = 0; d < dc; ++d) {
+          const int dn = d + 1 < dc ? d + 1 : d;
+          const double2 a0n = ld2(sa + dn * LD + GP1::row_of(ty, 0)), a1n = ld2(sa + dn * LD + GP1::row_of(ty, 2));
+          const double2 b0n = ld2(sbj + dn * LD + GP1::col_of(tx, 0)), b1n = ld2(sbj + dn * LD + GP1::col_of(tx, 2));
+          const double aa[4] = {a0.x, a0.y, a1.x, a1.y}, bb[4] = {b0.x, b0.y, b1.x, b1.y};
+          a0 = a0n; a1 = a1n; b0 = b0n; b1 = b1n;
           const double w = w_n;
           const bool in_tr = in_tr_n;
           w_n = a.kp.inv_ls2_c[dn];
@@ -302,73 +318,183 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
               d2[i][j] = fma(df * df, w, d2[i][j]);
               if (in_tr) lf[i][j] = fmax(lf[i][j], fabs(df));
             }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const double df = aa[i] - bb[j];
-              d2[i][j] = fma(df, df, d2[i][j]);
-            }
         }
-      }
-      for (int k = 0; k < dk; ++k) {
-        const double w = a.kp.inv_ls2_k[k];
+        for (int k = 0; k < dk; ++k) {
+          const double w = a.kp.inv_ls2_k[k];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int avz = za[k * LD + pair_row(GP1::row_of(ty, i))];   // za is staged in row order
+          for (int i = 0; i < 4; ++i) {
+            const int avz = za[k * LD + pair_row(GP1::row_of(ty, i))];   // za is staged in row order
 #pragma unroll
-          for (int j = 0; j < 4; ++j) d2[i][j] += (avz != zb[k * LD + GP1::col_of(tx, j)]) ? w : 0.0;
+            for (int j = 0; j < 4; ++j) d2[i][j] += (avz != zb[k * LD + GP1::col_of(tx, j)]) ? w : 0.0;
+          }
         }
-      }
-      VZ_ST(t_d2 += clock64() - tc; tc = clock64();)
-      // The L-inf distances are folded before the Matern block so that they are not live across it.
-      if (WITH_LINF) {
+        VZ_ST(t_d2 += clock64() - tc; tc = clock64();)
+        // The L-inf distances are folded before the Matern block so that they are not live across it.
 #pragma unroll
         for (int i = 0; i < 4; ++i)
 #pragma unroll
           for (int j = 0; j < 4; ++j)
             if ((jb * 64 + GP1::col_of(tx, j)) < a.tr.rows) lmin[i] = fmin(lmin[i], lf[i][j]);
-      }
-      // The sixteen kernel values as one straight-line block of the branch-free Matern (independent chains
-      // the scheduler can interleave); columns at or past n_valid are zeroed by a select.
-      double kv[4][4];
+        // The sixteen kernel values as one straight-line block of the branch-free Matern (independent chains
+        // the scheduler can interleave); columns at or past n_valid are zeroed by a select.
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) kv[i][j] = matern52_fast(d2[i][j], a.kp.sf2);
+          for (int j = 0; j < 4; ++j) kv[i][j] = matern52_fast(d2[i][j], a.kp.sf2);
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int cj = GP1::col_of(tx, j);
-          kv[i][j] = (jb * 64 + cj) < a.n_valid ? kv[i][j] : 0.0;
-          mu_part[i] = fma(kv[i][j], alj[cj], mu_part[i]);
+          for (int j = 0; j < 4; ++j) {
+            const int cj = GP1::col_of(tx, j);
+            kv[i][j] = (jb * 64 + cj) < a.n_valid ? kv[i][j] : 0.0;
+            mu_part[i] = fma(kv[i][j], alj[cj], mu_part[i]);
+          }
+        VZ_ST(t_mat += clock64() - tc; tc = clock64();)
+      } else {
+        // d2 = |a_c|^2 + |b_c|^2 - 2 a_c.b_c of the centred features, the cross term on the DMMA pipe: the warp's
+        // 32 x 16 region of the step is 2 x 2 m16n8 tiles whose accumulators start at n_a + n_b.  k slots fk and
+        // fk + 4 of k step ks are dimensions 8 ks + 2 fk and 8 ks + 2 fk + 1, the same on both operands (the A loads
+        // are LDS.128 of a row pair, the B loads LDS.64; with LD = 66 both are conflict-free).  Dimensions past dc
+        // are zero on both sides.  kv[2 mf + f][2 nf + c]: row 32 wm + 16 mf + 8 f + fr, column 16 wn + 8 nf + 2 fk + c.
+        const double* Ab = sa + 32 * wm + 2 * fr;   // pair (2 wm + mf) * 8 + fr: rows fr and fr + 8 of M fragment mf
+        const double* Bb = sbj + 16 * wn + fr;
+        // n_a of the lane's four rows, kept in this warp's slice of s_mu (free until the tile's partial means)
+        double* s_na = s_mu + wn * 64 + 32 * wm + fr;
+        if (jb == 0) {   // the staged -2 a_c squared and summed, times 1/4 (exact)
+          double na[4] = {0.0, 0.0, 0.0, 0.0};
+          for (int d = 0; d < dc; ++d)
+#pragma unroll
+            for (int mf = 0; mf < 2; ++mf) {
+              const double2 v = ld2(Ab + d * LD + 16 * mf);
+              na[2 * mf] = fma(v.x, v.x, na[2 * mf]);
+              na[2 * mf + 1] = fma(v.y, v.y, na[2 * mf + 1]);
+            }
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            if (fk == 0) s_na[8 * i] = 0.25 * na[i];
+          __syncwarp();
         }
-      VZ_ST(t_mat += clock64() - tc; tc = clock64();)
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int nf = 0; nf < 2; ++nf) { kv[i][2 * nf] = s_na[8 * i] + nbv[nf].x; kv[i][2 * nf + 1] = s_na[8 * i] + nbv[nf].y; }
+        auto frag = [&](int ks, double2 (&fa)[2][2], double (&fb)[2][2]) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int d = 8 * ks + 2 * fk + e;
+            const bool ok = d < dc;
+#pragma unroll
+            for (int mf = 0; mf < 2; ++mf) fa[e][mf] = ok ? ld2(Ab + d * LD + 16 * mf) : make_double2(0.0, 0.0);
+#pragma unroll
+            for (int nf = 0; nf < 2; ++nf) fb[e][nf] = ok ? Bb[d * LD + 8 * nf] : 0.0;
+          }
+        };
+        double2 fa[2][2];
+        double fb[2][2];
+        frag(0, fa, fb);
+        // A remainder of 1-4 dimensions takes one m16n8k4 step instead of a half-empty m16n8k8 one.
+        const int k4 = (dc & 7) != 0 && (dc & 7) <= 4, kc = k4 ? dc >> 3 : (dc + 7) >> 3;
+#pragma unroll 1
+        for (int ks = 0; ks < kc; ++ks) {   // the fragments of k step ks + 1 load under the DMMAs of ks
+          double2 ga[2][2];
+          double gb[2][2];
+          frag(ks + 1 < kc ? ks + 1 : ks, ga, gb);
+#pragma unroll
+          for (int mf = 0; mf < 2; ++mf)
+#pragma unroll
+            for (int nf = 0; nf < 2; ++nf)
+              dmma_16x8x8(kv[2 * mf][2 * nf], kv[2 * mf][2 * nf + 1], kv[2 * mf + 1][2 * nf], kv[2 * mf + 1][2 * nf + 1],
+                          fa[0][mf].x, fa[0][mf].y, fa[1][mf].x, fa[1][mf].y, fb[0][nf], fb[1][nf]);
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int q = 0; q < 2; ++q) { fa[e][q] = ga[e][q]; fb[e][q] = gb[e][q]; }
+        }
+        if (k4) {   // k slot fk is dimension 8 kc + fk
+          const int d = 8 * kc + fk;
+          const bool ok = d < dc;
+#pragma unroll
+          for (int mf = 0; mf < 2; ++mf) {
+            const double2 av = ok ? ld2(Ab + d * LD + 16 * mf) : make_double2(0.0, 0.0);
+#pragma unroll
+            for (int nf = 0; nf < 2; ++nf)
+              dmma_16x8x4(kv[2 * mf][2 * nf], kv[2 * mf][2 * nf + 1], kv[2 * mf + 1][2 * nf], kv[2 * mf + 1][2 * nf + 1],
+                          av.x, av.y, ok ? Bb[d * LD + 8 * nf] : 0.0);
+          }
+        }
+        for (int k = 0; k < dk; ++k) {
+          const double w = a.kp.inv_ls2_k[k];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int avz = za[k * LD + 32 * wm + 8 * i + fr];   // za is staged in row order
+#pragma unroll
+            for (int j = 0; j < 4; ++j) kv[i][j] += (avz != zb[k * LD + 16 * wn + 8 * (j >> 1) + 2 * fk + (j & 1)]) ? w : 0.0;
+          }
+        }
+        // Instrumented build: wait for the last DMMA's result, so that the d2 counter covers the cross term.
+        VZ_ST(if (kv[3][3] == -1.0) t_d2 += 1;)
+        VZ_ST(t_d2 += clock64() - tc; tc = clock64();)
+        // Rounding can leave d2 a few ulps of n_a + n_b below zero where a candidate is a trial.  matern52_fast needs
+        // no clamp for that: 5 d2 < 1e-100 selects s = 0, so k = sf2 exactly as at d2 = 0, while a NaN (a non-finite
+        // candidate feature) stays a NaN, as in the difference-first form.
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) kv[i][j] = matern52_fast(kv[i][j], a.kp.sf2);
+#pragma unroll
+        for (int nf = 0; nf < 2; ++nf) {
+          const int cj = 16 * wn + 8 * nf + 2 * fk;
+          const double2 al = ld2(alj + cj);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            kv[i][2 * nf] = (jb * 64 + cj) < a.n_valid ? kv[i][2 * nf] : 0.0;
+            kv[i][2 * nf + 1] = (jb * 64 + cj + 1) < a.n_valid ? kv[i][2 * nf + 1] : 0.0;
+            mu_part[i] = fma(kv[i][2 * nf], al.x, mu_part[i]);
+            mu_part[i] = fma(kv[i][2 * nf + 1], al.y, mu_part[i]);
+          }
+        }
+        VZ_ST(t_mat += clock64() - tc; tc = clock64();)
+      }
       if (nstg == 1) {   // the single staging buffer: the store of step jb-1 must have read it
         if (tid == 0) bulk_wait_read<0>();
         consumer_sync();
       }
       VZ_ST(t_sync += clock64() - tc; tc = clock64();)
-      // Rows i = 2 ip, 2 ip + 1 of this thread are pair p = 16 ip + ty: one 16-byte store per column, into chunk
-      // c = col % 8 of row p of box col / 8, swizzled to chunk c ^ (p % 8).  A 16-byte store is served 8 lanes at
-      // a time, lanes tx = 0-7 of one ty: tx 0-3 and 4-7 write the same chunks of two boxes (4 KB apart, the same
-      // banks), so lanes with tx >= 4 take their two columns of a chunk pair in swapped order, filling the odd
-      // chunks while tx 0-3 fill the even ones.
-      {
-        double* stg = sk + (jb % nstg) * kStgDoubles;
-        const bool swap = (tx & 4) != 0;
+      if constexpr (WITH_LINF) {
+        // Rows i = 2 ip, 2 ip + 1 of this thread are pair p = 16 ip + ty: one 16-byte store per column, into chunk
+        // c = col % 8 of row p of box col / 8, swizzled to chunk c ^ (p % 8).  A 16-byte store is served 8 lanes at
+        // a time, lanes tx = 0-7 of one ty: tx 0-3 and 4-7 write the same chunks of two boxes (4 KB apart, the same
+        // banks), so lanes with tx >= 4 take their two columns of a chunk pair in swapped order, filling the odd
+        // chunks while tx 0-3 fill the even ones.
+        {
+          double* stg = sk + (jb % nstg) * kStgDoubles;
+          const bool swap = (tx & 4) != 0;
 #pragma unroll
-        for (int ip = 0; ip < 2; ++ip) {
-          const int p = 16 * ip + ty;
+          for (int ip = 0; ip < 2; ++ip) {
+            const int p = 16 * ip + ty;
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = jj ^ 1;
-            const double v0 = swap ? kv[2 * ip][j] : kv[2 * ip][jj], v1 = swap ? kv[2 * ip + 1][j] : kv[2 * ip + 1][jj];
-            const int cj = GP1::col_of(tx, jj) ^ (swap ? 1 : 0);
-            *reinterpret_cast<double2*>(stg + (cj >> 3) * kABox + p * 16 + (((cj & 7) ^ (p & 7)) * 2)) = make_double2(v0, v1);
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = jj ^ 1;
+              const double v0 = swap ? kv[2 * ip][j] : kv[2 * ip][jj], v1 = swap ? kv[2 * ip + 1][j] : kv[2 * ip + 1][jj];
+              const int cj = GP1::col_of(tx, jj) ^ (swap ? 1 : 0);
+              *reinterpret_cast<double2*>(stg + (cj >> 3) * kABox + p * 16 + (((cj & 7) ^ (p & 7)) * 2)) = make_double2(v0, v1);
+            }
           }
+        }
+      } else {
+        // Rows fr and fr + 8 of M fragment mf are pair p = (2 wm + mf) * 8 + fr, and column 2 fk + c of N fragment nf
+        // is chunk 2 fk + c of row p of box 2 wn + nf, swizzled to chunk (2 fk + c) ^ fr.  The 8 lanes of a 16-byte
+        // store phase (fr = 2i, 2i + 1) fill the even chunks of one row and the odd ones of the next: no conflict.
+        double* stg = sk + (jb % nstg) * kStgDoubles;
+#pragma unroll
+        for (int mf = 0; mf < 2; ++mf) {
+          const int p = (2 * wm + mf) * 8 + fr;
+#pragma unroll
+          for (int nf = 0; nf < 2; ++nf)
+#pragma unroll
+            for (int c = 0; c < 2; ++c)
+              *reinterpret_cast<double2*>(stg + (2 * wn + nf) * kABox + p * 16 + (((2 * fk + c) ^ fr) * 2)) =
+                  make_double2(kv[2 * mf][2 * nf + c], kv[2 * mf + 1][2 * nf + c]);
         }
       }
       fence_proxy_async_smem();   // these writes before the TMA store that reads them (issued after the next barrier)
@@ -386,17 +512,27 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
     if (tid == 0) bulk_wait<0>();
     VZ_ST(t_sync += clock64() - tc;)
     cp_async_wait<0>();
+    if constexpr (WITH_LINF) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
+      for (int i = 0; i < 4; ++i) {
 #pragma unroll
-      for (int o = 8; o > 0; o >>= 1) {
-        mu_part[i] += __shfl_xor_sync(0xffffffffu, mu_part[i], o);
-        if (WITH_LINF) lmin[i] = fmin(lmin[i], __shfl_xor_sync(0xffffffffu, lmin[i], o));
+        for (int o = 8; o > 0; o >>= 1) {
+          mu_part[i] += __shfl_xor_sync(0xffffffffu, mu_part[i], o);
+          lmin[i] = fmin(lmin[i], __shfl_xor_sync(0xffffffffu, lmin[i], o));
+        }
+        if (tx == 0) {
+          s_mu[pair_row(GP1::row_of(ty, i))] = mu_part[i];
+          s_linf[pair_row(GP1::row_of(ty, i))] = lmin[i];
+        }
       }
-      if (tx == 0) {
-        s_mu[pair_row(GP1::row_of(ty, i))] = mu_part[i];
-        s_linf[pair_row(GP1::row_of(ty, i))] = lmin[i];
+    } else {   // the four lanes of a fragment row, then the four column quarters in the epilogue
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        mu_part[i] += __shfl_xor_sync(0xffffffffu, mu_part[i], 1);
+        mu_part[i] += __shfl_xor_sync(0xffffffffu, mu_part[i], 2);
+        if (fk == 0) s_mu[wn * 64 + 32 * wm + 8 * i + fr] = mu_part[i];
       }
+      if (tid < kTM) s_linf[tid] = INFINITY;
     }
     fence_proxy_async();  // generic-proxy writes (scratch tile, aliased smem) before async-proxy (TMA) accesses
     VZ_ST(const long long t1 = clock64();)
@@ -501,12 +637,13 @@ __global__ void __launch_bounds__(kBlockThreads, 1) k_score(const __grid_constan
       const int r = tid, m = m0 + r;
       if (m < a.M) {
         const double rs = (s_rowsq[r] + s_rowsq[64 + r]) + (s_rowsq[128 + r] + s_rowsq[192 + r]);
+        const double mu = WITH_LINF ? s_mu[r] : (s_mu[r] + s_mu[64 + r]) + (s_mu[128 + r] + s_mu[192 + r]);
         if (nsplit == 1) {
-          emit_score<GENERIC>(a, m, rs, s_mu[r], s_linf[r], clamped);
+          emit_score<GENERIC>(a, m, rs, mu, s_linf[r], clamped);
         } else {
           a.part[(size_t)split * a.mpad + m] = rs;
           if (split == 0) {
-            a.part[(size_t)nsplit * a.mpad + m] = s_mu[r];
+            a.part[(size_t)nsplit * a.mpad + m] = mu;
             a.part[(size_t)(nsplit + 1) * a.mpad + m] = s_linf[r];
           }
         }
@@ -638,7 +775,7 @@ int make_tensor_map_u8(void* map, const void* base, int rank, const uint64_t* di
 
 size_t score_smem_bytes(int dc, int dk, bool with_linf) {
   (void)with_linf; (void)dc;   // phase 1's plan for any dc fits in the ring (stg_buffers)
-  return 1024 + sizeof(double) * (kStages * kStageDoubles + 64 * 2 + 256 + 8) +
+  return 1024 + sizeof(double) * (kStages * kStageDoubles + 256 + 64 + 256 + 8) +
          sizeof(int32_t) * dk * 2 * kLD1 + kMaxDc;
 }
 

@@ -295,7 +295,7 @@ int launch_score_grad(vzgp_handle* const* hs, int E, const double* Xs, int M, co
       k_grad_solve<<<dim3(np / 64, mp / 64), 256, GradGemm::kSmemBytes, h->stream>>>(c.W, h->Linv.as<double>(), np, c.Ks);
       VZ_CHECK_LAUNCH();
       GradRowsArgs a;
-      a.Xp = c.Xp; a.XTu = h->XT.as<double>() + (size_t)np * dc; a.alpha = h->alpha.as<double>();
+      a.Xp = c.Xp; a.XTu = h->XT.as<double>() + xt_plane(1, dc, np); a.alpha = h->alpha.as<double>();
       a.W = c.W; a.V = c.Ks;
       a.np = np; a.n_valid = h->n_valid; a.dc = dc; a.want_linf = (e == 0 && want_linf) ? 1 : 0;
       a.kp = h->kp; a.sn2 = h->sn2; a.mean_const = h->mean_const;

@@ -210,7 +210,7 @@ __global__ void __launch_bounds__(kI8Threads, 1) k_score_i8(const __grid_constan
     uint64_t keep_policy;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;\n" : "=l"(keep_policy));
     const double* XTs = a.XT;
-    const double* XTu = a.XT + (size_t)dc * np;
+    const double* XTu = a.XT + xt_plane(1, dc, np);
     unsigned it = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
       const int m0 = tile * kTM;

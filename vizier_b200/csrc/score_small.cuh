@@ -21,7 +21,7 @@ struct ScoreArgs {
   const double* Xs;
   const int32_t* Zs;
   int M;
-  const double* XT;   // [2][dc][np]: scaled / unscaled transposed trials
+  const double* XT;   // [3][dc][np]: scaled / unscaled / centred transposed trials, then [np] norms, [dc] centre (common.cuh)
   const int32_t* Z;
   int np;
   int n_valid;
@@ -100,7 +100,7 @@ __device__ __forceinline__ void cross_small_core(const ScoreArgs& a, int jb, int
     sa[d * LD + r] = WITH_LINF ? v : v * a.kp.inv_ls_c[d];
   }
   {
-    const double* src = (WITH_LINF ? a.XT + (size_t)dc * np : a.XT) + jb * 64;
+    const double* src = (WITH_LINF ? a.XT + xt_plane(1, dc, np) : a.XT) + jb * 64;
     for (int e = tid; e < dc * 32; e += kSmallThreads) {
       const int d = e >> 5, q = e & 31;
       *reinterpret_cast<double2*>(sb + d * LD + 2 * q) = __ldg(reinterpret_cast<const double2*>(src + (size_t)d * np + 2 * q));
